@@ -2,6 +2,7 @@
 """bench.py — frames/sec of InpaintGenerator.forward on synthetic 432x240 5+3 clips (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--clips-per-gpu B] [--workload W]
+                    [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...        (N > 1, one rank per GPU, NCCL)
 
 Headline: a step = one forward over B clips per GPU (default 8 = BASELINE configs[3]'s per-GPU share: 64 clips over
@@ -35,7 +36,7 @@ WORKLOADS = {
     "hq720": ("model.e2fgvi_hq", 720, 1296, 8, 5, 1, 2),     # configs[2]: 720x1280, 5+3
     "hq1080": ("model.e2fgvi_hq", 1080, 1944, 16, 10, 1, 4),  # configs[4]: 1080x1920, 10+6, one clip per GPU
 }
-L2_BYTES = 126e6
+L2_BYTES = 50e6                                              # H100 SXM L2
 
 
 def log(msg):
@@ -59,12 +60,12 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 6650.0, 1590.0, 1400.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops", 989.0), d.get("bf16_tflops_sustained", 989.0), "measured"
+    return 3350.0, 989.0, 989.0, "fallback"                          # H100 SXM data sheet (dense bf16)
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md).
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region.
 
     The process is started BEFORE the warm-up steps: nvidia-smi needs 0.1-0.5 s to attach to the driver and, while it
     does, kernel launches of this process stall behind it — started right in front of the timed region (as this file
@@ -138,7 +139,7 @@ def workload_config(name, B, world, precision="strict"):
                         + f", {l_t} local + {T - l_t} ref frames, {B} clip(s) per GPU per step (BASELINE configs[{idx}]"
                         + (" per-GPU share)" if name == "base" else ")"),
             "global_batch_clips": B * world, "frames_per_clip": T, "parallelism": f"clip-dp{world}",
-            "l2": f"inputs rotate over {n_input_sets(set_mb * 1e6)} sets x {set_mb:.0f} MB (> 126 MB L2)",
+            "l2": f"inputs rotate over {n_input_sets(set_mb * 1e6)} sets x {set_mb:.0f} MB (> 50 MB L2)",
             "precision": precision,
             "weights": "random-init, reference default family (e2fgvi_b200.synth 'default', seed 0)"}
 
@@ -328,7 +329,8 @@ class Measurement:
                     landed[len(landed) - 3].synchronize()
             else:
                 x = inputs[i % self.n_sets]
-            pred, _ = self.model(x, self.l_t)
+            pred, flows = self.model(x, self.l_t)
+            self.last_out = (pred, flows)
             if to_host:
                 consumed[i % 2] = torch.cuda.Event()
                 consumed[i % 2].record(main)
@@ -367,6 +369,7 @@ class Measurement:
             self._loop(self.steps, self.dev_sets)
             e1.record()
             self.sync()
+            res["outputs"] = self.last_out                  # what the last timed step returned
             res["launches"] = ops.launch_count() - n0
             res["clocks"] = sampler.stop() if sampler else None
             ms = e0.elapsed_time(e1)
@@ -439,13 +442,36 @@ class Measurement:
 
 
 def traffic_for(name):
-    """DRAM bytes per launch from the committed `ncu` step capture of THIS workload (profiles/ncu_traffic.json,
+    """DRAM bytes per launch from an `ncu` step capture of THIS workload (profiles/ncu_traffic.json, when present,
     keyed by workload); None for workloads without a capture (never the bytes of another shape)."""
     tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")
     if not os.path.exists(tpath):
         return None
     d = json.load(open(tpath))
     return d.get(name) if isinstance(d.get(name), dict) else None
+
+
+def dump_outputs(out_dir, pred, flows, budget=64 << 20):
+    """Write what the timed forward returned in its last step as float32 .npy files under out_dir: every flow tensor in
+    full, the predicted frames in full when they fit the byte budget, else as pred_sample.npy, the elements
+    pred.flatten()[offset::stride] with a seeded offset (the same elements in every run with the same arguments)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {}
+    for i, f in enumerate(flows if isinstance(flows, (list, tuple)) else [flows]):
+        if f is not None:
+            arrays[f"flows_{i}"] = f.detach().float().cpu().numpy()
+    room = (budget - sum(a.nbytes for a in arrays.values())) // 4
+    flat = pred.detach().float().flatten()
+    if flat.numel() <= room:
+        arrays["pred"] = pred.detach().float().cpu().numpy()
+    else:
+        stride = -(-flat.numel() // room)
+        offset = int(torch.randint(stride, (1,), generator=torch.Generator().manual_seed(0)))
+        arrays["pred_sample"] = flat[offset::stride].cpu().numpy()
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), a)
+    log(f"outputs of the last timed step -> {out_dir}: " + ", ".join(f"{k} {tuple(a.shape)}" for k, a in arrays.items()))
 
 
 def graph_latency(model, one, l_t, reps=10):
@@ -499,6 +525,8 @@ def main():
                     help="skip the b1 / hq720 / hq1080 / video-driver sections of the default run")
     ap.add_argument("--precision", default="strict", choices=["strict", "tf32"],
                     help="library op precision (only matters for the few remaining torch glue ops)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as .npy files (float32, at most 64 MB) to DIR")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 0)
 
@@ -530,6 +558,9 @@ def main():
                    "peer-memory DMA pushes + stream-memop flags (clips.PeerStitcher)" if type(head.stitch).__name__ == "PeerStitcher"
                    else "all_gather_into_tensor (clips.ClipStitcher)")
     main_res = head.run(sample_clocks=True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *main_res["outputs"])
+    main_res.pop("outputs")
     kernels = kernel_rooflines(main_res["prof"], main_res["ms_prof"], traffic_for(name)) if rank == 0 else {}
     one_clip = head.dev_sets[0][:1].clone()
     head.free()

@@ -1,4 +1,4 @@
-"""e2fgvi_b200 — B200-native (sm_100a) implementation of E2FGVI's InpaintGenerator.forward hot path.
+"""e2fgvi_b200 — H100-native (sm_90a) implementation of E2FGVI's InpaintGenerator.forward hot path.
 
 Package map (only what the path needs):
   csrc/      hand-written CUDA kernels + the C ABI (include/e2fgvi_b200.h)

@@ -1,7 +1,7 @@
-"""In-tree build of the sm_100a C-ABI library (nvcc cross-compiles without a GPU).
+"""In-tree build of the sm_90a C-ABI library (nvcc cross-compiles without a GPU).
 
 ``python -m e2fgvi_b200.build`` or ``__graft_entry__.build()``.  Output: ``e2fgvi_b200/libe2fgvi_b200.so``
-(git-ignored, shipped to the GPU box with the tree).  No torch headers are involved: the boundary is plain C.
+(git-ignored).  No torch headers are involved: the boundary is plain C.
 """
 import hashlib
 import os
@@ -15,7 +15,7 @@ STAMP = LIB_PATH + ".stamp"
 
 SOURCES = ["api.cu", "flow_warp.cu", "dcn.cu", "focal_attn.cu", "t2t.cu", "gemm.cu", "conv.cu", "elementwise.cu", "video.cu", "spynet.cu", "conv_kxn.cu", "peer.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "-Xptxas", "-v",
@@ -66,7 +66,7 @@ def build(force=False, verbose=False):
             sys.stderr.write("\n".join(log))
             raise RuntimeError(f"nvcc failed on {src}")
         objs.append(obj)
-    cmd = [_nvcc(), "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart_static",
+    cmd = [_nvcc(), "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart_static",
                                                           "-ldl", "-lrt", "-lpthread"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     log.append(r.stdout)

@@ -1,4 +1,4 @@
-"""Clip-level data parallelism (SURVEY §8(e)): clips are independent units, so they shard across ranks with no
+"""Clip-level data parallelism: clips are independent units, so they shard across ranks with no
 data-path collective; the ONLY collective is one all-gather of the output frames for the stitch.
 
 One process per GPU (torchrun); ``nccl`` on GPUs, ``gloo`` in the CPU tests.
@@ -13,9 +13,8 @@ Round 2 (VERDICT r01 "Multi-GPU"):
 * on one NVLink / NVSwitch box the payload does not go through NCCL at all (``PeerStitcher``): every rank pushes its
   block of frames into the peers' landing buffers (CUDA IPC peer memory) with copy-engine DMA on a side stream and
   orders the pushes with flag words driven by stream memory operations — no kernel, no SM, so the persistent
-  one-CTA-per-SM kernels of the next forward keep the whole chip while the exchange runs.  Measured on 4 x B200
-  (profiles/r02/run22_*): the exchange costs ~0 ms per 35 ms step with either implementation (weak-scaling loss is the
-  slowest board under the power cap); the peer path is the default because it cannot compete for SMs as payloads grow.
+  one-CTA-per-SM kernels of the next forward keep the whole chip while the exchange runs.  The peer path is the
+  default because it cannot compete for SMs as payloads grow.
 """
 import os
 

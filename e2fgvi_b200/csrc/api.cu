@@ -21,7 +21,7 @@ int num_sms() {
   const int dev = current_device();
   int v = (dev >= 0 && dev < 64) ? cache[dev].load(std::memory_order_relaxed) : 0;
   if (!v) {
-    v = 148;
+    v = 132;
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
     if (dev >= 0 && dev < 64) cache[dev].store(v, std::memory_order_relaxed);
   }
@@ -48,7 +48,7 @@ using namespace e2f;
 
 extern "C" {
 
-const char* e2f_version(void) { return "e2fgvi_b200 0.1.0 sm_100a"; }
+const char* e2f_version(void) { return "e2fgvi_b200 0.1.0 sm_90a"; }
 
 const char* e2f_last_error(void) { return g_err; }
 

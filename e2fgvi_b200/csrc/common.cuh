@@ -1,8 +1,7 @@
-// Blackwell (sm_100a) device primitives used by every kernel in this library:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / st),
-// UMMA shared-memory + instruction descriptors, cp.async, and small math helpers.
-// Everything is inline PTX; no CUTLASS dependency.  Bit layouts of the descriptors
-// follow the PTX ISA "tcgen05 matrix descriptor" / "instruction descriptor" tables.
+// Hopper (sm_90a) device primitives used by every kernel in this library:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA with shared-memory descriptors, fp32 accumulators in
+// registers), cp.async, and small math helpers.  Everything is inline PTX; no CUTLASS dependency.  Bit layouts of
+// the descriptors follow the PTX ISA "wgmma matrix descriptor" table.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -43,7 +42,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       ".reg .pred p;\n"
       // suspend-time hint (ns): the waiting thread SLEEPS in hardware until the phase completes instead of
       // returning immediately — without it every waiting warp busy-polls and starves the working warps of
-      // issue slots (measured: 10x slowdown per instruction in the attention kernel, profiles/r01)
+      // issue slots
       "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n"
       "selp.b32 %0, 1, 0, p;\n"
       "}\n"
@@ -67,15 +66,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // ----------------------------------------------------------------------------- proxies / fences
-// generic-proxy smem writes -> visible to the async proxy (TMA / tcgen05.mma operand reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 
 // ----------------------------------------------------------------------------- cp.async (LDGSTS)
@@ -104,139 +97,130 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const void* tmap,
       : "memory");
 }
 
-// multicast variant: the box lands at the same CTA-relative offset of every CTA in cta_mask and signals the mbarrier at
-// the same offset in each of them
-__device__ __forceinline__ void tma_load_2d_mc(uint32_t smem_dst, const void* tmap, uint64_t* bar, int c0, int c1,
-                                               uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_dst),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
-      : "memory");
-}
-
-// ----------------------------------------------------------------------------- thread-block clusters
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-// all threads of all CTAs of the cluster
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// ----------------------------------------------------------------------------- TMEM
-// whole warp; writes the TMEM base address to *dst_smem.  ncols: power of two in [32,512]
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// ----------------------------------------------------------------------------- UMMA descriptors
+// ----------------------------------------------------------------------------- wgmma
 // Shared-memory matrix descriptor, 128-byte swizzle, 16-bit elements.
 //   bits [0,14)  start address >> 4        bits [16,30) leading-dim byte offset >> 4
-//   bits [32,46) stride-dim byte offset >> 4   bits [46,48) version = 1 (sm_100)
-//   bits [61,64) layout type: 2 = SWIZZLE_128B
+//   bits [32,46) stride-dim byte offset >> 4   bits [62,64) layout type: 1 = SWIZZLE_128B
 // K-major tile  [rows][64 halfs]: rows are 128 B, 8-row groups are 1024 B apart (SBO); LBO unused (=1).
 // MN-major tile [k][64 halfs]   : k-rows are 128 B, 8-k groups are SBO apart, the next 64 MN elements are LBO apart.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// The swizzle is a function of the absolute shared-memory address, so a start address moved by whole 128-byte rows
+// (or by 32 bytes along K inside a row) addresses the same swizzled data: descriptors advance by one 64-bit add.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// Descriptors of the same tile family differ only in the start-address field (bits [0,14), 16-byte units): advancing
-// by `bytes` is ONE 64-bit add.  Building descriptors from scratch per MMA costs ~40 dependent integer instructions in
-// the single issuing thread (~100 cycles per MMA measured) and caps the tensor pipe at ~60 %.
-__device__ __forceinline__ uint64_t umma_desc_adv(uint64_t desc, uint32_t bytes) { return desc + (bytes >> 4); }
+__device__ __forceinline__ uint64_t gmma_desc_adv(uint64_t desc, uint32_t bytes) { return desc + (bytes >> 4); }
 
-// Instruction descriptor for kind::f16 with fp16 A/B and fp32 accumulation.
-//   [4,6) c_format=1 (F32)  [7,10) a_format=0 (F16)  [10,13) b_format=0 (F16)
-//   [15] a_major (0=K,1=MN) [16] b_major  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (static_cast<uint32_t>(a_mn_major) << 15) | (static_cast<uint32_t>(b_mn_major) << 16) |
-         (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
+// D[64 x n] (+)= A[64 x 16] . B[n x 16]^T, A and B K-major in shared memory, issued by a whole warpgroup.  Accumulator
+// fragment of thread t (warp w = (t / 32) % 4, lane l): d[4j + {0,1}] = row 16w + l/4, columns 8j + 2(l%4) + {0,1};
+// d[4j + {2,3}] = the same columns of row 16w + l/4 + 8.  acc = 0 overwrites D.
+__device__ __forceinline__ void wgmma_n16_bf16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
   asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(acc));
 }
-// All previously issued tcgen05.mma of this thread arrive on `bar` when complete
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+__device__ __forceinline__ void wgmma_n16_f16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_n32_bf16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_n32_f16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_n64_bf16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_n64_f16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_n64_f16_rs_tb(float* d, const uint32_t (&a)[4], uint64_t bdesc, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(acc));
 }
 
-// ... arriving on the barrier at this offset in every CTA of cta_mask (stage release towards multicasting producers)
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
+// n = N (multiple of 16) as blocks of 64 / 32 / 16 columns; the B rows of the next block start n*128 bytes further
+template <int N, bool F16>
+__device__ __forceinline__ void wgmma_ss(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  static_assert(N % 16 == 0 && N > 0, "wgmma N");
+  if constexpr (N >= 64) {
+    if constexpr (F16) wgmma_n64_f16(d, adesc, bdesc, acc);
+    else wgmma_n64_bf16(d, adesc, bdesc, acc);
+    if constexpr (N > 64) wgmma_ss<N - 64, F16>(d + 32, adesc, gmma_desc_adv(bdesc, 64 * 128), acc);
+  } else if constexpr (N >= 32) {
+    if constexpr (F16) wgmma_n32_f16(d, adesc, bdesc, acc);
+    else wgmma_n32_bf16(d, adesc, bdesc, acc);
+    if constexpr (N > 32) wgmma_ss<N - 32, F16>(d + 16, adesc, gmma_desc_adv(bdesc, 32 * 128), acc);
+  } else {
+    if constexpr (F16) wgmma_n16_f16(d, adesc, bdesc, acc);
+    else wgmma_n16_bf16(d, adesc, bdesc, acc);
+  }
 }
 
-// ----------------------------------------------------------------------------- TMEM <-> registers
-// 32 lanes x 32 consecutive 32-bit columns: thread i of the warp gets row (lane base + i).
-// The warp may only touch TMEM lanes [32*(warp_id%4), +32).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
+// Accumulator staging: a warpgroup's fragments written to a [rows][N] fp32 shared-memory tile so that a thread can
+// read a whole row (the row-per-thread epilogues).  16-byte chunk c of row r sits at chunk c ^ (r & 7): row-parallel
+// 16-byte reads by 8 consecutive rows hit 8 different bank groups.
+__device__ __forceinline__ uint32_t acc_stage_offset(uint32_t row, uint32_t col, uint32_t n) {
+  return row * n * 4u + ((((col >> 2) ^ (row & 7u))) << 4) + (col & 3u) * 4u;
 }
-// 32 lanes x 8 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr)
-               : "memory");
+template <int N>
+__device__ __forceinline__ void acc_stage_store(uint32_t stage_smem, const float* d, int row0, int lane) {
+  // row0: first row of the calling warp's 16-row slice
+  const int r = row0 + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(stage_smem + acc_stage_offset(r, 8 * j + c, N)),
+                 "f"(d[4 * j]), "f"(d[4 * j + 1]) : "memory");
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(stage_smem + acc_stage_offset(r + 8, 8 * j + c, N)),
+                 "f"(d[4 * j + 2]), "f"(d[4 * j + 3]) : "memory");
+  }
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%32], "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31};" ::"r"(v[0]),
-      "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-      "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-      "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31]), "r"(taddr)
-      : "memory");
+// 32 consecutive columns [col0, col0 + 32) of row r (col0 % 32 == 0)
+__device__ __forceinline__ void acc_stage_load32(uint32_t stage_smem, uint32_t r, uint32_t col0, uint32_t n,
+                                                 uint32_t (&v)[32]) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(v[4 * i]), "=r"(v[4 * i + 1]), "=r"(v[4 * i + 2]), "=r"(v[4 * i + 3])
+                 : "r"(stage_smem + acc_stage_offset(r, col0 + 4 * i, n))
+                 : "memory");
 }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%16], "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15};" ::"r"(v[0]),
-      "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------- misc
 __device__ __forceinline__ bool elect_one() {
@@ -260,7 +244,7 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 // Byte offset of 16-byte chunk `chunk` (0..7) of row `row` inside a 128B-swizzled tile whose rows are 128 B
-// and whose base is 1024-byte aligned (the layout TMA SWIZZLE_128B writes and UMMA SWIZZLE_128B reads).
+// and whose base is 1024-byte aligned (the layout TMA SWIZZLE_128B writes and wgmma SWIZZLE_128B reads).
 __device__ __forceinline__ uint32_t sw128_offset(uint32_t row, uint32_t chunk) {
   return row * 128u + ((chunk ^ (row & 7u)) << 4);
 }

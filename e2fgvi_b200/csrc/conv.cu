@@ -1,5 +1,5 @@
 // 3x3 / stride 1 / pad 1 convolutions of the path (encoder e2fgvi.py:75-109, decoder :143-150, offset heads
-// feat_prop.py:20-28, backbones :73-77) as an implicit GEMM on tcgen05 with fp32-level accuracy (bf16 3-term split,
+// feat_prop.py:20-28, backbones :73-77) as an implicit GEMM on wgmma with fp32-level accuracy (bf16 3-term split,
 // see gemm.cu):   out[n,y,x,co] = act( sum_{tap,src,c} X_src[n, y+r-1, x+s-1, c] * W[co, tap, src, c] + b[co] ) (+ res)
 //
 //  * im2col is done by TMA: activations are NHWC bf16 (hi, lo); one 4-D box {64 ch, 16 x, 8 y, 1 n} per (tap, source,
@@ -18,7 +18,8 @@
 //    kernel width are zero; what those positions read is finite data of the same buffer.
 //  * epilogue: + bias, LeakyReLU(slope), optional residual add, fp32 NHWC store and/or the bf16 (hi, lo) split of
 //    the result — dense NHWC or row-gapped for a following window-packed conv (the zero gaps are written here).
-// Pipeline = gemm.cu: persistent CTAs, TMA warp / MMA warp / 4 epilogue warps, double-buffered TMEM accumulator.
+// Pipeline = gemm.cu: persistent CTAs, TMA warp + two consumer warpgroups (64 accumulator rows each, fp32 in registers);
+// a finished accumulator is staged through shared memory so that the epilogue can work row-per-thread.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cstdlib>
@@ -31,10 +32,10 @@ namespace conv {
 constexpr int BM = 128, BK = 64;
 constexpr int TILE_H = 8, TILE_W = 16;                  // 8 x 16 output pixels = 128 GEMM rows
 constexpr int A_TILE = BM * BK * 2;
-constexpr int EPI_WARPS = 8;                             // two warps per TMEM lane quarter, half of the tile's columns each
+constexpr int EPI_WARPS = 8;                             // two consumer warpgroups; in the epilogue two warps per 32 rows, half of the columns each
 constexpr int MAX_COUT = 512;                            // bias staged in shared memory once per CTA
 constexpr int EPI_STAGE = 2048;                          // per epilogue warp: 32 rows x 64 bytes store-transposition buffer
-constexpr int THREADS = (2 + EPI_WARPS) * 32;
+constexpr int THREADS = (EPI_WARPS + 1) * 32;                // + the TMA warp
 constexpr int MAX_SRC = 4;
 
 // N tile: 128 output channels; 64 / 32 for the layers with <= 64 / <= 32 output channels per group (decoder, encoder
@@ -44,11 +45,10 @@ template <int BN>
 struct Cfg {
   static constexpr int W_TILE = BN * BK * 2;
   static constexpr int STAGE = 2 * A_TILE + 2 * W_TILE;   // 64 KB (BN=128) / 48 KB (BN=64) / 40 KB (BN=32)
-  static constexpr int STAGES = (BN >= 96) ? 3 : 4;
-  static constexpr int ACC_COLS = 2 * BN;                 // accumulator: [Ah.Wh + Al.Wh | Ah.Wl], summed by the epilogue
-  // double-buffered; tcgen05.alloc wants a power of two (BN = 96: 384 columns used of 512)
-  static constexpr int TMEM_COLS = (4 * BN <= 128) ? 128 : (4 * BN <= 256) ? 256 : 512;
-  static constexpr int SMEM = STAGES * STAGE + 256 + MAX_COUT * 4 + EPI_WARPS * EPI_STAGE + 1024;
+  static constexpr int ACC_STAGE = BM * BN * 4;           // fp32 accumulator tile staged for the epilogue
+  // as many stages as fit next to the accumulator staging in the 227 KB a CTA may use
+  static constexpr int STAGES = (BN >= 96) ? 2 : (BN == 64) ? 3 : 4;
+  static constexpr int SMEM = STAGES * STAGE + 256 + MAX_COUT * 4 + EPI_WARPS * EPI_STAGE + ACC_STAGE + 1024;
 };
 
 struct Maps {
@@ -89,11 +89,6 @@ struct Params {
 
 constexpr int EPI_TANH = 1, EPI_NCHW = 2;     // both only on the element-wise store path (Cout % 4 != 0: the 3-channel output conv)
 
-__host__ __device__ constexpr uint32_t idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
-}
-
 __device__ __forceinline__ void tma_load_4d(uint32_t smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2,
                                             int c3) {
   asm volatile(
@@ -128,13 +123,11 @@ __device__ __forceinline__ TileCoord decode_tile(int tile, const Params& p, int 
   return t;
 }
 
-// Epilogue of one 128-pixel x BN-channel tile for the calling thread's accumulator row `r` (TMEM lane): sums the two
-// accumulator halves, + bias, LeakyReLU, optional residual, fp32 and/or bf16-split NHWC stores.  TW = tile width in
-// pixels (row r is pixel (y0 + r / TW, x0 + r % TW)); taddr = TMEM address of the row's first accumulator column.
+// Epilogue of one 128-pixel x BN-channel tile for the calling thread's accumulator row `r`: + bias, LeakyReLU, optional
+// residual, fp32 and/or bf16-split NHWC stores.  TW = tile width in pixels (row r is pixel (y0 + r / TW, x0 + r % TW));
+// acc_smem = the accumulator tile staged in shared memory (acc_stage_store layout).
 // The calling warp handles the 32-column chunks [c_begin, c_end) of the tile.  bias_s = the layer's bias in SHARED
-// memory (zeros when the layer has none): the per-channel __ldg's this replaces queued behind the epilogue's own
-// 32-line-per-instruction stores and made up 59 % of the epilogue warps' stall samples, which bounded every layer
-// whose main loop is shorter than ~10k cycles per tile (profiles/r01/ncu_conv_epilogue_r01.txt).
+// memory (zeros when the layer has none): per-channel __ldg's would queue behind the epilogue's own stores.
 //
 // Stores are STAGED through `stage` (2 KB of shared memory per epilogue warp): with thread = pixel, a direct 16-byte store
 // per thread hits 32 different 128-byte lines per instruction (pixels are Cout * 2 or 4 bytes apart), ~125 cycles each,
@@ -142,7 +135,7 @@ __device__ __forceinline__ TileCoord decode_tile(int tile, const Params& p, int 
 // 32 rows x 64 bytes through a conflict-free XOR-swizzled buffer so that 4 consecutive lanes write one pixel's 64
 // contiguous bytes (8 lines per instruction).  Chunks that are not 32 full, 16-byte-aligned channels take the direct path.
 template <int BN>
-__device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& t, uint32_t taddr, int r, int cog,
+__device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& t, uint32_t acc_smem, int r, int cog,
                                               const float* __restrict__ bias_s, int c_begin, int c_end,
                                               uint8_t* __restrict__ stage, const int TW, const int TH) {
   const int lane = r & 31;
@@ -162,12 +155,8 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
   const bool vec_ok = (p.Cout & 3) == 0;            // 16-byte aligned channel groups
 #pragma unroll 1
   for (int c = c_begin; c < c_end; ++c) {
-    uint32_t v[32], v2[32];
-    tmem_ld32(taddr + c * 32, v);
-    tmem_ld32(taddr + BN + c * 32, v2);              // the Ah.Wl half of the accumulator
-    tmem_ld_wait();
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) + __uint_as_float(v2[i]));
+    uint32_t v[32];
+    acc_stage_load32(acc_smem, r, c * 32, BN, v);
     const int co = t.co0 + c * 32;
     if (vec_ok && co + 32 <= co_end) {
       // ------------------------------------------------------------ staged, coalesced stores (warp-uniform branch)
@@ -353,34 +342,26 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
 
 template <int BN>
 __global__ void __launch_bounds__(THREADS, 1) conv3x3_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p) {
-  constexpr int W_TILE = Cfg<BN>::W_TILE, STAGE = Cfg<BN>::STAGE, STAGES = Cfg<BN>::STAGES, TMEM_COLS = Cfg<BN>::TMEM_COLS;
+  constexpr int W_TILE = Cfg<BN>::W_TILE, STAGE = Cfg<BN>::STAGE, STAGES = Cfg<BN>::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE);
   uint64_t* empty = full + STAGES;
-  uint64_t* acc_full = empty + STAGES;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
   float* bias_s = reinterpret_cast<float*>(smem + STAGES * STAGE + 256);
   uint8_t* epi_stage = smem + STAGES * STAGE + 256 + MAX_COUT * 4;
+  const uint32_t acc_smem = smem_u32(epi_stage + EPI_WARPS * EPI_STAGE);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int epi_warps = (blockDim.x >> 5) - 2;                // 8, or 4 when the launch has no room for 8 staging buffers
   for (int i = tid; i < MAX_COUT; i += blockDim.x) bias_s[i] = (p.bias && i < p.Cout) ? __ldg(p.bias + i) : 0.f;
   const int tiles_y = (p.H + p.tile_h - 1) / p.tile_h, tiles_x = (p.W + p.tile_w - 1) / p.tile_w;
   const int cog = p.Cout / p.groups;
   const int tiles_ng = (cog + BN - 1) / BN;
   const int num_tiles = p.N * tiles_y * tiles_x * p.nphase * p.groups * tiles_ng;
 
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&acc_full[s], 1);
-      mbar_init(&acc_empty[s], epi_warps);
+      mbar_init(&empty[s], EPI_WARPS);
     }
     fence_barrier_init();
     tma_prefetch_desc(&maps.w_hi);
@@ -390,14 +371,11 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_kernel(const __grid_consta
       tma_prefetch_desc(&maps.a_lo[i]);
     }
   }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tbase = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == EPI_WARPS) {
     // ------------------------------------------------------------------ TMA producer (im2col by coordinates)
-    if (elect_one()) {   // one thread, chosen by elect.sync: ptxas then emits bare UTCHMMA / UTMALDG (no per-instruction ELECT loop)
+    if (elect_one()) {
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const TileCoord t = decode_tile<BN>(tile, p, tiles_y, tiles_x, tiles_ng);
@@ -443,67 +421,54 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_kernel(const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (elect_one()) {   // one thread, chosen by elect.sync: ptxas then emits bare UTCHMMA / UTMALDG (no per-instruction ELECT loop)
-      // The Wh and Wl tiles are adjacent in a stage, so ONE N = 2*BN instruction multiplies Ah with both
-      // (accumulator columns [0,BN) and [BN,2BN)); a second, N = BN wide, adds Al.Wh to the first half.  Ah is read from
-      // shared memory once instead of twice: 3 -> 2 instructions per K step, ~20% less operand traffic on the
-      // shared-memory port that the TMA writes share.
-      const uint32_t idesc = idesc_bf16(BM, BN), idesc2 = idesc_bf16(BM, 2 * BN);
-      const uint64_t d_ah0 = umma_desc_sw128(smem_u32(smem), 16, 1024);
-      const uint64_t d_al0 = umma_desc_adv(d_ah0, A_TILE), d_wh0 = umma_desc_adv(d_ah0, 2 * A_TILE);
-      uint32_t it = 0, local = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-        const int buf = local & 1;
-        int num_kb = p.ks * p.rows_g;                     // window-packed K
-        if (!p.rows_px) {
-          const int ph = (tile / (tiles_ng * p.groups)) % p.nphase;
-          num_kb = (p.ph_tap0[ph + 1] - p.ph_tap0[ph]) * p.chunks_total;
-        }
-        mbar_wait(&acc_empty[buf], ((local >> 1) & 1) ^ 1);
-        tc_fence_after_sync();
-        const uint32_t d = tbase + buf * Cfg<BN>::ACC_COLS;
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int stage = it % STAGES;
-          mbar_wait(&full[stage], (it / STAGES) & 1);
-          tc_fence_after_sync();
-          const uint32_t soff = (stage * STAGE) >> 4;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t dah = d_ah0 + soff + 2 * k, dal = d_al0 + soff + 2 * k;
-            const uint64_t dwh = d_wh0 + soff + 2 * k;
-            umma_f16(d, dah, dwh, idesc2, (kb | k) != 0);   // [Ah.Wh | Ah.Wl]
-            umma_f16(d, dal, dwh, idesc, 1);                // + Al.Wh
-          }
-          umma_commit(&empty[stage]);
-        }
-        umma_commit(&acc_full[buf]);
-      }
-    }
   } else {
-    // ------------------------------------------------------------------ epilogue
-    const int q = warp & 3;                                   // TMEM lane quarter this warp may read
-    constexpr int NCH = BN / 32;                              // 32-column chunks per tile, split between the two warps of a quarter
-    const int c_split = epi_warps > 4 ? (NCH + 1) / 2 : NCH;
-    const int c_begin = (warp - 2) < 4 ? 0 : c_split, c_end = (warp - 2) < 4 ? c_split : NCH;
-    uint8_t* my_stage = epi_stage + (warp - 2) * EPI_STAGE;
-    uint32_t local = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-      const int buf = local & 1;
+    // ------------------------------------------------------------------ consumers: wgmma main loop, then the epilogue
+    // warpgroup wg owns accumulator rows [64 wg, 64 wg + 64); this warpgroup's A rows start 64 * 128 B into the A tiles
+    const int wg = warp >> 2, wq = warp & 3;
+    const uint64_t d_ah0 = gmma_desc_sw128(smem_u32(smem) + wg * 64 * 128, 16, 1024);
+    const uint64_t d_al0 = gmma_desc_adv(d_ah0, A_TILE);
+    const uint64_t d_wh0 = gmma_desc_sw128(smem_u32(smem) + 2 * A_TILE, 16, 1024);
+    const uint64_t d_wl0 = gmma_desc_adv(d_wh0, W_TILE);
+    // epilogue: warp wq reads rows 64 wg + 32 (wq & 1) + lane, the first or second half of the 32-column chunks
+    constexpr int NCH = BN / 32;
+    const int c_split = (NCH + 1) / 2;
+    const int c_begin = (wq >> 1) ? c_split : 0, c_end = (wq >> 1) ? NCH : c_split;
+    uint8_t* my_stage = epi_stage + warp * EPI_STAGE;
+    float acc[BN / 2];
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      int num_kb = p.ks * p.rows_g;                     // window-packed K
+      if (!p.rows_px) {
+        const int ph = (tile / (tiles_ng * p.groups)) % p.nphase;
+        num_kb = (p.ph_tap0[ph + 1] - p.ph_tap0[ph]) * p.chunks_total;
+      }
+      for (int kb = 0; kb < num_kb; ++kb, ++it) {
+        const int stage = it % STAGES;
+        mbar_wait(&full[stage], (it / STAGES) & 1);
+        const uint32_t soff = (stage * STAGE) >> 4;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint64_t dah = d_ah0 + soff + 2 * k, dal = d_al0 + soff + 2 * k;
+          const uint64_t dwh = d_wh0 + soff + 2 * k, dwl = d_wl0 + soff + 2 * k;
+          wgmma_ss<BN, false>(acc, dal, dwh, (kb | k) != 0);   // small terms first
+          wgmma_ss<BN, false>(acc, dah, dwl, 1);
+          wgmma_ss<BN, false>(acc, dah, dwh, 1);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                                  // the previous K block's MMAs are done: release its stage
+        if (kb > 0 && lane == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
+      }
+      wgmma_wait<0>();
+      if (num_kb > 0 && lane == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
+      acc_stage_store<BN>(acc_smem, acc, wg * 64 + wq * 16, lane);
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // this warpgroup's 64 rows staged
       const TileCoord t = decode_tile<BN>(tile, p, tiles_y, tiles_x, tiles_ng);
-      mbar_wait(&acc_full[buf], (local >> 1) & 1);
-      tc_fence_after_sync();
-      epilogue_tile<BN>(p, t, tbase + (static_cast<uint32_t>(q * 32) << 16) + buf * Cfg<BN>::ACC_COLS, q * 32 + lane, cog,
-                        bias_s, c_begin, c_end, my_stage, p.tile_w, p.tile_h);
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
+      epilogue_tile<BN>(p, t, acc_smem, wg * 64 + 32 * (wq & 1) + lane, cog, bias_s, c_begin, c_end, my_stage, p.tile_w,
+                        p.tile_h);
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // staging read before the next tile overwrites it
     }
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tbase, TMEM_COLS);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -512,14 +477,13 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_kernel(const __grid_consta
 // chip-wide): every 64-channel chunk of a tile is fetched nine times, once per tap, and the matching weight tile comes
 // along every time — 432 KB per 128 x 64 output tile against 3456 MMA cycles.  Here
 //  * the tile is 8 x 16 pixels and ONE TMA box {64 ch, 10 x, 18 y} per (chunk, hi | lo) brings its whole halo
-//    (23 KB instead of 9 x 16 KB); tap (dy, dx) reads it in place through a UMMA descriptor whose start address is shifted
+//    (23 KB instead of 9 x 16 KB); tap (dy, dx) reads it in place through a wgmma descriptor whose start address is shifted
 //    by (dy*10 + dx) pixels of 128 B and whose 8-row-group stride (SBO) is one halo row, 1280 B.  The 128B swizzle is a
-//    function of absolute shared-memory address bits, so the shifted start needs no base offset (tools/halo_probe.cu,
-//    profiles/r01/halo_probe.log);
+//    function of absolute shared-memory address bits, so the shifted start needs no base offset;
 //  * all weight tiles of the layer (9 taps x chunks x [Wh | Wl]) are loaded ONCE per persistent CTA and stay in shared
-//    memory (144 KB for 64 -> 64), so steady-state L2 traffic is the 46 KB halo pair per chunk;
-//  * the halo ring holds single (hi or lo) pieces: all Ah MMAs of a chunk (9 taps x 4, N = 2*BN against [Wh | Wl]) are
-//    issued from one piece, then all Al MMAs (N = BN against Wh) from the next.
+//    memory, so steady-state L2 traffic is the 46 KB halo pair per chunk;
+//  * the halo ring holds single (hi or lo) pieces: all Ah MMAs of a chunk (9 taps x 4, against Wh and Wl) are issued
+//    from one piece, then all Al MMAs (against Wh) from the next.
 constexpr int HTILE_W = 8, HTILE_H = 16, HALO_W = HTILE_W + 2, HALO_H = HTILE_H + 2;
 constexpr int HALO_BYTES = HALO_W * HALO_H * BK * 2;     // 23040
 constexpr int HALO_SLOT = 23552;                        // rounded up to the 1024-byte swizzle atom
@@ -531,36 +495,28 @@ __host__ __device__ constexpr int halo_w_bytes(int bn, int chunks_total) { retur
 template <int BN>
 __global__ void __launch_bounds__(THREADS, 1) conv3x3_halo_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p,
                                                                   const int nslots) {
-  constexpr int W_TILE = Cfg<BN>::W_TILE, TMEM_COLS = Cfg<BN>::TMEM_COLS;
+  constexpr int W_TILE = Cfg<BN>::W_TILE;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int w_bytes = halo_w_bytes(BN, p.chunks_total);
   uint8_t* ring = smem + w_bytes;                                   // w_bytes is a multiple of 1024
   uint64_t* a_full = reinterpret_cast<uint64_t*>(ring + nslots * HALO_SLOT);
   uint64_t* a_empty = a_full + HALO_MAX_SLOTS;
-  uint64_t* acc_full = a_empty + HALO_MAX_SLOTS;
-  uint64_t* acc_empty = acc_full + 2;
-  uint64_t* w_full = acc_empty + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(w_full + 1);
+  uint64_t* w_full = a_empty + HALO_MAX_SLOTS;
   float* bias_s = reinterpret_cast<float*>(ring + nslots * HALO_SLOT + 256);
   uint8_t* epi_stage = ring + nslots * HALO_SLOT + 256 + MAX_COUT * 4;
+  const uint32_t acc_smem = smem_u32(epi_stage + EPI_WARPS * EPI_STAGE);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int epi_warps = (blockDim.x >> 5) - 2;                // 8, or 4 when the launch has no room for 8 staging buffers
   for (int i = tid; i < MAX_COUT; i += blockDim.x) bias_s[i] = (p.bias && i < p.Cout) ? __ldg(p.bias + i) : 0.f;
   const int tiles_y = (p.H + HTILE_H - 1) / HTILE_H, tiles_x = (p.W + HTILE_W - 1) / HTILE_W;
   const int num_tiles = p.N * tiles_y * tiles_x;
   const int pieces = 2 * p.chunks_total;                            // (chunk, hi | lo) halo pieces per tile
 
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
   if (tid == 0) {
     for (int s = 0; s < nslots; ++s) {
       mbar_init(&a_full[s], 1);
-      mbar_init(&a_empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&acc_full[s], 1);
-      mbar_init(&acc_empty[s], epi_warps);
+      mbar_init(&a_empty[s], EPI_WARPS);
     }
     mbar_init(w_full, 1);
     fence_barrier_init();
@@ -571,14 +527,11 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_halo_kernel(const __grid_c
       tma_prefetch_desc(&maps.a_lo[i]);
     }
   }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tbase = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == EPI_WARPS) {
     // ------------------------------------------------------------------ TMA producer
-    if (elect_one()) {   // one thread, chosen by elect.sync: ptxas then emits bare UTCHMMA / UTMALDG (no per-instruction ELECT loop)
+    if (elect_one()) {
       // resident weights: slot (tap, chunk) = [Wh (BN rows) | Wl (BN rows)], K column of the packed weight = (tap, chunk)
       mbar_arrive_expect_tx(w_full, static_cast<uint32_t>(w_bytes));
       for (int tap = 0; tap < 9; ++tap)
@@ -603,60 +556,57 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_halo_kernel(const __grid_c
             }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (elect_one()) {   // one thread, chosen by elect.sync: ptxas then emits bare UTCHMMA / UTMALDG (no per-instruction ELECT loop)
-      const uint32_t idesc = idesc_bf16(BM, BN), idesc2 = idesc_bf16(BM, 2 * BN);
-      const uint64_t d_a0 = umma_desc_sw128(smem_u32(ring), 16, HALO_W * 128);
-      const uint64_t d_w0 = umma_desc_sw128(smem_u32(smem), 16, 1024);
-      mbar_wait(w_full, 0);
-      uint32_t it = 0, local = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-        const int buf = local & 1;
-        mbar_wait(&acc_empty[buf], ((local >> 1) & 1) ^ 1);
-        tc_fence_after_sync();
-        const uint32_t d = tbase + buf * Cfg<BN>::ACC_COLS;
-        for (int pc = 0; pc < pieces; ++pc, ++it) {
-          const int slot = it % nslots;
-          const int chunk = pc >> 1, lo = pc & 1;
-          mbar_wait(&a_full[slot], (it / nslots) & 1);
-          tc_fence_after_sync();
-          // Issue loop kept as tight as possible — the layers served here are bound by the issuing thread, not by the
-          // tensor pipe (N <= 128: the pipe needs <= 64 cycles per MMA): taps fully unrolled so that the halo shift
-          // (dy*10 + dx pixels) is an immediate, one running 64-bit add per weight slot, hi / lo pieces in separate loops.
-          const uint64_t da = d_a0 + ((slot * HALO_SLOT) >> 4);
-          uint64_t dw = d_w0 + ((chunk * 2 * W_TILE) >> 4);
-          const uint32_t wstep = static_cast<uint32_t>(p.chunks_total * 2 * W_TILE) >> 4;
-          if (lo) {
+  } else {
+    // ------------------------------------------------------------------ consumers: wgmma main loop, then the epilogue
+    // warpgroup wg owns tile rows [8 wg, 8 wg + 8) = accumulator rows [64 wg, 64 wg + 64): its A operand starts 8 halo
+    // rows further
+    const int wg = warp >> 2, wq = warp & 3;
+    const uint64_t d_a0 = gmma_desc_sw128(smem_u32(ring) + wg * 8 * HALO_W * 128, 16, HALO_W * 128);
+    const uint64_t d_w0 = gmma_desc_sw128(smem_u32(smem), 16, 1024);
+    constexpr int NCH = BN / 32;
+    const int c_split = (NCH + 1) / 2;
+    const int c_begin = (wq >> 1) ? c_split : 0, c_end = (wq >> 1) ? NCH : c_split;
+    uint8_t* my_stage = epi_stage + warp * EPI_STAGE;
+    float acc[BN / 2];
+    mbar_wait(w_full, 0);
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      for (int pc = 0; pc < pieces; ++pc, ++it) {
+        const int slot = it % nslots;
+        const int chunk = pc >> 1, lo = pc & 1;
+        mbar_wait(&a_full[slot], (it / nslots) & 1);
+        // taps fully unrolled so that the halo shift (dy*10 + dx pixels) is an immediate, one running 64-bit add per
+        // weight slot, hi / lo pieces in separate loops
+        const uint64_t da = d_a0 + ((slot * HALO_SLOT) >> 4);
+        uint64_t dw = d_w0 + ((chunk * 2 * W_TILE) >> 4);
+        const uint32_t wstep = static_cast<uint32_t>(p.chunks_total * 2 * W_TILE) >> 4;
+        wgmma_fence();
+        if (lo) {
 #pragma unroll
-            for (int tap = 0; tap < 9; ++tap, dw += wstep) {
-              const uint64_t dat = da + ((((tap / 3) * HALO_W + tap % 3) * 128) >> 4);
+          for (int tap = 0; tap < 9; ++tap, dw += wstep) {
+            const uint64_t dat = da + ((((tap / 3) * HALO_W + tap % 3) * 128) >> 4);
 #pragma unroll
-              for (int k = 0; k < BK / 16; ++k) umma_f16(d, dat + 2 * k, dw + 2 * k, idesc, 1);                 // + Al.Wh
-            }
-          } else {
+            for (int k = 0; k < BK / 16; ++k) wgmma_ss<BN, false>(acc, dat + 2 * k, dw + 2 * k, 1);      // + Al.Wh
+          }
+        } else {
 #pragma unroll
-            for (int tap = 0; tap < 9; ++tap, dw += wstep) {
-              const uint64_t dat = da + ((((tap / 3) * HALO_W + tap % 3) * 128) >> 4);
+          for (int tap = 0; tap < 9; ++tap, dw += wstep) {
+            const uint64_t dat = da + ((((tap / 3) * HALO_W + tap % 3) * 128) >> 4);
 #pragma unroll
-              for (int k = 0; k < BK / 16; ++k) umma_f16(d, dat + 2 * k, dw + 2 * k, idesc2, (pc | tap | k) != 0);   // [Ah.Wh | Ah.Wl]
+            for (int k = 0; k < BK / 16; ++k) {
+              wgmma_ss<BN, false>(acc, dat + 2 * k, dw + (W_TILE >> 4) + 2 * k, (pc | tap | k) != 0);    // Ah.Wl
+              wgmma_ss<BN, false>(acc, dat + 2 * k, dw + 2 * k, 1);                                       // + Ah.Wh
             }
           }
-          umma_commit(&a_empty[slot]);
         }
-        umma_commit(&acc_full[buf]);
+        wgmma_commit();
+        wgmma_wait<1>();                                  // the previous piece's MMAs are done: release its slot
+        if (pc > 0 && lane == 0) mbar_arrive(&a_empty[(it - 1) % nslots]);
       }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue
-    const int q = warp & 3;                                   // TMEM lane quarter this warp may read
-    constexpr int NCH = BN / 32;                              // 32-column chunks per tile, split between the two warps of a quarter
-    const int c_split = epi_warps > 4 ? (NCH + 1) / 2 : NCH;
-    const int c_begin = (warp - 2) < 4 ? 0 : c_split, c_end = (warp - 2) < 4 ? c_split : NCH;
-    uint8_t* my_stage = epi_stage + (warp - 2) * EPI_STAGE;
-    uint32_t local = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-      const int buf = local & 1;
+      wgmma_wait<0>();
+      if (pieces > 0 && lane == 0) mbar_arrive(&a_empty[(it - 1) % nslots]);
+      acc_stage_store<BN>(acc_smem, acc, wg * 64 + wq * 16, lane);
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
       TileCoord t;
       t.x0 = (tile % tiles_x) * HTILE_W;
       t.y0 = ((tile / tiles_x) % tiles_y) * HTILE_H;
@@ -664,18 +614,11 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_halo_kernel(const __grid_c
       t.g = 0;
       t.co0 = 0;
       t.ph = t.oy = t.ox = 0;
-      mbar_wait(&acc_full[buf], (local >> 1) & 1);
-      tc_fence_after_sync();
-      epilogue_tile<BN>(p, t, tbase + (static_cast<uint32_t>(q * 32) << 16) + buf * Cfg<BN>::ACC_COLS, q * 32 + lane,
-                        p.Cout, bias_s, c_begin, c_end, my_stage, HTILE_W, HTILE_H);
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
+      epilogue_tile<BN>(p, t, acc_smem, wg * 64 + 32 * (wq & 1) + lane, p.Cout, bias_s, c_begin, c_end, my_stage, HTILE_W,
+                        HTILE_H);
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
     }
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tbase, TMEM_COLS);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -756,7 +699,7 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
   // own size: the A boxes shrink from 16 KB to 1-4 KB per K block, and these few-CTA launches are bound by the per-SM L2
   // port.  Otherwise the tile_w x tile_h <= 128 box that covers the image with the FEWEST tiles: at 60 x 108 (every
   // propagation / encoder conv of a 432x240 clip) 12 x 10 tiles the image exactly with 54 tiles where 16 x 8 needs 56 —
-  // at 8 clips that is 432 instead of 448 tiles on 148 SMs, i.e. 3 waves instead of 4.
+  // at 8 clips that is 432 instead of 448 tiles.
   int tile_w = TILE_W, tile_h = TILE_H;
   if (geom) {
     tile_w = geom->tile_w;
@@ -794,8 +737,7 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
   }
   const int cog = cout / groups;
   int bn = cog <= 32 ? 32 : (cog <= 64 ? 64 : (cog == 96 ? 96 : 128));
-  // few tiles (single-clip propagation steps: 51 pixel tiles on 148 SMs): halve the N tile so that twice as many SMs
-  // work; a tile then costs (64 + 55) instead of (128 + 64) tensor-pipe cycles per K step (tools/mma_rate_probe.cu)
+  // few tiles (single-clip propagation steps: 51 pixel tiles): halve the N tile so that twice as many SMs work
   if (bn == 128 && cog % 64 == 0 && !in_rows) {
     const long long t128 = static_cast<long long>(n) * ((h + tile_h - 1) / tile_h) * ((w + tile_w - 1) / tile_w) * groups *
                            ((cog + 127) / 128) * (geom ? geom->nphase : 1);
@@ -867,16 +809,13 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
   // in shared memory next to >= 3 halo slots.  E2F_CONV_HALO=0 forces the generic kernel (A/B timing, debugging).
   int chunks_all = 0;
   for (int i = 0; i < nsrc; ++i) chunks_all += (src_channels[i] / groups + BK - 1) / BK;
-  int halo_slots = 0, halo_epi = 8;
+  int halo_slots = 0;
   if (!geom && !in_rows && ks == 3 && stride == 1 && pad == 1 && groups == 1 && cout <= 64) {
     static const bool enabled = [] {
       const char* e = getenv("E2F_CONV_HALO");
       return !(e && e[0] == '0');
     }();
-    // 8 epilogue warps when their staging buffers fit next to the resident weights, else 4 (64 -> 64: 144 KB of weights)
-    const int room8 = SMEM_LIMIT - 1024 - 256 - MAX_COUT * 4 - halo_w_bytes(bn, chunks_all) - 8 * EPI_STAGE;
-    halo_epi = room8 >= 3 * HALO_SLOT ? 8 : 4;
-    const int room = room8 + (8 - halo_epi) * EPI_STAGE;
+    const int room = SMEM_LIMIT - 1024 - 256 - MAX_COUT * 4 - halo_w_bytes(bn, chunks_all) - EPI_WARPS * EPI_STAGE - BM * bn * 4;
     if (enabled && room >= 3 * HALO_SLOT) halo_slots = room / HALO_SLOT < HALO_MAX_SLOTS ? room / HALO_SLOT : HALO_MAX_SLOTS;
   }
   const cuuint32_t estr4[4] = {1, static_cast<cuuint32_t>(stride), static_cast<cuuint32_t>(stride), 1};
@@ -957,12 +896,12 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
       return -2;
     }
     const int hgrid = htiles < num_sms() ? static_cast<int>(htiles) : num_sms();
-    const int hsmem = 1024 + halo_w_bytes(bn, chunks_all) + halo_slots * HALO_SLOT + 256 + MAX_COUT * 4 + halo_epi * EPI_STAGE;
-    const int hthreads = (2 + halo_epi) * 32;
+    const int hsmem = 1024 + halo_w_bytes(bn, chunks_all) + halo_slots * HALO_SLOT + 256 + MAX_COUT * 4 + EPI_WARPS * EPI_STAGE +
+                      BM * bn * 4;
     if (bn == 32)
-      conv3x3_halo_kernel<32><<<hgrid, hthreads, hsmem, stream>>>(maps, p, halo_slots);
+      conv3x3_halo_kernel<32><<<hgrid, THREADS, hsmem, stream>>>(maps, p, halo_slots);
     else
-      conv3x3_halo_kernel<64><<<hgrid, hthreads, hsmem, stream>>>(maps, p, halo_slots);
+      conv3x3_halo_kernel<64><<<hgrid, THREADS, hsmem, stream>>>(maps, p, halo_slots);
     count_launch();
     return static_cast<int>(cudaGetLastError());
   }

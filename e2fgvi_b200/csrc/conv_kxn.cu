@@ -1,18 +1,18 @@
 // "kx-in-N" convolution for the layers with FEW OUTPUT CHANNELS: SPyNet's 64 -> 32 and 32 -> 16 7x7 convs
 // (model/modules/flow_comp.py:181-215) and the decoder's 64 -> 3 output conv (model/e2fgvi.py:149-150, + tanh :262).
 //
-// Why: with pixels as the M dimension of the implicit GEMM, one tcgen05.mma (M = 128, K = 16) re-reads its 4 KB A tile
-// from shared memory whatever N is — ~55 cycles per instruction for N <= 64 (tools/mma_rate_probe.cu) — so a conv with
-// Cout = 32 keeps the tensor pipe ~25 % busy and one with Cout = 3 ~3 % (conv_bench: 240 / 94 / 24 TFLOP/s).  Here the
-// kernel COLUMN taps go into N instead of K:
+// Why: with pixels as the M dimension of the implicit GEMM, every MMA re-reads its A tile from shared memory whatever N
+// is, so a conv with Cout = 32 or Cout = 3 leaves the tensor pipe mostly idle.  Here the kernel COLUMN taps go into N
+// instead of K:
 //     D[(y, xin), (kx, co)] = sum_{ky, c} X[y + ky - pad, xin, c] * W[co, c, ky, kx]          (K = ks * C, N = ks * Cout)
 //     out[y, x, co]         = sum_{kx}    D[(y, x + kx - pad), (kx, co)]
 // One A tile read now feeds ks times more output columns (N = 224 for 7 x 32: the MMA is math-bound again), the K loop is
 // ks times shorter, and the horizontal shift-and-add of the second line is done by the epilogue: a tile is 4 rows x 32
-// columns of D, i.e. ONE WARP PER TILE ROW, so `D[.., x + kx - pad]` is a warp shuffle away.  Cost: the 2 * pad border
-// columns of every 32-column tile are recomputed by its neighbour (26 / 32 useful for 7x7, 30 / 32 for 3x3).
-// fp32-level accuracy as everywhere: bf16 (hi, lo) operand pairs, D += Ah.Wh + Ah.Wl + Al.Wh, fp32 accumulation in TMEM.
-// Pipeline = conv.cu: persistent CTAs, TMA warp / MMA warp / 4 epilogue warps, double-buffered TMEM accumulator.
+// columns of D; the accumulator columns of one kx at a time are staged in shared memory and every thread adds
+// `D[.., x + kx - pad]` of its output pixel.  Cost: the 2 * pad border columns of every 32-column tile are recomputed by
+// its neighbour (26 / 32 useful for 7x7, 30 / 32 for 3x3).
+// fp32-level accuracy as everywhere: bf16 (hi, lo) operand pairs, D += Ah.Wh + Ah.Wl + Al.Wh, fp32 accumulation.
+// Pipeline = conv.cu: persistent CTAs, TMA warp + two consumer warpgroups (64 accumulator rows each, in registers).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cstdlib>
@@ -24,7 +24,10 @@ namespace kxn {
 
 constexpr int BM = 128, BK = 64, TW = 32, TH = 4;
 constexpr int A_TILE = BM * BK * 2;
-constexpr int THREADS = 6 * 32;                       // TMA, MMA, 4 epilogue warps
+constexpr int CONSUMER_WARPS = 8;                     // two warpgroups x 64 accumulator rows
+constexpr int THREADS = (CONSUMER_WARPS + 1) * 32;    // + the TMA warp
+// one kx slice of the accumulator, [128 rows][co_pad + 4] fp32 (the +4 keeps row-parallel 16-byte reads conflict-free)
+constexpr int KSTAGE_BYTES = 128 * (32 + 4) * 4;
 constexpr int EPI_TANH = 1, EPI_NCHW = 2;
 
 constexpr int MAX_SRC = 2;
@@ -49,10 +52,6 @@ struct Params {
   __nv_bfloat16* out_lo;
 };
 
-__host__ __device__ constexpr uint32_t idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
-
 __device__ __forceinline__ void tma_load_4d(uint32_t smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2, int c3) {
   asm volatile(
       "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
@@ -64,40 +63,32 @@ __device__ __forceinline__ void tma_load_4d(uint32_t smem_dst, const void* tmap,
 // ONE box of TH + ks - 1 rows per chunk brings the tile's whole vertical halo; the A tile of tap row ky is rows
 // [32*ky, 32*ky + 128) of it — a descriptor start shifted by ky * 4096 B, a multiple of the 1024-byte swizzle atom — and only
 // the weights stream per ky through their own ring.  A bytes per tile drop 2x (3x3) to 2.8x (7x7).
-template <bool HALO>
+template <bool HALO, int KS, int CO_PAD>
 __global__ void __launch_bounds__(THREADS, 1) conv_kxn_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p) {
+  constexpr int NB = KS * CO_PAD;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int ring_bytes = HALO ? p.a_slots * p.a_slot_bytes + p.w_slots * p.w_slot_bytes : p.stages * p.stage_bytes;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + ring_bytes);      // plain: stage full / HALO: A slot full
   uint64_t* empty = full + 4;
-  uint64_t* acc_full = empty + 4;
-  uint64_t* acc_empty = acc_full + 2;
-  uint64_t* w_full = acc_empty + 2;                                      // HALO: weight ring
+  uint64_t* w_full = empty + 4;                                          // HALO: weight ring
   uint64_t* w_empty = w_full + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(w_empty + 4);
   float* bias_s = reinterpret_cast<float*>(smem + ring_bytes + 256);     // [512]
+  float* kstage = bias_s + 512;                                          // [128][CO_PAD + 4]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int W_TILE = p.NB * BK * 2;
+  constexpr int W_TILE = NB * BK * 2;
   const int step_x = TW - 2 * p.pad;                                   // output columns a tile produces
   const int tiles_x = (p.W + step_x - 1) / step_x, tiles_y = (p.H + TH - 1) / TH;
   const int num_tiles = p.N * tiles_y * tiles_x * p.groups;
-  const int num_kb = p.ks * p.chunks;
-  const uint32_t tmem_cols = (2 * p.NB <= 256) ? 256u : 512u;
   for (int i = tid; i < 512; i += THREADS) bias_s[i] = (p.bias && i < p.cout_total) ? __ldg(p.bias + i) : 0.f;
 
-  if (warp == 1) tmem_alloc(tmem_slot, tmem_cols);
   if (tid == 0) {
     for (int s = 0; s < 4; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], CONSUMER_WARPS);
       mbar_init(&w_full[s], 1);
-      mbar_init(&w_empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&acc_full[s], 1);
-      mbar_init(&acc_empty[s], 4);
+      mbar_init(&w_empty[s], CONSUMER_WARPS);
     }
     fence_barrier_init();
     for (int i = 0; i < p.nsrc; ++i) {
@@ -107,12 +98,9 @@ __global__ void __launch_bounds__(THREADS, 1) conv_kxn_kernel(const __grid_const
     tma_prefetch_desc(&maps.w_hi);
     tma_prefetch_desc(&maps.w_lo);
   }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tbase = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == CONSUMER_WARPS) {
     // ------------------------------------------------------------------ TMA producer
     if (elect_one()) {
       if (HALO) {
@@ -170,80 +158,69 @@ __global__ void __launch_bounds__(THREADS, 1) conv_kxn_kernel(const __grid_const
       }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (elect_one()) {
-      const uint32_t idesc = idesc_bf16(BM, p.NB);
+  } else {
+    // ------------------------------------------------------------------ consumers: wgmma main loop
+    // warpgroup wg owns accumulator rows [64 wg, 64 wg + 64) = tile rows 2 wg, 2 wg + 1
+    const int wg = warp >> 2, wq = warp & 3;
+    float d[NB / 2];
+    uint32_t it = 0, ia = 0, iw = 0;
+    const uint64_t d_w0 = gmma_desc_sw128(smem_u32(smem + (HALO ? p.a_slots * p.a_slot_bytes : 2 * A_TILE)), 16, 1024);
+    const uint64_t d_a0 = gmma_desc_sw128(smem_u32(smem) + wg * 64 * 128, 16, 1024);
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       if (HALO) {
         const int HR = TH + p.ks - 1;
         const uint32_t lo_off = static_cast<uint32_t>(HR * TW * 128) >> 4;
-        const uint64_t d_a0 = umma_desc_sw128(smem_u32(smem), 16, 1024);
-        const uint64_t d_w0 = umma_desc_sw128(smem_u32(smem + p.a_slots * p.a_slot_bytes), 16, 1024);
-        uint32_t ia = 0, iw = 0, local = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-          const int buf = local & 1;
-          mbar_wait(&acc_empty[buf], ((local >> 1) & 1) ^ 1);
-          tc_fence_after_sync();
-          const uint32_t d = tbase + buf * p.NB;
-          for (int chunk = 0; chunk < p.chunks; ++chunk, ++ia) {
-            const int aslot = ia % p.a_slots;
-            mbar_wait(&full[aslot], (ia / p.a_slots) & 1);
-            const uint64_t d_ah = d_a0 + (static_cast<uint32_t>(aslot * p.a_slot_bytes) >> 4);
-            for (int ky = 0; ky < p.ks; ++ky, ++iw) {
-              const int wslot = iw % p.w_slots;
-              mbar_wait(&w_full[wslot], (iw / p.w_slots) & 1);
-              tc_fence_after_sync();
-              const uint64_t dah0 = d_ah + ((static_cast<uint32_t>(ky) * TW * 128) >> 4);   // rows [32 ky, 32 ky + 128) of the halo
-              const uint64_t dwh0 = d_w0 + (static_cast<uint32_t>(wslot * p.w_slot_bytes) >> 4);
-              const uint64_t dwl0 = dwh0 + (static_cast<uint32_t>(W_TILE) >> 4);
+        for (int chunk = 0; chunk < p.chunks; ++chunk, ++ia) {
+          const int aslot = ia % p.a_slots;
+          mbar_wait(&full[aslot], (ia / p.a_slots) & 1);
+          const uint64_t d_ah = d_a0 + (static_cast<uint32_t>(aslot * p.a_slot_bytes) >> 4);
+          for (int ky = 0; ky < KS; ++ky, ++iw) {
+            const int wslot = iw % p.w_slots;
+            mbar_wait(&w_full[wslot], (iw / p.w_slots) & 1);
+            const uint64_t dah0 = d_ah + ((static_cast<uint32_t>(ky) * TW * 128) >> 4);   // rows [32 ky, 32 ky + 128) of the halo
+            const uint64_t dwh0 = d_w0 + (static_cast<uint32_t>(wslot * p.w_slot_bytes) >> 4);
+            const uint64_t dwl0 = dwh0 + (static_cast<uint32_t>(W_TILE) >> 4);
+            wgmma_fence();
 #pragma unroll
-              for (int k = 0; k < BK / 16; ++k) {
-                const uint64_t dah = dah0 + 2 * k, dal = dah0 + lo_off + 2 * k;
-                umma_f16(d, dal, dwh0 + 2 * k, idesc, (chunk | ky | k) != 0);   // small terms first
-                umma_f16(d, dah, dwl0 + 2 * k, idesc, 1);
-                umma_f16(d, dah, dwh0 + 2 * k, idesc, 1);
-              }
-              umma_commit(&w_empty[wslot]);
+            for (int k = 0; k < BK / 16; ++k) {
+              const uint64_t dah = dah0 + 2 * k, dal = dah0 + lo_off + 2 * k;
+              wgmma_ss<NB, false>(d, dal, dwh0 + 2 * k, (chunk | ky | k) != 0);   // small terms first
+              wgmma_ss<NB, false>(d, dah, dwl0 + 2 * k, 1);
+              wgmma_ss<NB, false>(d, dah, dwh0 + 2 * k, 1);
             }
-            umma_commit(&empty[aslot]);
+            wgmma_commit();
+            wgmma_wait<0>();
+            if (lane == 0) mbar_arrive(&w_empty[wslot]);
           }
-          umma_commit(&acc_full[buf]);
+          if (lane == 0) mbar_arrive(&empty[aslot]);
         }
       } else {
-      const uint64_t d_ah0 = umma_desc_sw128(smem_u32(smem), 16, 1024);
-      const uint64_t d_al0 = umma_desc_adv(d_ah0, A_TILE), d_wh0 = umma_desc_adv(d_ah0, 2 * A_TILE);
-      const uint64_t d_wl0 = umma_desc_adv(d_wh0, W_TILE);
-      uint32_t it = 0, local = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-        const int buf = local & 1;
-        mbar_wait(&acc_empty[buf], ((local >> 1) & 1) ^ 1);
-        tc_fence_after_sync();
-        const uint32_t d = tbase + buf * p.NB;
+        const int num_kb = KS * p.chunks;
+        const uint64_t d_al0 = gmma_desc_adv(d_a0, A_TILE), d_wl0 = gmma_desc_adv(d_w0, W_TILE);
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
           const int stage = it % p.stages;
           mbar_wait(&full[stage], (it / p.stages) & 1);
-          tc_fence_after_sync();
           const uint32_t soff = static_cast<uint32_t>(stage * p.stage_bytes) >> 4;
+          wgmma_fence();
 #pragma unroll
           for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t dah = d_ah0 + soff + 2 * k, dal = d_al0 + soff + 2 * k;
-            const uint64_t dwh = d_wh0 + soff + 2 * k, dwl = d_wl0 + soff + 2 * k;
-            umma_f16(d, dal, dwh, idesc, (kb | k) != 0);   // small terms first
-            umma_f16(d, dah, dwl, idesc, 1);
-            umma_f16(d, dah, dwh, idesc, 1);
+            const uint64_t dah = d_a0 + soff + 2 * k, dal = d_al0 + soff + 2 * k;
+            const uint64_t dwh = d_w0 + soff + 2 * k, dwl = d_wl0 + soff + 2 * k;
+            wgmma_ss<NB, false>(d, dal, dwh, (kb | k) != 0);   // small terms first
+            wgmma_ss<NB, false>(d, dah, dwl, 1);
+            wgmma_ss<NB, false>(d, dah, dwh, 1);
           }
-          umma_commit(&empty[stage]);
+          wgmma_commit();
+          wgmma_wait<1>();                                    // the previous K block's MMAs are done: release its stage
+          if (kb > 0 && lane == 0) mbar_arrive(&empty[(it - 1) % p.stages]);
         }
-        umma_commit(&acc_full[buf]);
+        wgmma_wait<0>();
+        if (num_kb > 0 && lane == 0) mbar_arrive(&empty[(it - 1) % p.stages]);
       }
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue: one warp per tile row
-    const int q = warp & 3;                                   // TMEM lane quarter == tile row
-    uint32_t local = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-      const int buf = local & 1;
+
+      // ---------------------------------------------------------------- epilogue: warp -> tile row q, lane -> output column
+      const int q = warp & 3, half = warp >> 2;               // tile row; first or second half of the 8-channel chunks
+      constexpr int CCH = CO_PAD / 16;                        // 8-channel chunks per warp
       const int g = tile % p.groups, tp = tile / p.groups;
       const int tx = tp % tiles_x, ty = (tp / tiles_x) % tiles_y, n = tp / (tiles_x * tiles_y);
       const int cbase = g * p.Cout;                                       // first output channel of the group
@@ -251,23 +228,36 @@ __global__ void __launch_bounds__(THREADS, 1) conv_kxn_kernel(const __grid_const
       const int y = ty * TH + q, x = tx * step_x + lane - p.pad;          // this lane's OUTPUT pixel
       const bool ok = lane >= p.pad && lane < TW - p.pad && y < p.H && x < p.W;
       const size_t pix = (static_cast<size_t>(n) * p.H + y) * p.W + x;
-      mbar_wait(&acc_full[buf], (local >> 1) & 1);
-      tc_fence_after_sync();
-      const uint32_t taddr = tbase + (static_cast<uint32_t>(q * 32) << 16) + buf * p.NB;
-#pragma unroll 1
-      for (int cc = 0; cc < p.co_pad / 8; ++cc) {
-        float acc[8];
+      float accs[CCH][8];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-#pragma unroll 1
-        for (int kx = 0; kx < p.ks; ++kx) {
-          uint32_t v[8];
-          tmem_ld8(taddr + kx * p.co_pad + cc * 8, v);
-          tmem_ld_wait();
-          const int src = lane + kx - p.pad;                  // D column this output needs for tap kx (same tile row)
+      for (int u = 0; u < CCH; ++u)
 #pragma unroll
-          for (int i = 0; i < 8; ++i) acc[i] += __shfl_sync(0xffffffffu, __uint_as_float(v[i]), src & 31);
+        for (int i = 0; i < 8; ++i) accs[u][i] = 0.f;
+#pragma unroll
+      for (int kx = 0; kx < KS; ++kx) {
+        // stage accumulator columns [kx * CO_PAD, +CO_PAD) of all 128 rows
+        const int r = wg * 64 + wq * 16 + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+        for (int j = kx * CO_PAD / 8; j < (kx + 1) * CO_PAD / 8; ++j) {
+          const int col = 8 * j + c - kx * CO_PAD;
+          *reinterpret_cast<float2*>(kstage + r * (CO_PAD + 4) + col) = make_float2(d[4 * j], d[4 * j + 1]);
+          *reinterpret_cast<float2*>(kstage + (r + 8) * (CO_PAD + 4) + col) = make_float2(d[4 * j + 2], d[4 * j + 3]);
         }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        const int sr = q * 32 + ((lane + kx - p.pad) & 31);       // D column this output needs for tap kx (same tile row)
+#pragma unroll
+        for (int u = 0; u < CCH; ++u) {
+          const float4* s4 = reinterpret_cast<const float4*>(kstage + sr * (CO_PAD + 4) + (half * CCH + u) * 8);
+          const float4 a = s4[0], b = s4[1];
+          accs[u][0] += a.x; accs[u][1] += a.y; accs[u][2] += a.z; accs[u][3] += a.w;
+          accs[u][4] += b.x; accs[u][5] += b.y; accs[u][6] += b.z; accs[u][7] += b.w;
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+      }
+#pragma unroll
+      for (int u = 0; u < CCH; ++u) {
+        float* acc = accs[u];
+        const int cc = half * CCH + u;
         const int co0 = cc * 8;
         if (ok && co0 < p.Cout) {
 #pragma unroll
@@ -308,14 +298,8 @@ __global__ void __launch_bounds__(THREADS, 1) conv_kxn_kernel(const __grid_const
           }
         }
       }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
     }
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tbase, tmem_cols);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -353,8 +337,8 @@ int launch_conv_kxn(int nsrc, const void* const* src_hi, const void* const* src_
     return -2;
   }
   const int cog = cout / groups;
-  if ((ks != 3 && ks != 7) || co_pad % 8 || cog > co_pad || co_pad > 32 || NB % 16 || NB > 256) {
-    set_error("conv_kxn: unsupported shape (ks=%d cout/groups=%d co_pad=%d): needs ks in {3,7}, co_pad %% 8 == 0 <= 32, ks*co_pad %% 16 == 0", ks, cog, co_pad);
+  if ((ks != 3 && ks != 7) || (co_pad != 16 && co_pad != 32) || cog > co_pad) {
+    set_error("conv_kxn: unsupported shape (ks=%d cout/groups=%d co_pad=%d): needs ks in {3,7}, co_pad in {16,32}", ks, cog, co_pad);
     return -2;
   }
   if (out_hi && (cog % 8 || cout % 8)) {
@@ -381,18 +365,19 @@ int launch_conv_kxn(int nsrc, const void* const* src_hi, const void* const* src_
   }
   const int w_tile = NB * BK * 2;
   p.stage_bytes = 2 * A_TILE + 2 * w_tile;                      // multiple of 1024 (NB % 16 == 0 -> NB*128 % 2048 == 0)
-  p.stages = (3 * p.stage_bytes + 4096 <= 225 * 1024) ? 3 : 2;
+  const int extra = 4096 + KSTAGE_BYTES;                        // barriers, bias, kx staging, alignment
+  p.stages = (3 * p.stage_bytes + extra <= 227 * 1024) ? 3 : 2;
   // HALO variant where A dominates the operand traffic and two halo slots + >= 2 weight slots fit
   const int HR = TH + ks - 1;
   p.a_slot_bytes = 2 * HR * TW * 128;
   p.a_slots = 2;
   p.w_slot_bytes = 2 * w_tile;
   p.w_slots = 3;
-  // measured (profiles/r02/kxn_bench_run11*.log): the halo variant wins for the two-chunk 3x3 grouped layer (enc7: 843 ->
-  // 804 us) and loses where a tile has ONE chunk (no A prefetch across the tile boundary hides behind 3 or 7 tap rows)
+  // the halo variant pays off for the multi-chunk 3x3 layers; where a tile has ONE chunk no A prefetch across the tile
+  // boundary hides behind the 3 or 7 tap rows
   bool halo = NB <= 112 && ks == 3 && p.chunks >= 2;
-  if (halo && p.a_slots * p.a_slot_bytes + p.w_slots * p.w_slot_bytes + 4096 > 227 * 1024) p.w_slots = 2;
-  if (halo && p.a_slots * p.a_slot_bytes + p.w_slots * p.w_slot_bytes + 4096 > 227 * 1024) halo = false;
+  if (halo && p.a_slots * p.a_slot_bytes + p.w_slots * p.w_slot_bytes + extra > 227 * 1024) p.w_slots = 2;
+  if (halo && p.a_slots * p.a_slot_bytes + p.w_slots * p.w_slot_bytes + extra > 227 * 1024) halo = false;
   {
     static const bool off = [] {
       const char* e = getenv("E2F_KXN_HALO");
@@ -400,7 +385,7 @@ int launch_conv_kxn(int nsrc, const void* const* src_hi, const void* const* src_
     }();
     if (off) halo = false;
   }
-  if (!halo && p.stages * p.stage_bytes + 4096 > 227 * 1024) {
+  if (!halo && p.stages * p.stage_bytes + extra > 227 * 1024) {
     set_error("conv_kxn: stage does not fit in shared memory");
     return -2;
   }
@@ -439,8 +424,11 @@ int launch_conv_kxn(int nsrc, const void* const* src_hi, const void* const* src_
   static DeviceOnce cfg;
   const int dev = current_device();
   if (!device_done(cfg, dev)) {
-    cudaError_t e = cudaFuncSetAttribute(conv_kxn_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_kxn_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaError_t e = cudaSuccess;
+    for (auto kern : {conv_kxn_kernel<false, 3, 16>, conv_kxn_kernel<false, 3, 32>, conv_kxn_kernel<false, 7, 16>,
+                      conv_kxn_kernel<false, 7, 32>, conv_kxn_kernel<true, 3, 16>, conv_kxn_kernel<true, 3, 32>,
+                      conv_kxn_kernel<true, 7, 16>, conv_kxn_kernel<true, 7, 32>})
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return static_cast<int>(e);
     device_mark(cfg, dev);
   }
@@ -452,13 +440,12 @@ int launch_conv_kxn(int nsrc, const void* const* src_hi, const void* const* src_
     return -2;
   }
   const int grid = tiles < num_sms() ? static_cast<int>(tiles) : num_sms();
-  if (halo) {
-    const int smem = p.a_slots * p.a_slot_bytes + p.w_slots * p.w_slot_bytes + 4096;
-    conv_kxn_kernel<true><<<grid, THREADS, smem, stream>>>(maps, p);
-  } else {
-    const int smem = p.stages * p.stage_bytes + 4096;
-    conv_kxn_kernel<false><<<grid, THREADS, smem, stream>>>(maps, p);
-  }
+  const int smem = (halo ? p.a_slots * p.a_slot_bytes + p.w_slots * p.w_slot_bytes : p.stages * p.stage_bytes) + extra;
+  auto kern = halo ? (ks == 3 ? (co_pad == 16 ? conv_kxn_kernel<true, 3, 16> : conv_kxn_kernel<true, 3, 32>)
+                              : (co_pad == 16 ? conv_kxn_kernel<true, 7, 16> : conv_kxn_kernel<true, 7, 32>))
+                   : (ks == 3 ? (co_pad == 16 ? conv_kxn_kernel<false, 3, 16> : conv_kxn_kernel<false, 3, 32>)
+                              : (co_pad == 16 ? conv_kxn_kernel<false, 7, 16> : conv_kxn_kernel<false, 7, 32>));
+  kern<<<grid, THREADS, smem, stream>>>(maps, p);
   count_launch();
   return static_cast<int>(cudaGetLastError());
 }

@@ -3,9 +3,10 @@
 // the offset/mask epilogue of feat_prop.py:41-53 (10*tanh + flow.flip(1), sigmoid) folded into the sampler.
 //
 // GEMM view: out[M=N*H*W, 128] = A[M, K=2304] * Wp[128, K]^T + bias, where the im2col matrix A is never written
-// to global memory: 16 producer warps bilinearly sample x (NHWC fp16, one sample point = 16 channels = 32 B per
-// corner) and store fp16 rows straight into the 128B-swizzled K-major shared-memory tile that tcgen05.mma reads;
-// the packed weight streams in by TMA (SWIZZLE_128B); accumulation is fp32 in TMEM.
+// to global memory: 8 producer warps bilinearly sample x (NHWC fp16, one sample point = 16 channels = 32 B per
+// corner) and store fp16 rows straight into the 128B-swizzled K-major shared-memory tile that wgmma reads; the
+// packed weight streams in by TMA (SWIZZLE_128B).  The same 8 warps are the two consumer warpgroups (64 rows each):
+// the wgmma of K block j runs asynchronously while they sample K block j+1; accumulation is fp32 in registers.
 //   K order: k = sp*16 + c,  sp = g*9 + tap  (so offset channels of sp are 2*sp, 2*sp+1 and its mask channel sp)
 //   one 64-wide K block = 4 consecutive sample points; 36 K blocks; 4-stage mbarrier ring.
 // Roofline (SURVEY §8d): 2*128*2304*M FLOP per call (3.82 GFLOP at M=6480) on the tensor pipe; min bytes
@@ -18,12 +19,10 @@
 namespace e2f {
 namespace dcn {
 
-// 256-bit read-only load (sm_100+, PTX 8.8): the 16 fp16 channels of one (pixel, deform group) are 32 contiguous, 32-byte
-// aligned bytes in both input layouts.  The sampler is bound by L1 tag look-ups (ncu: l1tex 86 %), one per thread and request.
+// the 16 fp16 channels of one (pixel, deform group) are 32 contiguous, 32-byte aligned bytes in both input layouts
 __device__ __forceinline__ void ldg256(const uint4* p, uint4& a, uint4& b) {
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
-               : "l"(p));
+  a = __ldg(p);
+  b = __ldg(p + 1);
 }
 
 constexpr int CIN = 256, COUT = 128, DG = 16, CPG = CIN / DG, TAPS = 9;
@@ -35,11 +34,9 @@ constexpr int SP_PER_KB = BLOCK_K / CPG;     // 4
 constexpr int STAGES = 4;
 constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
 constexpr int B_BYTES = COUT * BLOCK_K * 2;
-constexpr int PRODUCER_WARPS = 16;
-constexpr int PRODUCER_THREADS = PRODUCER_WARPS * 32;   // 512 = 128 rows x 4 sample points
-constexpr int TMA_WARP = PRODUCER_WARPS, MMA_WARP = PRODUCER_WARPS + 1;
-constexpr int THREADS = (PRODUCER_WARPS + 2) * 32;
-constexpr int TMEM_COLS = 128;
+constexpr int PRODUCER_WARPS = 8;                       // 256 threads = 128 rows x 2 pairs of sample points
+constexpr int TMA_WARP = PRODUCER_WARPS;
+constexpr int THREADS = (PRODUCER_WARPS + 1) * 32;
 constexpr int SMEM_BYTES = STAGES * (A_BYTES + B_BYTES) + 256 + 1024;  // + barriers + alignment slack
 
 __device__ __forceinline__ float fast_tanh(float v) {
@@ -65,30 +62,23 @@ dcn_kernel(const __grid_constant__ CUtensorMap tmap_w, const __half* __restrict_
   uint64_t* full_a = reinterpret_cast<uint64_t*>(smem + STAGES * (A_BYTES + B_BYTES));
   uint64_t* full_b = full_a + STAGES;
   uint64_t* empty = full_b + STAGES;
-  uint64_t* accum_bar = empty + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
-  if (warp == MMA_WARP) tmem_alloc(tmem_slot, TMEM_COLS);
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_a[s], PRODUCER_WARPS);
       mbar_init(&full_b[s], 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], PRODUCER_WARPS);
     }
-    mbar_init(accum_bar, 1);
     fence_barrier_init();
   }
   if (warp == TMA_WARP && lane == 0) tma_prefetch_desc(&tmap_w);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tbase = *tmem_slot;
 
   if (warp < PRODUCER_WARPS) {
     // ------------------------------------------------------------------ A producer: sampler + im2col
-    const int r = tid >> 2, s = tid & 3;
+    const int r = tid >> 1, s0 = 2 * (tid & 1);          // row, first of this thread's two sample points
     const long long m = static_cast<long long>(blockIdx.x) * BLOCK_M + r;
     const bool row_valid = m < M;
     const long long mm = row_valid ? m : 0;
@@ -104,127 +94,138 @@ dcn_kernel(const __grid_constant__ CUtensorMap tmap_w, const __half* __restrict_
       fl1 = __ldg(flow1 + mm);
       fl2 = __ldg(flow2 + mm);
     }
-    const uint32_t row_off0 = sw128_offset(r, 2 * s), row_off1 = sw128_offset(r, 2 * s + 1);
+    uint32_t row_off[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) row_off[i] = sw128_offset(r, 2 * s0 + i);
+    const int wg = warp >> 2, wq = warp & 3;
+    // this warpgroup's 64 A rows start 64 * 128 B into the A tile
+    const uint64_t d_a0 = gmma_desc_sw128(smem_u32(sA) + wg * 64 * 128, 16, 1024);
+    const uint64_t d_b0 = gmma_desc_sw128(smem_u32(sB), 16, 1024);
+    float accf[COUT / 2];
 
-    float2 o_next = __ldg(reinterpret_cast<const float2*>(off_p) + s);
-    float m_next = __ldg(msk_p + s);
+    float2 o_next[2];
+    float m_next[2];
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      o_next[u] = __ldg(reinterpret_cast<const float2*>(off_p) + s0 + u);
+      m_next[u] = __ldg(msk_p + s0 + u);
+    }
     for (int j = 0; j < NUM_KB; ++j) {
       const int stage = j % STAGES;
       const uint32_t phase = (j / STAGES) & 1;
-      const int sp = j * SP_PER_KB + s;
-      float2 o = o_next;
-      float mk = m_next;
-      if (j + 1 < NUM_KB) {
-        o_next = __ldg(reinterpret_cast<const float2*>(off_p) + sp + SP_PER_KB);
-        m_next = __ldg(msk_p + sp + SP_PER_KB);
-      }
-      const int g = sp / TAPS, tap = sp - g * TAPS;
-      if (FUSED) {
-        // offset = max_res * tanh(o) + flow.flip(1): even channel (dy) gets v, odd (dx) gets u (feat_prop.py:41-50)
-        const float2 fl = (sp < NSP / 2) ? fl1 : fl2;
-        o.x = fmaf(max_res, fast_tanh(o.x), fl.y);
-        o.y = fmaf(max_res, fast_tanh(o.y), fl.x);
-        mk = fast_sigmoid(mk);
-      }
-      const int ti = tap / 3, tj = tap - ti * 3;
-      const float h_im = static_cast<float>(py - 1 + ti) + o.x;
-      const float w_im = static_cast<float>(px - 1 + tj) + o.y;
-      const bool inside = row_valid && (h_im > -1.f) && (w_im > -1.f) && (h_im < static_cast<float>(H)) &&
-                          (w_im < static_cast<float>(W));
-      float acc[16];
+      uint4 vv[4];
 #pragma unroll
-      for (int i = 0; i < 16; ++i) acc[i] = 0.f;
-      if (inside) {
-        const float fy = floorf(h_im), fx = floorf(w_im);
-        const float ly = h_im - fy, lx = w_im - fx;
-        const int y0 = static_cast<int>(fy), x0 = static_cast<int>(fx);
-        const __half* xg = GROUPED ? xn + static_cast<long long>(g) * H * W * CPG : xn + g * CPG;
-        uint4 lo[4], hi[4];
-        float wgt[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int dy = k >> 1, dx = k & 1;
-          const int yy = y0 + dy, xx = x0 + dx;
-          const bool in = (yy >= 0) && (yy < H) && (xx >= 0) && (xx < W);
-          wgt[k] = in ? (dy ? ly : 1.f - ly) * (dx ? lx : 1.f - lx) * mk : 0.f;
-          const int po = min(max(yy, 0), H - 1) * W + min(max(xx, 0), W - 1);
-          const uint4* p = reinterpret_cast<const uint4*>(xg + static_cast<long long>(po) * PIX_STRIDE);
-          ldg256(p, lo[k], hi[k]);        // one 32-byte request per corner (LDG.E.256): half the L1 tag look-ups of 2 x LDG.128
+      for (int u = 0; u < 2; ++u) {
+        const int sp = j * SP_PER_KB + s0 + u;
+        float2 o = o_next[u];
+        float mk = m_next[u];
+        if (j + 1 < NUM_KB) {
+          o_next[u] = __ldg(reinterpret_cast<const float2*>(off_p) + sp + SP_PER_KB);
+          m_next[u] = __ldg(msk_p + sp + SP_PER_KB);
         }
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const __half2* pl = reinterpret_cast<const __half2*>(&lo[k]);
-          const __half2* ph = reinterpret_cast<const __half2*>(&hi[k]);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float2 a = __half22float2(pl[i]);
-            const float2 b = __half22float2(ph[i]);
-            acc[2 * i] = fmaf(wgt[k], a.x, acc[2 * i]);
-            acc[2 * i + 1] = fmaf(wgt[k], a.y, acc[2 * i + 1]);
-            acc[8 + 2 * i] = fmaf(wgt[k], b.x, acc[8 + 2 * i]);
-            acc[8 + 2 * i + 1] = fmaf(wgt[k], b.y, acc[8 + 2 * i + 1]);
+        const int g = sp / TAPS, tap = sp - g * TAPS;
+        if (FUSED) {
+          // offset = max_res * tanh(o) + flow.flip(1): even channel (dy) gets v, odd (dx) gets u (feat_prop.py:41-50)
+          const float2 fl = (sp < NSP / 2) ? fl1 : fl2;
+          o.x = fmaf(max_res, fast_tanh(o.x), fl.y);
+          o.y = fmaf(max_res, fast_tanh(o.y), fl.x);
+          mk = fast_sigmoid(mk);
+        }
+        const int ti = tap / 3, tj = tap - ti * 3;
+        const float h_im = static_cast<float>(py - 1 + ti) + o.x;
+        const float w_im = static_cast<float>(px - 1 + tj) + o.y;
+        const bool inside = row_valid && (h_im > -1.f) && (w_im > -1.f) && (h_im < static_cast<float>(H)) &&
+                            (w_im < static_cast<float>(W));
+        float acc[16];
+  #pragma unroll
+        for (int i = 0; i < 16; ++i) acc[i] = 0.f;
+        if (inside) {
+          const float fy = floorf(h_im), fx = floorf(w_im);
+          const float ly = h_im - fy, lx = w_im - fx;
+          const int y0 = static_cast<int>(fy), x0 = static_cast<int>(fx);
+          const __half* xg = GROUPED ? xn + static_cast<long long>(g) * H * W * CPG : xn + g * CPG;
+          uint4 lo[4], hi[4];
+          float wgt[4];
+  #pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const int dy = k >> 1, dx = k & 1;
+            const int yy = y0 + dy, xx = x0 + dx;
+            const bool in = (yy >= 0) && (yy < H) && (xx >= 0) && (xx < W);
+            wgt[k] = in ? (dy ? ly : 1.f - ly) * (dx ? lx : 1.f - lx) * mk : 0.f;
+            const int po = min(max(yy, 0), H - 1) * W + min(max(xx, 0), W - 1);
+            const uint4* p = reinterpret_cast<const uint4*>(xg + static_cast<long long>(po) * PIX_STRIDE);
+            ldg256(p, lo[k], hi[k]);
+          }
+  #pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const __half2* pl = reinterpret_cast<const __half2*>(&lo[k]);
+            const __half2* ph = reinterpret_cast<const __half2*>(&hi[k]);
+  #pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const float2 a = __half22float2(pl[i]);
+              const float2 b = __half22float2(ph[i]);
+              acc[2 * i] = fmaf(wgt[k], a.x, acc[2 * i]);
+              acc[2 * i + 1] = fmaf(wgt[k], a.y, acc[2 * i + 1]);
+              acc[8 + 2 * i] = fmaf(wgt[k], b.x, acc[8 + 2 * i]);
+              acc[8 + 2 * i + 1] = fmaf(wgt[k], b.y, acc[8 + 2 * i + 1]);
+            }
           }
         }
+        uint4& v0 = vv[2 * u];
+        uint4& v1 = vv[2 * u + 1];
+        v0.x = pack_half2(acc[0], acc[1]);   v0.y = pack_half2(acc[2], acc[3]);
+        v0.z = pack_half2(acc[4], acc[5]);   v0.w = pack_half2(acc[6], acc[7]);
+        v1.x = pack_half2(acc[8], acc[9]);   v1.y = pack_half2(acc[10], acc[11]);
+        v1.z = pack_half2(acc[12], acc[13]); v1.w = pack_half2(acc[14], acc[15]);
+
       }
-      uint4 v0, v1;
-      v0.x = pack_half2(acc[0], acc[1]);   v0.y = pack_half2(acc[2], acc[3]);
-      v0.z = pack_half2(acc[4], acc[5]);   v0.w = pack_half2(acc[6], acc[7]);
-      v1.x = pack_half2(acc[8], acc[9]);   v1.y = pack_half2(acc[10], acc[11]);
-      v1.z = pack_half2(acc[12], acc[13]); v1.w = pack_half2(acc[14], acc[15]);
 
       mbar_wait(&empty[stage], phase ^ 1);
       uint8_t* a_tile = sA + stage * A_BYTES;
-      *reinterpret_cast<uint4*>(a_tile + row_off0) = v0;
-      *reinterpret_cast<uint4*>(a_tile + row_off1) = v1;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) *reinterpret_cast<uint4*>(a_tile + row_off[i]) = vv[i];
       fence_proxy_async_smem();
       __syncwarp();
       if (lane == 0) mbar_arrive(&full_a[stage]);
-    }
 
-    // ------------------------------------------------------------------ epilogue: TMEM -> +bias -> global
-    mbar_wait(accum_bar, 0);
-    tc_fence_after_sync();
-    const int q = warp & 3, cc = warp >> 2;   // TMEM lane quarter (fixed by warp id % 4), 32-column chunk
-    uint32_t v[32];
-    tmem_ld32(tbase + (static_cast<uint32_t>(q * 32) << 16) + cc * 32, v);
-    tmem_ld_wait();
-    const long long om = static_cast<long long>(blockIdx.x) * BLOCK_M + q * 32 + lane;
-    if (om < M) {
-      float f[32];
+      // K block j on the tensor pipe (asynchronous: it runs while block j+1 is sampled); block j-1 is then complete
+      mbar_wait(&full_a[stage], phase);
+      mbar_wait(&full_b[stage], phase);
+      const uint64_t da = d_a0 + ((stage * A_BYTES) >> 4), db = d_b0 + ((stage * B_BYTES) >> 4);
+      wgmma_fence();
 #pragma unroll
-      for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]) + (bias ? __ldg(bias + cc * 32 + i) : 0.f);
-      if constexpr (sizeof(OutT) == 4) {
-        float4* dst = reinterpret_cast<float4*>(out + om * COUT + cc * 32);
+      for (int k = 0; k < BLOCK_K / 16; ++k) wgmma_ss<COUT, true>(accf, da + 2 * k, db + 2 * k, (j | k) != 0);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (j > 0 && lane == 0) mbar_arrive(&empty[(j - 1) % STAGES]);
+    }
+    wgmma_wait<0>();
+
+    // ------------------------------------------------------------------ epilogue: accumulator fragment -> +bias -> global
+    // rows r0 and r0 + 8 of the tile, column pairs 8c + 2(lane % 4)
+    const long long r0 = static_cast<long long>(blockIdx.x) * BLOCK_M + wg * 64 + wq * 16 + (lane >> 2);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) dst[i] = make_float4(f[4 * i], f[4 * i + 1], f[4 * i + 2], f[4 * i + 3]);
-        if (out_hi) {
-          // bf16 (hi, lo) split of the same values: the operand pair of the backbone conv that consumes the aligned
-          // features (feat_prop.py:131-136), so no standalone split pass runs between the DCN and that conv
-          uint4* dh = reinterpret_cast<uint4*>(out_hi + om * COUT + cc * 32);
-          uint4* dl = reinterpret_cast<uint4*>(out_lo + om * COUT + cc * 32);
+    for (int c = 0; c < COUT / 8; ++c) {
+      const int col = 8 * c + 2 * (lane & 3);
+      const float b0 = bias ? __ldg(bias + col) : 0.f, b1 = bias ? __ldg(bias + col + 1) : 0.f;
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            uint32_t hp[4], lp[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const __nv_bfloat162 hb = __floats2bfloat162_rn(f[8 * i + 2 * j], f[8 * i + 2 * j + 1]);
-              const float2 hf = __bfloat1622float2(hb);
-              const __nv_bfloat162 lb = __floats2bfloat162_rn(f[8 * i + 2 * j] - hf.x, f[8 * i + 2 * j + 1] - hf.y);
-              hp[j] = *reinterpret_cast<const uint32_t*>(&hb);
-              lp[j] = *reinterpret_cast<const uint32_t*>(&lb);
-            }
-            dh[i] = make_uint4(hp[0], hp[1], hp[2], hp[3]);
-            dl[i] = make_uint4(lp[0], lp[1], lp[2], lp[3]);
+      for (int h = 0; h < 2; ++h) {
+        const long long om = r0 + 8 * h;
+        if (om >= M) continue;
+        const float f0 = accf[4 * c + 2 * h] + b0, f1 = accf[4 * c + 2 * h + 1] + b1;
+        if constexpr (sizeof(OutT) == 4) {
+          *reinterpret_cast<float2*>(out + om * COUT + col) = make_float2(f0, f1);
+          if (out_hi) {
+            // bf16 (hi, lo) split of the same values: the operand pair of the backbone conv that consumes the aligned
+            // features (feat_prop.py:131-136), so no standalone split pass runs between the DCN and that conv
+            const __nv_bfloat162 hb = __floats2bfloat162_rn(f0, f1);
+            const float2 hf = __bfloat1622float2(hb);
+            const __nv_bfloat162 lb = __floats2bfloat162_rn(f0 - hf.x, f1 - hf.y);
+            *reinterpret_cast<__nv_bfloat162*>(out_hi + om * COUT + col) = hb;
+            *reinterpret_cast<__nv_bfloat162*>(out_lo + om * COUT + col) = lb;
           }
-        }
-      } else {
-        uint4* dst = reinterpret_cast<uint4*>(out + om * COUT + cc * 32);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          uint4 u;
-          u.x = pack_half2(f[8 * i], f[8 * i + 1]);     u.y = pack_half2(f[8 * i + 2], f[8 * i + 3]);
-          u.z = pack_half2(f[8 * i + 4], f[8 * i + 5]); u.w = pack_half2(f[8 * i + 6], f[8 * i + 7]);
-          dst[i] = u;
+        } else {
+          *reinterpret_cast<uint32_t*>(out + om * COUT + col) = pack_half2(f0, f1);
         }
       }
     }
@@ -239,28 +240,7 @@ dcn_kernel(const __grid_constant__ CUtensorMap tmap_w, const __half* __restrict_
         tma_load_2d(smem_u32(sB + stage * B_BYTES), &tmap_w, &full_b[stage], j * BLOCK_K, 0);
       }
     }
-  } else {
-    // ------------------------------------------------------------------ MMA issuer
-    if (elect_one()) {   // one thread, chosen by elect.sync: ptxas then emits bare UTCHMMA / UTMALDG (no per-instruction ELECT loop)
-      const uint32_t idesc = umma_idesc_f16(BLOCK_M, COUT, 0, 0);
-      const uint64_t d_a0 = umma_desc_sw128(smem_u32(sA), 16, 1024), d_b0 = umma_desc_sw128(smem_u32(sB), 16, 1024);
-      for (int j = 0; j < NUM_KB; ++j) {
-        const int stage = j % STAGES;
-        const uint32_t phase = (j / STAGES) & 1;
-        mbar_wait(&full_a[stage], phase);
-        mbar_wait(&full_b[stage], phase);
-        tc_fence_after_sync();
-        const uint64_t da = d_a0 + ((stage * A_BYTES) >> 4), db = d_b0 + ((stage * B_BYTES) >> 4);
-#pragma unroll
-        for (int k = 0; k < BLOCK_K / 16; ++k) umma_f16(tbase, da + 2 * k, db + 2 * k, idesc, (j | k) != 0);
-        umma_commit(&empty[stage]);
-      }
-      umma_commit(accum_bar);
-    }
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == MMA_WARP) tmem_dealloc(tbase, TMEM_COLS);
 }
 
 __global__ void pack_weight_kernel(const float* __restrict__ w, __half* __restrict__ wp, int cout, int cin, int dg) {

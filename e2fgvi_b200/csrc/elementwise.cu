@@ -23,11 +23,11 @@ __device__ __forceinline__ void split_store8(const float (&f)[8], __nv_bfloat16*
   *reinterpret_cast<uint4*>(lo) = make_uint4(lp[0], lp[1], lp[2], lp[3]);
 }
 
-// 256-bit read-only load of 8 consecutive, 32-byte aligned floats (sm_100+, PTX 8.8: LDG.E.256)
+// read-only load of 8 consecutive, 32-byte aligned floats (two 128-bit loads)
 __device__ __forceinline__ void ldg256_f32(const float4* p, float (&v)[8]) {
-  asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
-               : "l"(p));
+  const float4 a = __ldg(p), b = __ldg(p + 1);
+  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w;
+  v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
 }
 
 // one thread per (output pixel, 8 channels); source index arithmetic mirrors ATen's upsample_bilinear2d.

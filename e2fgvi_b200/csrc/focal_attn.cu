@@ -12,18 +12,14 @@
 //   Keys are ordered [multiplicity-1 ring keys | pooled keys | multiplicity>=2 ring keys | padding], so only the
 //   last key tile(s) carry a non-zero logit bias and every other tile takes a bias-free fast path.
 //
-// One CTA = one (128-query tile, head, window), TWO CTAs co-resident per SM (98 KB smem, 256 TMEM columns each) so
-// one CTA's hand-off bubbles (barrier round trips, gather latency, prologue / epilogue) are filled by the other —
-// the r01 ablation showed those bubbles were > 50 % of the v1-v3 kernels at one CTA per SM.
-// Warp roles (288 threads):
-//   warps 0-3  softmax: thread r owns query row r (= TMEM lane r): S (64 keys) -> registers, online softmax with lazy
-//              rescale, P packed to fp16 and written BACK INTO THE S TILE'S TMEM COLUMNS (tcgen05.st) — no P tile in
-//              shared memory, no stores / proxy fences on this path; final O / l -> global (un-partitioned layout)
-//   warps 4-7  loaders: per-key source addresses (wrap / pooled / padding) then coalesced 16-byte cp.async gathers of
+// One CTA = one (128-query tile, head, window).
+// Warp roles (384 threads):
+//   warps 0-7  two softmax warpgroups, 64 query rows each: S = Q K^T by wgmma (Q, K K-major in smem) into registers,
+//              online softmax with lazy rescale on the accumulator fragment (a row lives in the 4 threads of a quad),
+//              P packed to fp16 IN REGISTERS as the A operand of O += P V (wgmma, V an MN-major B operand in smem) —
+//              no P tile in shared memory; final O / l -> global (un-partitioned layout)
+//   warps 8-11 loaders: per-key source addresses (wrap / pooled / padding) then coalesced 16-byte cp.async gathers of
 //              K and V rows (256 B each) into swizzled smem, 2-stage ring of 64-key tiles
-//   warp  8    tcgen05 issuer: S = Q K^T (A, B K-major in smem), O += P V with P as the A operand FROM TENSOR MEMORY
-//              and V as an MN-major B operand; issue order S0 S1 PV0 S2 PV1 S3 ... so S(kt+2) may overwrite the
-//              buffer that held P(kt) without any extra barrier (the tensor pipe executes in order)
 // Roofline (SURVEY §8d): 4*B*nW*heads*(T*wh*ww)*(T*(wh*ww+ring+fh*fw))*128 FLOP on the tensor pipe.
 #include <cstdlib>
 #include <type_traits>
@@ -42,13 +38,9 @@ constexpr int QTILE = 2 * QATOM;           // 32 KB
 constexpr int KTILE = 2 * KATOM;           // 16 KB
 constexpr int KV_STAGES = 2;
 constexpr int BIAS_SLOTS = 4;              // logit-bias rows outlive their K stage (the K stage is recycled after S, not PV)
-constexpr int SOFTMAX_WARPS = 4, LOADER_WARPS = 4;
+constexpr int SOFTMAX_WARPS = 8, LOADER_WARPS = 4;
 constexpr int SOFTMAX_THREADS = SOFTMAX_WARPS * 32;
-constexpr int MMA_WARP = SOFTMAX_WARPS + LOADER_WARPS;
-constexpr int THREADS = (MMA_WARP + 1) * 32;   // 288
-constexpr int CTAS_PER_SM = 2;
-constexpr int TMEM_COLS = 256;                 // S0/P0 [0,64) S1/P1 [64,128) O [128,256)
-constexpr uint32_t COL_S = 0, COL_O = 128;
+constexpr int THREADS = (SOFTMAX_WARPS + LOADER_WARPS) * 32;   // 384
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr float RESCALE_THRESHOLD = 8.0f;      // log2 domain: P stays <= 2^8
 constexpr int MAX_RING = 256;                  // expanded-window positions (153 for the 5x9 window)
@@ -63,9 +55,8 @@ struct Smem {
   static constexpr int FTAB = BIAS + BIAS_SLOTS * BN * 4;       // [MAX_FRAME_KEYS] int32: key offset inside its frame
   static constexpr int FBIAS = FTAB + MAX_FRAME_KEYS * 4;       // [MAX_FRAME_KEYS] float: logit bias (log2 multiplicity)
   static constexpr int BARS = FBIAS + MAX_FRAME_KEYS * 4;
-  static constexpr int NUM_BARS = 1 + 4 * KV_STAGES + 2 + 2 + 2;
-  static constexpr int TMEM_SLOT = BARS + NUM_BARS * 8;
-  static constexpr int BYTES = TMEM_SLOT + 16;
+  static constexpr int NUM_BARS = 1 + 4 * KV_STAGES;
+  static constexpr int BYTES = BARS + NUM_BARS * 8;
 };
 constexpr int SMEM_BYTES = Smem::BYTES + 1024;
 
@@ -80,7 +71,7 @@ struct Params {
   int use_pooled;
   float scale_log2;               // scale * log2(e)
 #ifdef E2F_ATTN_DEVTOOLS          // developer builds only (-DE2F_ATTN_DEVTOOLS): never compiled into the shipped library
-  int debug;                      // perf-experiment bits (E2F_ATTN_DEBUG): 1 skip softmax math, 2 skip gathers, 4 skip MMAs
+  int debug;                      // perf-experiment bits (E2F_ATTN_DEBUG): 2 skip gathers
   long long* trace;               // optional [3 roles][64 events] clock64 stamps of CTA (0,0,0) (E2F_ATTN_TRACE)
 #endif
   int n1, n2;                     // expanded-window positions listed once / more than once by the reference
@@ -112,7 +103,6 @@ __host__ __device__ inline int key_multiplicity(int er, int ec, int wh, int ww, 
 }
 
 __device__ __forceinline__ void loader_barrier() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
-__device__ __forceinline__ void softmax_barrier() { asm volatile("bar.sync 2, 256;" ::: "memory"); }
 
 // coalesced gather of ROWS rows x 256 B (two 64-half atoms of ROWS*128 B) into a swizzled tile; 16 lanes cover one
 // row, the 4 loader warps split the rows.
@@ -132,63 +122,12 @@ __device__ __forceinline__ void gather_rows(uint32_t tile_smem, const uint64_t* 
   }
 }
 
-// One 32-logit chunk of a query row: p = exp2(s * scale [+ bias] - m) as 16 packed fp16 pairs + 4 partial row sums.
-// MODE is a compile-time constant so the 32 exps form one branch-free block the scheduler can pipeline
-// (a per-element mode test serialised every 4-element group on the MUFU latency: 3.3k cycles per 64 keys, r01 trace).
-enum { MODE_FAST = 0, MODE_BIASED = 1, MODE_NOEXP = 2 };
-template <int MODE>
-__device__ __forceinline__ void softmax_chunk(const uint32_t (&sv)[32], const float4* __restrict__ bias4, float sc,
-                                              float neg_m, uint32_t (&pk)[16], float& l0, float& l1, float& l2,
-                                              float& l3) {
-  float p[32];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    float a0 = __uint_as_float(sv[4 * i]), a1 = __uint_as_float(sv[4 * i + 1]);
-    float a2 = __uint_as_float(sv[4 * i + 2]), a3 = __uint_as_float(sv[4 * i + 3]);
-    if (MODE == MODE_BIASED) {
-      const float4 bb = bias4[i];
-      a0 = fmaf(a0, sc, bb.x) + neg_m; a1 = fmaf(a1, sc, bb.y) + neg_m;
-      a2 = fmaf(a2, sc, bb.z) + neg_m; a3 = fmaf(a3, sc, bb.w) + neg_m;
-    } else if (MODE == MODE_FAST) {
-      a0 = fmaf(a0, sc, neg_m); a1 = fmaf(a1, sc, neg_m); a2 = fmaf(a2, sc, neg_m); a3 = fmaf(a3, sc, neg_m);
-    }
-    if (MODE == MODE_NOEXP) {
-      p[4 * i] = a0 * 1e-3f; p[4 * i + 1] = a1 * 1e-3f; p[4 * i + 2] = a2 * 1e-3f; p[4 * i + 3] = a3 * 1e-3f;
-    } else {
-      p[4 * i] = fast_exp2(a0); p[4 * i + 1] = fast_exp2(a1); p[4 * i + 2] = fast_exp2(a2); p[4 * i + 3] = fast_exp2(a3);
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    l0 += p[4 * i]; l1 += p[4 * i + 1]; l2 += p[4 * i + 2]; l3 += p[4 * i + 3];
-    pk[2 * i] = pack_half2(p[4 * i], p[4 * i + 1]);
-    pk[2 * i + 1] = pack_half2(p[4 * i + 2], p[4 * i + 3]);
-  }
-}
-
-template <int MODE>
-__device__ __forceinline__ float max_chunk(const uint32_t (&sv)[32], const float4* __restrict__ bias4, float sc) {
-  float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;   // 4 independent chains
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    float a0 = __uint_as_float(sv[4 * i]), a1 = __uint_as_float(sv[4 * i + 1]);
-    float a2 = __uint_as_float(sv[4 * i + 2]), a3 = __uint_as_float(sv[4 * i + 3]);
-    if (MODE == MODE_BIASED) {
-      const float4 bb = bias4[i];
-      a0 = fmaf(a0, sc, bb.x); a1 = fmaf(a1, sc, bb.y); a2 = fmaf(a2, sc, bb.z); a3 = fmaf(a3, sc, bb.w);
-    }
-    m0 = fmaxf(m0, a0); m1 = fmaxf(m1, a1); m2 = fmaxf(m2, a2); m3 = fmaxf(m3, a3);
-  }
-  const float m = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-  return MODE == MODE_BIASED ? m : m * sc;      // scale > 0: max commutes with the scaling
-}
-
 struct SplitBf16 {                // output tag: bf16 (hi, lo) two-term split of the result (operand of e2f_linear_bf16x3)
   __nv_bfloat16 v;
 };
 
 template <typename OutT>
-__global__ void __launch_bounds__(THREADS, CTAS_PER_SM) focal_attn_kernel(const __grid_constant__ Params prm) {
+__global__ void __launch_bounds__(THREADS, 1) focal_attn_kernel(const __grid_constant__ Params prm) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* key_ptr = reinterpret_cast<uint64_t*>(smem + Smem::KEYPTR);
@@ -199,12 +138,8 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) focal_attn_kernel(const 
   uint64_t* q_full = bars;
   uint64_t* k_full = bars + 1;
   uint64_t* v_full = k_full + KV_STAGES;
-  uint64_t* k_empty = v_full + KV_STAGES;       // K stage read by S(kt): free again as soon as that MMA group completes
+  uint64_t* k_empty = v_full + KV_STAGES;       // K stage read by S(kt): free again as soon as that MMA completes
   uint64_t* v_empty = k_empty + KV_STAGES;      // V stage read by PV(kt)
-  uint64_t* s_full = v_empty + KV_STAGES;       // [2] S tile written by the MMA
-  uint64_t* p_full = s_full + 2;                // [2] P written into the S tile's columns by the softmax warps
-  uint64_t* pv_done = p_full + 2;               // [2] PV MMA of that buffer complete (O updated, buffer reusable)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + Smem::TMEM_SLOT);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   // The ablation bits and the clock64 trace of round 1 exist only in developer builds: in the shipped library `dbg` is
@@ -213,7 +148,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) focal_attn_kernel(const 
   const int dbg = prm.debug;
   const bool tracing = prm.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
   int tr_n = 0;
-  auto stamp = [&](int role) {     // role 0 softmax (warp 0 lane 0), 1 loader (warp 4 lane 0), 2 MMA thread
+  auto stamp = [&](int role) {     // role 1: loader (warp 8 lane 0)
     if (tracing && tr_n < 64) prm.trace[role * 64 + tr_n++] = clock64();
   };
 #else
@@ -245,174 +180,165 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) focal_attn_kernel(const 
   const int bias_kt = (NK % BN) ? min(nB / BN, num_kt - 1) : ((prm.n2 > 0) ? nB / BN : num_kt);
   const size_t C3 = 3 * static_cast<size_t>(prm.C);
 
-  if (warp == MMA_WARP) tmem_alloc(tmem_slot, TMEM_COLS);
   if (tid == 0) {
     mbar_init(q_full, LOADER_WARPS);
     for (int s = 0; s < KV_STAGES; ++s) {
       mbar_init(&k_full[s], LOADER_WARPS);
       mbar_init(&v_full[s], LOADER_WARPS);
-      mbar_init(&k_empty[s], 1);
-      mbar_init(&v_empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&s_full[s], 1);
-      mbar_init(&p_full[s], SOFTMAX_WARPS);
-      mbar_init(&pv_done[s], 1);
+      mbar_init(&k_empty[s], SOFTMAX_WARPS);
+      mbar_init(&v_empty[s], SOFTMAX_WARPS);
     }
     fence_barrier_init();
   }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tbase = *tmem_slot;
 
   if (warp < SOFTMAX_WARPS) {
     // =================================================================== softmax + epilogue
-    const int r = tid;                                  // query row in the tile == TMEM lane
-    const uint32_t lane_addr = tbase + (static_cast<uint32_t>(warp * 32) << 16);
-    float m_used = n_masked > 0 ? -100.0f * LOG2E : -INFINITY;
-    float l = static_cast<float>(n_masked);
+    // accumulator fragments (common.cuh): this thread holds rows rw and rw + 8 of its warpgroup's 64 query rows, key /
+    // channel column pairs 8j + 2(lane % 4); the 4 threads of a quad share a row
+    const int wg = warp >> 2, wq = warp & 3, quad = lane & 3;
+    const int rw = wg * 64 + wq * 16 + (lane >> 2);
+    float m_used[2], l[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      m_used[h] = n_masked > 0 ? -100.0f * LOG2E : -INFINITY;
+      l[h] = quad == 0 ? static_cast<float>(n_masked) : 0.f;     // partial row sums, reduced over the quad at the end
+    }
     const float sc = prm.scale_log2;
+    const uint64_t dq0 = gmma_desc_sw128(smem_u32(smem + Smem::Q) + wg * 64 * 128, 16, 1024);
+    const uint64_t dq1 = gmma_desc_adv(dq0, QATOM);
+    const uint64_t dk0 = gmma_desc_sw128(smem_u32(smem + Smem::K), 16, 1024);
+    const uint64_t dv0 = gmma_desc_sw128(smem_u32(smem + Smem::V), KATOM, 1024);
+    float o[HD / 2];
+    mbar_wait(q_full, 0);
 
     for (int kt = 0; kt < num_kt; ++kt) {
-      const int sb = kt & 1, stage = kt % KV_STAGES;
+      const int stage = kt % KV_STAGES;
       const bool biased = kt >= bias_kt;                // uniform over the CTA
-      if (biased) mbar_wait(&k_full[stage], (kt / KV_STAGES) & 1);   // acquire the loaders' bias writes
-      if (tid == 0 && kt < 10) stamp(0);                 // [6kt+0] start of tile
-      mbar_wait(&s_full[sb], (kt >> 1) & 1);
-      if (tid == 0 && kt < 10) stamp(0);                 // [6kt+1] S ready
-      tc_fence_after_sync();
-      // Two passes over the S tile in 32-column chunks (TMEM re-reads are cheap; holding all 64 logits plus the 32
-      // packed outputs in registers does not fit the 96-register budget of 2 CTAs/SM and went to local memory).
-      const uint32_t s_addr = lane_addr + COL_S + sb * BN;
-      const float4* bias4 = reinterpret_cast<const float4*>(key_bias + (kt & (BIAS_SLOTS - 1)) * BN);
-      float mx = -INFINITY;
-      if (dbg & 1) {
-        mx = 0.f;
-      } else {
-#pragma unroll 1
-        for (int c = 0; c < 2; ++c) {
-          uint32_t sv[32];
-          tmem_ld32(s_addr + c * 32, sv);
-          tmem_ld_wait();
-          mx = fmaxf(mx, biased ? max_chunk<MODE_BIASED>(sv, bias4 + c * 8, sc) : max_chunk<MODE_FAST>(sv, bias4, sc));
-        }
-      }
-      if (tid == 0 && kt < 10 && (dbg & 8)) stamp(0);   // (fine trace) max done
-      // lazy rescale: only move the reference max when it grew by more than 2^8
-      float alpha = 1.0f;
-      bool need = false;
-      if (m_used == -INFINITY) {
-        m_used = mx;                       // first tile without masked keys: nothing accumulated yet
-      } else if (mx - m_used > RESCALE_THRESHOLD) {
-        alpha = fast_exp2(m_used - mx);
-        m_used = mx;
-        need = true;
-      }
-      const bool any_need = __any_sync(0xffffffffu, need);
-      if (tid == 0 && kt < 10 && (dbg & 8)) stamp(0);   // (fine trace) rescale decided
-      if (any_need) {
-        l *= alpha;
-        if (kt > 0) {                      // O holds PV(0..kt-1): wait for PV(kt-1), then scale the row in TMEM
-          mbar_wait(&pv_done[(kt - 1) & 1], ((kt - 1) >> 1) & 1);
-          tc_fence_after_sync();
-#pragma unroll 1
-          for (int c = 0; c < 4; ++c) {
-            uint32_t ov[32];
-            tmem_ld32(lane_addr + COL_O + c * 32, ov);
-            tmem_ld_wait();
+      mbar_wait(&k_full[stage], (kt / KV_STAGES) & 1);
+      // ---- S = Q K^T (64 rows x 64 keys per warpgroup)
+      float s[BN / 2];
+      const uint64_t dk = dk0 + ((stage * KTILE) >> 4);
+      wgmma_fence();
 #pragma unroll
-            for (int i = 0; i < 32; ++i) ov[i] = __float_as_uint(__uint_as_float(ov[i]) * alpha);
-            tmem_st32(lane_addr + COL_O + c * 32, ov);
+      for (int k = 0; k < HD / 16; ++k)
+        wgmma_n64_f16(s, (k < 4 ? dq0 : dq1) + 2 * (k & 3), dk + (k < 4 ? 0 : (KATOM >> 4)) + 2 * (k & 3), k != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&k_empty[stage]);      // S(kt) was the only reader of this K stage
+
+      // ---- online softmax, log2 domain
+      const float* kb = key_bias + (kt & (BIAS_SLOTS - 1)) * BN;
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = 8 * j + 2 * quad;
+        const float b0 = biased ? kb[c] : 0.f, b1 = biased ? kb[c + 1] : 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float a0 = s[4 * j + 2 * h], a1 = s[4 * j + 2 * h + 1];
+          if (biased) {
+            a0 = fmaf(a0, sc, b0);
+            a1 = fmaf(a1, sc, b1);
           }
-          tmem_st_wait();
+          mx[h] = fmaxf(mx[h], fmaxf(a0, a1));
         }
       }
-      // P = exp2(s - m) as packed fp16 pairs, written over the first 32 columns of the S tile just consumed: chunk c
-      // (logit columns [32c, 32c+32)) becomes packed columns [16c, 16c+16).  Chunk 1's logits are still intact when
-      // chunk 0's P lands in columns [0,16).  S(kt) complete => PV(kt-2), the previous reader of this buffer, is too.
-      float l0 = 0.f, l1 = 0.f, l2 = 0.f, l3 = 0.f;
-      const float neg_m = -m_used;
-#pragma unroll 1
-      for (int c = 0; c < 2; ++c) {
-        uint32_t sv[32];
-        tmem_ld32(s_addr + c * 32, sv);
-        tmem_ld_wait();
-        uint32_t pk[16];
-        if (dbg & 1) softmax_chunk<MODE_NOEXP>(sv, bias4, sc, neg_m, pk, l0, l1, l2, l3);
-        else if (biased) softmax_chunk<MODE_BIASED>(sv, bias4 + c * 8, sc, neg_m, pk, l0, l1, l2, l3);
-        else softmax_chunk<MODE_FAST>(sv, bias4, sc, neg_m, pk, l0, l1, l2, l3);
-        tmem_st16(s_addr + c * 16, pk);
+      float neg_m[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+        mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+        if (!biased) mx[h] *= sc;                        // scale > 0: max commutes with the scaling
+        // lazy rescale: only move the reference max when it grew by more than 2^8
+        if (m_used[h] == -INFINITY) {
+          m_used[h] = mx[h];                             // first tile without masked keys: nothing accumulated yet
+        } else if (mx[h] - m_used[h] > RESCALE_THRESHOLD) {
+          const float alpha = fast_exp2(m_used[h] - mx[h]);
+          m_used[h] = mx[h];
+          l[h] *= alpha;
+          if (kt > 0) {
+#pragma unroll
+            for (int j = 0; j < HD / 8; ++j) {
+              o[4 * j + 2 * h] *= alpha;
+              o[4 * j + 2 * h + 1] *= alpha;
+            }
+          }
+        }
+        neg_m[h] = -m_used[h];
       }
-      l += (l0 + l1) + (l2 + l3);
-      if (tid == 0 && kt < 10) stamp(0);                 // math done
-      tmem_st_wait();
-      if (tid == 0 && kt < 10) stamp(0);                 // P stored
-      tc_fence_before_sync();
+      // P = exp2(s - m) packed to fp16: pk[j][h] = keys 8j + 2(lane % 4) + {0, 1} of row h, which is exactly the
+      // register A fragment of the next MMA (k step kk takes j = 2kk and 2kk + 1)
+      uint32_t pk[BN / 8][2];
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = 8 * j + 2 * quad;
+        const float b0 = biased ? kb[c] : 0.f, b1 = biased ? kb[c + 1] : 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float a0 = s[4 * j + 2 * h], a1 = s[4 * j + 2 * h + 1];
+          if (biased) {
+            a0 = fmaf(a0, sc, b0) + neg_m[h];
+            a1 = fmaf(a1, sc, b1) + neg_m[h];
+          } else {
+            a0 = fmaf(a0, sc, neg_m[h]);
+            a1 = fmaf(a1, sc, neg_m[h]);
+          }
+          const float p0 = fast_exp2(a0), p1 = fast_exp2(a1);
+          l[h] += p0 + p1;
+          pk[j][h] = pack_half2(p0, p1);
+        }
+      }
+
+      // ---- O += P V
+      mbar_wait(&v_full[stage], (kt / KV_STAGES) & 1);
+      const uint64_t dv = dv0 + ((stage * KTILE) >> 4);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < BN / 16; ++kk) {
+        const uint32_t a[4] = {pk[2 * kk][0], pk[2 * kk][1], pk[2 * kk + 1][0], pk[2 * kk + 1][1]};
+        const uint64_t bdesc = dv + kk * (2048 >> 4);    // 16 keys = two 8-key groups of 1024 B
+        const uint32_t acc = (kt | kk) != 0;
+        wgmma_n64_f16_rs_tb(o, a, bdesc, acc);                        // channels [0, 64)
+        wgmma_n64_f16_rs_tb(o + 32, a, bdesc + (KATOM >> 4), acc);    // channels [64, 128)
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&p_full[sb]);
-      if (tid == 0 && kt < 10) stamp(0);                 // [6kt+5] arrived
+      if (lane == 0) mbar_arrive(&v_empty[stage]);
     }
 
     // ---- epilogue: O / l -> out[b, t, y, x, head*128 ..]
-    mbar_wait(&pv_done[(num_kt - 1) & 1], ((num_kt - 1) >> 1) & 1);
-    tc_fence_after_sync();
-    const int qi = qt * BM + r;
-    const float inv_l = 1.0f / l;
-    OutT* dst = nullptr;
-    size_t dst_off = 0;
-    if (qi < nq) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
+      l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
+      const int qi = qt * BM + rw + 8 * h;
+      if (qi >= nq) continue;
+      const float inv_l = 1.0f / l[h];
       const int t = qi / area, p = qi - t * area;
       const int y = wi * prm.wh + p / prm.ww, x = wj * prm.ww + p % prm.ww;
       const size_t tok = ((static_cast<size_t>(b) * prm.T + t) * prm.H + y) * prm.W + x;
-      dst_off = tok * prm.C + head * HD;
-      dst = static_cast<OutT*>(prm.out) + dst_off;
-    }
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-      uint32_t ov[32];
-      tmem_ld32(lane_addr + COL_O + c * 32, ov);
-      tmem_ld_wait();
-      if (dst) {
+      const size_t dst_off = tok * prm.C + head * HD;
+#pragma unroll
+      for (int j = 0; j < HD / 8; ++j) {
+        const size_t e = dst_off + 8 * j + 2 * quad;
+        const float f0 = o[4 * j + 2 * h] * inv_l, f1 = o[4 * j + 2 * h + 1] * inv_l;
         if constexpr (std::is_same<OutT, SplitBf16>::value) {
-          uint4* dh = reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(prm.out) + dst_off + c * 32);
-          uint4* dl = reinterpret_cast<uint4*>(static_cast<__nv_bfloat16*>(prm.out_lo) + dst_off + c * 32);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            uint32_t hp[4], lp[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float f0 = __uint_as_float(ov[8 * i + 2 * j]) * inv_l, f1 = __uint_as_float(ov[8 * i + 2 * j + 1]) * inv_l;
-              const __nv_bfloat162 hb = __floats2bfloat162_rn(f0, f1);
-              const float2 hf = __bfloat1622float2(hb);
-              const __nv_bfloat162 lb = __floats2bfloat162_rn(f0 - hf.x, f1 - hf.y);
-              hp[j] = *reinterpret_cast<const uint32_t*>(&hb);
-              lp[j] = *reinterpret_cast<const uint32_t*>(&lb);
-            }
-            dh[i] = make_uint4(hp[0], hp[1], hp[2], hp[3]);
-            dl[i] = make_uint4(lp[0], lp[1], lp[2], lp[3]);
-          }
+          const __nv_bfloat162 hb = __floats2bfloat162_rn(f0, f1);
+          const float2 hf = __bfloat1622float2(hb);
+          *reinterpret_cast<__nv_bfloat162*>(static_cast<__nv_bfloat16*>(prm.out) + e) = hb;
+          *reinterpret_cast<__nv_bfloat162*>(static_cast<__nv_bfloat16*>(prm.out_lo) + e) =
+              __floats2bfloat162_rn(f0 - hf.x, f1 - hf.y);
         } else if constexpr (sizeof(OutT) == 4) {
-          float4* d4 = reinterpret_cast<float4*>(dst + c * 32);
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            d4[i] = make_float4(__uint_as_float(ov[4 * i]) * inv_l, __uint_as_float(ov[4 * i + 1]) * inv_l,
-                                __uint_as_float(ov[4 * i + 2]) * inv_l, __uint_as_float(ov[4 * i + 3]) * inv_l);
+          *reinterpret_cast<float2*>(static_cast<float*>(prm.out) + e) = make_float2(f0, f1);
         } else {
-          uint4* d4 = reinterpret_cast<uint4*>(dst + c * 32);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            uint4 u;
-            u.x = pack_half2(__uint_as_float(ov[8 * i]) * inv_l, __uint_as_float(ov[8 * i + 1]) * inv_l);
-            u.y = pack_half2(__uint_as_float(ov[8 * i + 2]) * inv_l, __uint_as_float(ov[8 * i + 3]) * inv_l);
-            u.z = pack_half2(__uint_as_float(ov[8 * i + 4]) * inv_l, __uint_as_float(ov[8 * i + 5]) * inv_l);
-            u.w = pack_half2(__uint_as_float(ov[8 * i + 6]) * inv_l, __uint_as_float(ov[8 * i + 7]) * inv_l);
-            d4[i] = u;
-          }
+          *reinterpret_cast<uint32_t*>(static_cast<__half*>(prm.out) + e) = pack_half2(f0, f1);
         }
       }
     }
-  } else if (warp < MMA_WARP) {
+  } else {
     // =================================================================== loaders
     const int lt = tid - SOFTMAX_THREADS;               // 0..127
     const int lwarp = lt >> 5;
@@ -489,10 +415,9 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) focal_attn_kernel(const 
         }
       }
       if (lt == 0 && kt < 12) stamp(1);                  // [5kt+0] index math done
-      // The K stage is recycled as soon as S(kt-2) has read it (k_empty, committed right behind that MMA group), the V
-      // stage only after PV(kt-2) (v_empty): the gather of K(kt) — the operand the next S waits for — overlaps the
-      // softmax and the PV of the tiles in flight instead of starting after them.  Round 1 recycled both on PV(kt-2),
-      // which exposed one full gather latency per key tile (profiles/r01 attn_trace).
+      // The K stage is recycled as soon as S(kt-2) has read it (k_empty), the V stage only after PV(kt-2) (v_empty): the
+      // gather of K(kt) — the operand the next S waits for — overlaps the softmax and the PV of the tiles in flight
+      // instead of starting after them.
       mbar_wait(&k_empty[stage], ((kt / KV_STAGES) & 1) ^ 1);
       if (lt == 0 && kt < 12) stamp(1);                  // [5kt+1] K stage free
       if (lt < BN) {
@@ -523,69 +448,7 @@ __global__ void __launch_bounds__(THREADS, CTAS_PER_SM) focal_attn_kernel(const 
     fence_proxy_async_smem();
     __syncwarp();
     if (lane == 0) mbar_arrive(&v_full[(num_kt - 1) % KV_STAGES]);
-  } else {
-    // =================================================================== tcgen05 issuer
-    if (elect_one()) {   // one thread, chosen by elect.sync: ptxas then emits bare UTCHMMA (no per-instruction ELECT loop)
-      const uint32_t idesc_s = umma_idesc_f16(BM, BN, 0, 0);   // S = Q K^T, both K-major (d contiguous)
-      const uint32_t idesc_o = umma_idesc_f16(BM, HD, 0, 1);   // O = P V: P from TMEM, V MN-major (d contiguous per key)
-      const uint32_t sQ = smem_u32(smem + Smem::Q), sK = smem_u32(smem + Smem::K);
-      const uint32_t sV = smem_u32(smem + Smem::V);
-      const bool run_mma = !(dbg & 4);
-      // descriptors hoisted out of the issue loops (one 64-bit add per K step instead of ~40 integer instructions)
-      const uint64_t dq0 = umma_desc_sw128(sQ, 16, 1024), dq1 = umma_desc_adv(dq0, QATOM);
-      const uint64_t dk0 = umma_desc_sw128(sK, 16, 1024);
-      const uint64_t dv0 = umma_desc_sw128(sV, KATOM, 1024);
-      auto issue_s = [&](int kt) {
-        const int stage = kt % KV_STAGES, sb = kt & 1;
-        mbar_wait(&k_full[stage], (kt / KV_STAGES) & 1);
-        tc_fence_after_sync();
-        const uint64_t dk = dk0 + ((stage * KTILE) >> 4);
-        if (run_mma || kt < 2) {
-#pragma unroll
-          for (int k = 0; k < HD / 16; ++k)
-            umma_f16(tbase + COL_S + sb * BN, (k < 4 ? dq0 : dq1) + 2 * (k & 3),
-                     dk + (k < 4 ? 0 : (KATOM >> 4)) + 2 * (k & 3), idesc_s, k != 0);
-        }
-        umma_commit(&s_full[sb]);
-        umma_commit(&k_empty[stage]);                    // S(kt) was the only reader of this K stage
-      };
-      mbar_wait(q_full, 0);
-      issue_s(0);
-      if (num_kt > 1) issue_s(1);
-      for (int kt = 0; kt < num_kt; ++kt) {
-        const int stage = kt % KV_STAGES, sb = kt & 1;
-        if (kt < 15) stamp(2);                           // [4kt+0] waiting for P
-        mbar_wait(&p_full[sb], (kt >> 1) & 1);
-        if (kt < 15) stamp(2);                           // [4kt+1] P ready
-        mbar_wait(&v_full[stage], (kt / KV_STAGES) & 1);
-        tc_fence_after_sync();
-        const uint64_t dv = dv0 + ((stage * KTILE) >> 4);
-        const uint32_t p_tmem = tbase + COL_S + sb * BN;       // packed fp16 P: 8 columns per 16 keys
-#pragma unroll
-        for (int k = 0; k < BN / 16; ++k) {
-          if (run_mma || kt < 2) {
-            const uint64_t bdesc = dv + k * (2048 >> 4);
-            const uint32_t acc = (kt | k) != 0;
-            asm volatile(
-                "{\n"
-                ".reg .pred p;\n"
-                "setp.ne.b32 p, %4, 0;\n"
-                "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-                "}\n" ::"r"(tbase + COL_O), "r"(p_tmem + k * 8), "l"(bdesc), "r"(idesc_o), "r"(acc)
-                : "memory");
-          }
-        }
-        umma_commit(&v_empty[stage]);
-        umma_commit(&pv_done[sb]);
-        if (kt < 15) stamp(2);                           // [4kt+2] PV issued
-        if (kt + 2 < num_kt) issue_s(kt + 2);           // tensor pipe order: ... PV(kt), S(kt+2), PV(kt+1), ...
-        if (kt < 15) stamp(2);                           // [4kt+3] S(kt+2) issued
-      }
-    }
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == MMA_WARP) tmem_dealloc(tbase, TMEM_COLS);
 }
 
 }  // namespace attn

@@ -1,17 +1,16 @@
 // Linear layers of the transformer path (nn.Linear at tfocal_transformer.py:44 ss.embedding, :68 sc.embedding,
-// :221 attn.qkv, :398 attn.proj, :89/:97 mlp.conv1/conv2) as ONE persistent tcgen05 GEMM with fp32-level accuracy:
+// :221 attn.qkv, :398 attn.proj, :89/:97 mlp.conv1/conv2) as ONE persistent wgmma GEMM with fp32-level accuracy:
 //     out[M,N] = A[M,K] . W[N,K]^T + bias[N] (+ residual[M,N])
 // fp32 operands are split into two bf16 terms (x = hi + lo, |lo| <= 2^-9 |x|) and the product is evaluated as
 //     Ah.Wh + Ah.Wl + Al.Wh      (the dropped Al.Wl term is ~2^-18 relative)
-// on the bf16 tensor pipe with fp32 accumulation in TMEM — bf16 keeps the full fp32 exponent range, so no scaling
-// is needed.  Relative error per output ~2^-17, versus 2^-11 for TF32; the SIMT fp32 cuBLAS path it replaces
-// runs at ~60 TFLOP/s.
+// on the bf16 tensor pipe with fp32 accumulation — bf16 keeps the full fp32 exponent range, so no scaling is needed.
+// Relative error per output ~2^-17, versus 2^-11 for TF32.
 //
-// Structure (canonical Blackwell GEMM): persistent CTAs over a static tile schedule (n fastest, so concurrently
-// running CTAs share A row-panels in L2); warp 0 = TMA producer (4 tensor maps: Ah, Al, Wh, Wl, SWIZZLE_128B,
-// K tail / row tails zero-filled by TMA), warp 1 = MMA issuer (12 tcgen05.mma per 64-wide K block), warps 2-5 =
-// epilogue (tcgen05.ld -> +bias (+residual) -> fp32/fp16 global store) on a double-buffered TMEM accumulator, so
-// tile i's epilogue overlaps tile i+1's main loop.  smem ring: STAGES x (Ah 16K + Al 16K + Wh + Wl).
+// Structure (Hopper warp-specialised GEMM): persistent CTAs over a static tile schedule (n fastest, so concurrently
+// running CTAs share A row-panels in L2); warp 8 = TMA producer (4 tensor maps: Ah, Al, Wh, Wl, SWIZZLE_128B, K tail /
+// row tails zero-filled by TMA); warps 0-7 = two consumer warpgroups, each owning 64 rows of the 128-row tile: 12
+// wgmma per 64-wide K block with the accumulator in registers, one K block in flight while the previous stage is
+// released, then +bias (+residual) -> fp32/fp16 global store straight from the accumulator fragment.
 // Roofline: tensor-bound, 3 x 2*M*N*K bf16 FLOP of tensor work per 2*M*N*K algorithmic fp32 FLOP.
 #include <cuda.h>
 #include <cstdlib>
@@ -24,31 +23,18 @@ namespace gemm {
 
 constexpr int BM = 128, BK = 64;
 constexpr int A_TILE = BM * BK * 2;                // 16 KB (one bf16 term)
-constexpr int EPI_WARPS = 8;                       // two warps per TMEM lane quadrant, each owning half of the tile's columns
-constexpr int THREADS = (2 + EPI_WARPS) * 32;      // 320
-constexpr int EPI_STAGE = 2048;                    // per epilogue warp: 32 rows x 64 bytes transposition buffer
+constexpr int CONSUMER_WARPS = 8;                  // two warpgroups x 64 accumulator rows
+constexpr int THREADS = (CONSUMER_WARPS + 1) * 32; // + the TMA warp
 
 template <int BN>
 struct Cfg {
   static constexpr int W_TILE = BN * BK * 2;
   static constexpr int STAGE = 2 * A_TILE + 2 * W_TILE;
   static constexpr int STAGES = (BN == 128) ? 3 : 2;
-  static constexpr int TMEM_COLS = 2 * BN;          // double-buffered accumulator (256 or 512 columns)
-  // + per-tile bias slice (double-buffered) + the epilogue warps' store/load transposition buffers
-  static constexpr int SMEM = STAGES * STAGE + 256 + 2 * BN * 4 + EPI_WARPS * EPI_STAGE + 1024;
+  static constexpr int SMEM = STAGES * STAGE + 256 + 1024;
 };
 
-// kind::f16 instruction descriptor with BF16 operands (a_format = b_format = 1), fp32 accumulate, K-major A and B
-__host__ __device__ constexpr uint32_t idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
-}
-
-// CL = 2: thread-block clusters of two CTAs that work on two M tiles of the same N tile in lockstep.  Each CTA
-// fetches HALF of the W tile and multicasts it to both (W is the larger operand: 64 of the 96 KB per K chunk at
-// BN = 256), which cuts the L2 -> SM traffic that bounds the short-K GEMMs by a third.  A stage is released to the
-// producers of BOTH CTAs by a multicast tcgen05.commit; everything else (MMA, TMEM, epilogue) stays CTA-local.
-template <int BN, typename OutT, int CL>
+template <int BN, typename OutT>
 __global__ void __launch_bounds__(THREADS, 1)
 linear_kernel(const __grid_constant__ CUtensorMap tm_ah, const __grid_constant__ CUtensorMap tm_al,
               const __grid_constant__ CUtensorMap tm_wh, const __grid_constant__ CUtensorMap tm_wl,
@@ -59,31 +45,16 @@ linear_kernel(const __grid_constant__ CUtensorMap tm_ah, const __grid_constant__
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE);
   uint64_t* empty = full + C::STAGES;
-  uint64_t* acc_full = empty + C::STAGES;     // [2]
-  uint64_t* acc_empty = acc_full + 2;         // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* sbias = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE + 256);   // [2][BN]
-  uint8_t* epi_stage = smem + C::STAGES * C::STAGE + 256 + 2 * BN * 4;           // [EPI_WARPS][EPI_STAGE]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int tiles_m = (M + BM - 1) / BM, tiles_n = (N + BN - 1) / BN;
   const int num_kb = (K + BK - 1) / BK;
-  // work item = (N tile, group of CL consecutive M tiles); a cluster walks the items, CTA `rank` takes M tile `rank`
-  // of the group (a tile past the end computes on zero-filled rows and stores nothing)
-  const int rank = CL > 1 ? static_cast<int>(cluster_ctarank()) : 0;
-  const int first_item = blockIdx.x / CL, item_step = gridDim.x / CL;
-  const int num_items = ((tiles_m + CL - 1) / CL) * tiles_n;
-  constexpr uint16_t MC_MASK = (1u << CL) - 1;
+  const int num_items = tiles_m * tiles_n;
 
-  if (warp == 1) tmem_alloc(tmem_slot, C::TMEM_COLS);
   if (tid == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], CL);                    // released by the MMA warps of all CTAs that receive the multicast
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&acc_full[s], 1);
-      mbar_init(&acc_empty[s], EPI_WARPS);
+      mbar_init(&empty[s], CONSUMER_WARPS);
     }
     fence_barrier_init();
     tma_prefetch_desc(&tm_ah);
@@ -91,18 +62,14 @@ linear_kernel(const __grid_constant__ CUtensorMap tm_ah, const __grid_constant__
     tma_prefetch_desc(&tm_wh);
     tma_prefetch_desc(&tm_wl);
   }
-  tc_fence_before_sync();
-  if (CL > 1) cluster_sync_all();                  // barriers of every CTA initialised before any remote arrive / copy
-  else __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tbase = *tmem_slot;
+  __syncthreads();
 
-  if (warp == 0) {
+  if (warp == CONSUMER_WARPS) {
     // ------------------------------------------------------------------ TMA producer
-    if (elect_one()) {   // one thread, chosen by elect.sync: ptxas then emits bare UTCHMMA / UTMALDG (no per-instruction ELECT loop)
+    if (elect_one()) {
       uint32_t it = 0;
-      for (int item = first_item; item < num_items; item += item_step) {
-        const int m0 = ((item / tiles_n) * CL + rank) * BM, n0 = (item % tiles_n) * BN;
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+        const int m0 = (item / tiles_n) * BM, n0 = (item % tiles_n) * BN;
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
           const int stage = it % C::STAGES;
           mbar_wait(&empty[stage], ((it / C::STAGES) & 1) ^ 1);
@@ -110,211 +77,82 @@ linear_kernel(const __grid_constant__ CUtensorMap tm_ah, const __grid_constant__
           const uint32_t s0 = smem_u32(smem + stage * C::STAGE);
           tma_load_2d(s0, &tm_ah, &full[stage], kb * BK, m0);
           tma_load_2d(s0 + A_TILE, &tm_al, &full[stage], kb * BK, m0);
-          if (CL > 1) {
-            // rows [rank*BN/CL, +BN/CL) of the W tile (the maps' box is BN/CL rows), broadcast to the whole cluster
-            const uint32_t part = rank * (C::W_TILE / CL);
-            tma_load_2d_mc(s0 + 2 * A_TILE + part, &tm_wh, &full[stage], kb * BK, n0 + rank * (BN / CL), MC_MASK);
-            tma_load_2d_mc(s0 + 2 * A_TILE + C::W_TILE + part, &tm_wl, &full[stage], kb * BK, n0 + rank * (BN / CL),
-                           MC_MASK);
-          } else {
-            tma_load_2d(s0 + 2 * A_TILE, &tm_wh, &full[stage], kb * BK, n0);
-            tma_load_2d(s0 + 2 * A_TILE + C::W_TILE, &tm_wl, &full[stage], kb * BK, n0);
-          }
+          tma_load_2d(s0 + 2 * A_TILE, &tm_wh, &full[stage], kb * BK, n0);
+          tma_load_2d(s0 + 2 * A_TILE + C::W_TILE, &tm_wl, &full[stage], kb * BK, n0);
         }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (elect_one()) {   // one thread, chosen by elect.sync: ptxas then emits bare UTCHMMA / UTMALDG (no per-instruction ELECT loop)
-      const uint32_t idesc = idesc_bf16(BM, BN);
-      // stage-0 descriptors; stage s / K step k are reached with one 64-bit add each
-      const uint64_t d_ah0 = umma_desc_sw128(smem_u32(smem), 16, 1024);
-      const uint64_t d_al0 = umma_desc_adv(d_ah0, A_TILE), d_wh0 = umma_desc_adv(d_ah0, 2 * A_TILE);
-      const uint64_t d_wl0 = umma_desc_adv(d_wh0, C::W_TILE);
-      uint32_t it = 0, local = 0;
-      for (int item = first_item; item < num_items; item += item_step, ++local) {
-        const int buf = local & 1;
-        mbar_wait(&acc_empty[buf], ((local >> 1) & 1) ^ 1);
-        tc_fence_after_sync();
-        const uint32_t d = tbase + buf * BN;
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int stage = it % C::STAGES;
-          mbar_wait(&full[stage], (it / C::STAGES) & 1);
-          tc_fence_after_sync();
-          const uint32_t soff = (stage * C::STAGE) >> 4;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t dah = d_ah0 + soff + 2 * k, dal = d_al0 + soff + 2 * k;
-            const uint64_t dwh = d_wh0 + soff + 2 * k, dwl = d_wl0 + soff + 2 * k;
-            umma_f16(d, dal, dwh, idesc, (kb | k) != 0);   // small terms first
-            umma_f16(d, dah, dwl, idesc, 1);
-            umma_f16(d, dah, dwh, idesc, 1);
-          }
-          if (CL > 1) umma_commit_mc(&empty[stage], MC_MASK);
-          else umma_commit(&empty[stage]);
-        }
-        umma_commit(&acc_full[buf]);
       }
     }
   } else {
-    // ------------------------------------------------------------------ epilogue
-    // 8 warps: TMEM lane quadrant q = warp % 4 (hardware rule), column half = (warp - 2) / 4.  Per tile the bias slice
-    // goes to shared memory once; the residual of chunk c+1 is fetched while chunk c is converted and stored, and the
-    // first chunk's residual is requested BEFORE waiting for the accumulator, so its latency hides behind the main
-    // loop (short-K GEMMs such as attn.proj used to be bound by these serialised loads).
-    const int q = warp & 3, half = (warp - 2) >> 2;
-    const int et = tid - 64;                                  // 0..255 among the epilogue threads
-    constexpr int CH = BN / 64;                               // 32-column chunks per warp
-    // Global accesses are TRANSPOSED through a per-warp 32-row x 64-byte buffer (same scheme as conv.cu, XOR-swizzled,
-    // conflict-free): with thread = row, a direct 16-byte access per thread touches 32 different 128-byte lines per
-    // instruction (rows are N*4 bytes apart) and the LSU, not the tensor pipe, bounded every short-K GEMM
-    // (attn.proj K=512: 20 us per tile against a 6.5 us main loop, profiles/r02).  Transposed, 4 consecutive lanes
-    // move one row's 64 contiguous bytes: 8 lines per instruction, for the stores AND the residual loads.
-    const uint32_t stg = smem_u32(epi_stage + (warp - 2) * EPI_STAGE);
-    const uint32_t wsw = (lane >> 1) & 3;
-    const int sub = lane & 3, prow = lane >> 2;
-    auto st_own = [&](int cc, uint32_t a, uint32_t b, uint32_t c2, uint32_t d) {       // own row, logical chunk cc
-      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(stg + lane * 64 + ((cc ^ wsw) << 4)), "r"(a), "r"(b), "r"(c2), "r"(d)
-                   : "memory");
-    };
-    auto ld_own = [&](int cc) {
-      uint4 u;
-      asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(u.x), "=r"(u.y), "=r"(u.z), "=r"(u.w)
-                   : "r"(stg + lane * 64 + ((cc ^ wsw) << 4)) : "memory");
-      return u;
-    };
-    auto st_row = [&](int rr, uint4 u) {                                                 // row rr, logical chunk `sub`
-      asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(stg + rr * 64 + ((sub ^ ((rr >> 1) & 3)) << 4)), "r"(u.x), "r"(u.y), "r"(u.z), "r"(u.w)
-                   : "memory");
-    };
-    auto ld_row = [&](int rr) {
-      uint4 u;
-      asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(u.x), "=r"(u.y), "=r"(u.z), "=r"(u.w)
-                   : "r"(stg + rr * 64 + ((sub ^ ((rr >> 1) & 3)) << 4)) : "memory");
-      return u;
-    };
-    const bool vec_ok = (N & 3) == 0;                         // rows start on 16-byte boundaries
-    uint32_t local = 0;
-    for (int item = first_item; item < num_items; item += item_step, ++local) {
-      const int buf = local & 1;
-      const int m0 = ((item / tiles_n) * CL + rank) * BM, n0 = (item % tiles_n) * BN;
-      const int rbase = m0 + q * 32;                          // first row of this warp's TMEM lane quarter
-      const int row = rbase + lane;
-      float* sb = sbias + buf * BN;
-      if (et < BN) sb[et] = (bias && n0 + et < N) ? __ldg(bias + n0 + et) : 0.f;
-      const bool row_ok = row < M;
-      const size_t orow = static_cast<size_t>(row) * N;
-      // residual of one 32-column chunk as eight coalesced 16-byte loads per lane (4 lanes = one row's 64 bytes); the
-      // loads of chunk c+1 are issued before chunk c is stored, and chunk 0's before the accumulator is awaited, so
-      // their latency hides behind the main loop / the previous chunk's stores
-      uint4 ru[2][4], rn[2][4];
-      auto fetch = [&](int c, uint4 (&r)[2][4]) {
-        const int col0 = n0 + (half * CH + c) * 32;
-        const bool on = residual && vec_ok && c < CH && col0 + 32 <= N;
+    // ------------------------------------------------------------------ consumers: wgmma main loop + epilogue
+    const int wg = warp >> 2, wq = warp & 3;
+    // stage-0 descriptors (this warpgroup's 64 A rows start 64 * 128 B into the A tiles); stage s / K step k are
+    // reached with one 64-bit add each
+    const uint64_t d_ah0 = gmma_desc_sw128(smem_u32(smem) + wg * 64 * 128, 16, 1024);
+    const uint64_t d_al0 = gmma_desc_adv(d_ah0, A_TILE);
+    const uint64_t d_wh0 = gmma_desc_sw128(smem_u32(smem) + 2 * A_TILE, 16, 1024);
+    const uint64_t d_wl0 = gmma_desc_adv(d_wh0, C::W_TILE);
+    const bool vec_ok = (N & 1) == 0;                         // rows start on 8-byte boundaries
+    float acc[BN / 2];
+    uint32_t it = 0;
+    for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+      const int m0 = (item / tiles_n) * BM, n0 = (item % tiles_n) * BN;
+      for (int kb = 0; kb < num_kb; ++kb, ++it) {
+        const int stage = it % C::STAGES;
+        mbar_wait(&full[stage], (it / C::STAGES) & 1);
+        const uint32_t soff = (stage * C::STAGE) >> 4;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint64_t dah = d_ah0 + soff + 2 * k, dal = d_al0 + soff + 2 * k;
+          const uint64_t dwh = d_wh0 + soff + 2 * k, dwl = d_wl0 + soff + 2 * k;
+          wgmma_ss<BN, false>(acc, dal, dwh, (kb | k) != 0);   // small terms first
+          wgmma_ss<BN, false>(acc, dah, dwl, 1);
+          wgmma_ss<BN, false>(acc, dah, dwh, 1);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                                      // the previous K block's MMAs are done: release its stage
+        if (kb > 0 && lane == 0) mbar_arrive(&empty[(it - 1) % C::STAGES]);
+      }
+      wgmma_wait<0>();
+      if (num_kb > 0 && lane == 0) mbar_arrive(&empty[(it - 1) % C::STAGES]);
+      // fragment: rows r0 and r0 + 8, column pairs 8j + 2(lane % 4)
+      const int r0 = m0 + wg * 64 + wq * 16 + (lane >> 2);
+      const int cb = n0 + 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = cb + 8 * j;
+        if (col >= N) continue;
+        const bool pair = vec_ok && col + 1 < N;
+        const float b0 = bias ? __ldg(bias + col) : 0.f;
+        const float b1 = (bias && col + 1 < N) ? __ldg(bias + col + 1) : 0.f;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int R = rbase + j * 8 + prow;
-            r[h][j] = make_uint4(0u, 0u, 0u, 0u);
-            if (on && R < M) r[h][j] = __ldg(reinterpret_cast<const uint4*>(residual + static_cast<size_t>(R) * N + col0 + h * 16 + sub * 4));
-          }
-        }
-      };
-      fetch(0, ru);
-      asm volatile("bar.sync 1, 256;" ::: "memory");           // bias slice visible to all epilogue warps
-      mbar_wait(&acc_full[buf], (local >> 1) & 1);
-      tc_fence_after_sync();
-      const uint32_t taddr = tbase + (static_cast<uint32_t>(q * 32) << 16) + buf * BN + half * (BN / 2);
-#pragma unroll 1
-      for (int c = 0; c < CH; ++c) {
-        uint32_t v[32];
-        tmem_ld32(taddr + c * 32, v);
-        fetch(c + 1, rn);
-        tmem_ld_wait();
-        const int cl = (half * CH + c) * 32;                  // column offset inside the tile
-        const int col0 = n0 + cl;
-        if (col0 < N && vec_ok && col0 + 32 <= N) {
-          float f[32];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 b4 = *reinterpret_cast<const float4*>(sb + cl + 4 * i);
-            f[4 * i] = __uint_as_float(v[4 * i]) + b4.x;
-            f[4 * i + 1] = __uint_as_float(v[4 * i + 1]) + b4.y;
-            f[4 * i + 2] = __uint_as_float(v[4 * i + 2]) + b4.z;
-            f[4 * i + 3] = __uint_as_float(v[4 * i + 3]) + b4.w;
-          }
-          if (residual) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-#pragma unroll
-              for (int j = 0; j < 4; ++j) st_row(j * 8 + prow, ru[h][j]);
-              __syncwarp();
-#pragma unroll
-              for (int cc = 0; cc < 4; ++cc) {
-                const uint4 u = ld_own(cc);
-                f[h * 16 + cc * 4] += __uint_as_float(u.x);     f[h * 16 + cc * 4 + 1] += __uint_as_float(u.y);
-                f[h * 16 + cc * 4 + 2] += __uint_as_float(u.z); f[h * 16 + cc * 4 + 3] += __uint_as_float(u.w);
-              }
-              __syncwarp();
+          const int R = r0 + 8 * h;
+          if (R >= M) continue;
+          const size_t o = static_cast<size_t>(R) * N + col;
+          float v0 = acc[4 * j + 2 * h] + b0, v1 = acc[4 * j + 2 * h + 1] + b1;
+          if (pair) {
+            if (residual) {
+              const float2 r2 = __ldg(reinterpret_cast<const float2*>(residual + o));
+              v0 += r2.x;
+              v1 += r2.y;
+            }
+            if constexpr (sizeof(OutT) == 4) *reinterpret_cast<float2*>(out + o) = make_float2(v0, v1);
+            else *reinterpret_cast<uint32_t*>(out + o) = pack_half2(v0, v1);
+          } else {
+            if (residual) v0 += __ldg(residual + o);
+            if constexpr (sizeof(OutT) == 4) out[o] = v0;
+            else out[o] = __float2half_rn(v0);
+            if (col + 1 < N) {
+              if (residual) v1 += __ldg(residual + o + 1);
+              if constexpr (sizeof(OutT) == 4) out[o + 1] = v1;
+              else out[o + 1] = __float2half_rn(v1);
             }
           }
-          if constexpr (sizeof(OutT) == 4) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-#pragma unroll
-              for (int cc = 0; cc < 4; ++cc)
-                st_own(cc, __float_as_uint(f[h * 16 + cc * 4]), __float_as_uint(f[h * 16 + cc * 4 + 1]),
-                       __float_as_uint(f[h * 16 + cc * 4 + 2]), __float_as_uint(f[h * 16 + cc * 4 + 3]));
-              __syncwarp();
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const int rr = j * 8 + prow, R = rbase + rr;
-                const uint4 u = ld_row(rr);
-                if (R < M) *reinterpret_cast<uint4*>(out + static_cast<size_t>(R) * N + col0 + h * 16 + sub * 4) = u;
-              }
-              __syncwarp();
-            }
-          } else {                                            // fp16: 32 columns = 64 bytes per row, one pass
-#pragma unroll
-            for (int cc = 0; cc < 4; ++cc)
-              st_own(cc, pack_half2(f[cc * 8], f[cc * 8 + 1]), pack_half2(f[cc * 8 + 2], f[cc * 8 + 3]),
-                     pack_half2(f[cc * 8 + 4], f[cc * 8 + 5]), pack_half2(f[cc * 8 + 6], f[cc * 8 + 7]));
-            __syncwarp();
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const int rr = j * 8 + prow, R = rbase + rr;
-              const uint4 u = ld_row(rr);
-              if (R < M) *reinterpret_cast<uint4*>(out + static_cast<size_t>(R) * N + col0 + sub * 8) = u;
-            }
-            __syncwarp();
-          }
-        } else if (row_ok) {
-          const size_t o = orow + col0;
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {     // static indexing keeps v[] in registers
-            if (col0 + i < N) {
-              const float val = __uint_as_float(v[i]) + sb[cl + i] + (residual ? __ldg(residual + o + i) : 0.f);
-              if constexpr (sizeof(OutT) == 4) out[o + i] = val;
-              else out[o + i] = __float2half_rn(val);
-            }
-          }
-        }
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) ru[h][j] = rn[h][j];
         }
       }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
     }
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tbase, C::TMEM_COLS);
-  if (CL > 1) cluster_sync_all();                  // no CTA leaves while a peer may still multicast into it
 }
 
 // x = hi + lo with hi = bf16(x), lo = bf16(x - hi); 8 elements per thread
@@ -369,64 +207,26 @@ static int make_map(CUtensorMap* tm, const void* base, int rows, int k, int box_
   return 0;
 }
 
-template <int BN, typename OutT, int CL>
+template <int BN, typename OutT>
 static int launch_variant(const void* ah, const void* al, const void* wh, const void* wl, const float* bias,
                           const float* residual, void* out, int m, int n, int k, cudaStream_t stream) {
   CUtensorMap tah, tal, twh, twl;
   int st;
   if ((st = make_map(&tah, ah, m, k, BM))) return st;
   if ((st = make_map(&tal, al, m, k, BM))) return st;
-  if ((st = make_map(&twh, wh, n, k, BN / CL))) return st;
-  if ((st = make_map(&twl, wl, n, k, BN / CL))) return st;
-  auto kern = linear_kernel<BN, OutT, CL>;
-  // co-resident CTAs (1 per SM; for clusters: CL * active clusters), per device ordinal (0 = not configured yet)
-  static std::atomic<int> max_ctas_dev[64];
+  if ((st = make_map(&twh, wh, n, k, BN))) return st;
+  if ((st = make_map(&twl, wl, n, k, BN))) return st;
+  auto kern = linear_kernel<BN, OutT>;
+  static DeviceOnce cfg;
   const int dev = current_device();
-  int max_ctas = (dev >= 0 && dev < 64) ? max_ctas_dev[dev].load(std::memory_order_acquire) : 0;
-  if (!max_ctas) {
+  if (!device_done(cfg, dev)) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM);
     if (e != cudaSuccess) return static_cast<int>(e);
-    max_ctas = num_sms();
-    if (CL > 1) {
-      cudaLaunchConfig_t qc = {};
-      qc.gridDim = dim3(num_sms() / CL * CL);
-      qc.blockDim = dim3(THREADS);
-      qc.dynamicSmemBytes = Cfg<BN>::SMEM;
-      cudaLaunchAttribute qa[1];
-      qa[0].id = cudaLaunchAttributeClusterDimension;
-      qa[0].val.clusterDim.x = CL;
-      qa[0].val.clusterDim.y = 1;
-      qa[0].val.clusterDim.z = 1;
-      qc.attrs = qa;
-      qc.numAttrs = 1;
-      int clusters = 0;
-      e = cudaOccupancyMaxActiveClusters(&clusters, kern, &qc);
-      if (e != cudaSuccess || clusters < 1) {
-        max_ctas = 0;
-        set_error("linear: cudaOccupancyMaxActiveClusters failed (%s)", cudaGetErrorString(e));
-        return -4;
-      }
-      max_ctas = clusters * CL;
-    }
-    if (dev >= 0 && dev < 64) max_ctas_dev[dev].store(max_ctas, std::memory_order_release);
+    device_mark(cfg, dev);
   }
-  const int tiles_m = (m + BM - 1) / BM, tiles_n = (n + BN - 1) / BN;
-  const int items = ((tiles_m + CL - 1) / CL) * tiles_n;
-  const int grid = (items * CL < max_ctas) ? items * CL : max_ctas;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(THREADS);
-  cfg.dynamicSmemBytes = Cfg<BN>::SMEM;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CL;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  cudaError_t le = cudaLaunchKernelEx(&cfg, kern, tah, tal, twh, twl, bias, residual, static_cast<OutT*>(out), m, n, k);
-  if (le != cudaSuccess) return static_cast<int>(le);
+  const int items = ((m + BM - 1) / BM) * ((n + BN - 1) / BN);
+  const int grid = items < num_sms() ? items : num_sms();     // persistent: one CTA per SM
+  kern<<<grid, THREADS, Cfg<BN>::SMEM, stream>>>(tah, tal, twh, twl, bias, residual, static_cast<OutT*>(out), m, n, k);
   count_launch();
   return static_cast<int>(cudaGetLastError());
 }
@@ -448,18 +248,11 @@ int launch_linear_bf16x3(const void* a_hi, const void* a_lo, const void* w_hi, c
                          cudaStream_t stream) {
   using namespace gemm;
   if (m == 0 || n == 0) return 0;
-  // clusters of 2 (W multicast) unless there is a single M tile or E2F_LINEAR_CLUSTER=1 asks for the plain kernel
-  static const bool no_cluster = [] {
-    const char* e = getenv("E2F_LINEAR_CLUSTER");
-    return e && e[0] == '1';
-  }();
-  const bool cl2 = !no_cluster && m > BM;
-#define E2F_LINEAR_GO(BNV, T)                                                                                       \
-  (cl2 ? launch_variant<BNV, T, 2>(a_hi, a_lo, w_hi, w_lo, bias, residual, out, m, n, k, stream)                    \
-       : launch_variant<BNV, T, 1>(a_hi, a_lo, w_hi, w_lo, bias, residual, out, m, n, k, stream))
-  if (block_n == 256) return out_dtype == 1 ? E2F_LINEAR_GO(256, __half) : E2F_LINEAR_GO(256, float);
-  return out_dtype == 1 ? E2F_LINEAR_GO(128, __half) : E2F_LINEAR_GO(128, float);
-#undef E2F_LINEAR_GO
+  if (block_n == 256)
+    return out_dtype == 1 ? launch_variant<256, __half>(a_hi, a_lo, w_hi, w_lo, bias, residual, out, m, n, k, stream)
+                          : launch_variant<256, float>(a_hi, a_lo, w_hi, w_lo, bias, residual, out, m, n, k, stream);
+  return out_dtype == 1 ? launch_variant<128, __half>(a_hi, a_lo, w_hi, w_lo, bias, residual, out, m, n, k, stream)
+                        : launch_variant<128, float>(a_hi, a_lo, w_hi, w_lo, bias, residual, out, m, n, k, stream);
 }
 
 }  // namespace e2f

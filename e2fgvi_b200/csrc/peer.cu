@@ -1,13 +1,11 @@
-// Output stitch over NVLink / NVSwitch PEER MEMORY (SURVEY §8(e): clips shard across ranks, the only exchange is the
+// Output stitch over NVLink / NVSwitch PEER MEMORY (clips shard across ranks, the only exchange is the
 // all-gather of the output frames).  Every rank owns a landing buffer allocated here, exports it with a CUDA IPC handle,
 // and PUSHES its block of frames into every peer's landing buffer with DMA copies on a side stream — copy engines, no SMs.
 // Why not NCCL for the payload: an NCCL kernel holds SMs for as long as it runs (and spins on them while it waits for
 // the slowest rank), and the kernels of the next forward are persistent, one CTA per SM with static tile striding — a CTA
 // that cannot be placed starts only when another one exits.  The ordering flags are therefore 32-bit words in the same
 // peer memory, written and awaited by STREAM MEMORY OPERATIONS (cuStreamWriteValue32 / cuStreamWaitValue32: executed by
-// the GPU front end, no kernel).  Measured on 4 x B200 (profiles/r02/run22_*): at 80 MB per rank and step both this path
-// and the NCCL all-gather cost ~0 ms of a 35 ms step — scaling is set by the slowest board — so this is about not
-// depending on spare SMs, not about a measured win at this payload.  NCCL / torch.distributed stay for the plumbing
+// the GPU front end, no kernel), so the exchange does not depend on spare SMs.  NCCL / torch.distributed stay for the plumbing
 // (process group, exchange of the IPC handles).  Host side: e2fgvi_b200/clips.py (PeerStitcher).
 #include <cuda.h>
 #include <cuda_runtime.h>

@@ -484,7 +484,7 @@ int launch_t2t_unfold(const float* img, float* tok, void* tok_hi_v, void* tok_lo
 // ---------------------------------------------------------------------------------------------------------------------
 // FFN middle, second generation (round 2): fold -> / fold(ones) -> (GELU) -> unfold of FusionFeedForward
 // (tfocal_transformer.py:89-96) for the 7/3/3 geometry, one block per (4-channel chunk x token-column tile, token-row band,
-// image).  ncu of the first-generation kernel (profiles/r02): 200 M warp instructions per launch for 90 M elements, 53 %
+// image).  The first-generation kernel executed 200 M warp instructions per launch for 90 M elements, 53 %
 // of them integer / predicate arithmetic (per-token divisions, per-element band checks), issue slots 68 % busy at 24 %
 // occupancy — instruction-bound, 0.37 of the HBM peak; on the HQ shapes the full-width image left one block per SM
 // (0.18).  Changes:
@@ -700,7 +700,7 @@ static void fold733_configure() {
 // Fused fold/normalise/unfold(/GELU).  Returns -2 (unsupported) when the geometry is not 7/3/3 or no band fits in
 // shared memory; the caller then composes launch_t2t_fold + launch_t2t_unfold.
 // First-generation launch (whole image width per block): measured faster than the x-tiled kernel while the image is
-// narrow enough for >= 2 blocks per SM (432x240 clips: 280 vs 310 us per launch at 8 clips, profiles/r02).
+// narrow enough for >= 2 blocks per SM.
 static int launch_fold733_fullwidth(const float* tin, float* tok, void* tok_hi, void* tok_lo, int bt, int c, int h, int w,
                                     int fh, int fw, int gelu, int out_pitch, cudaStream_t stream) {
   constexpr int CC = 4;

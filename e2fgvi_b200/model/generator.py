@@ -27,7 +27,7 @@ _ENC = ((3, 64, 2, 1), (64, 64, 1, 1), (64, 128, 2, 1), (128, 256, 1, 1), (256, 
 @contextlib.contextmanager
 def library_precision(mode):
     """TF32 switch of torch's LIBRARY ops around forward.  No cuDNN / cuBLAS kernel is left on the path (every conv and
-    Linear runs on the bf16x3 tcgen05 kernels, DCN / attention on fp16 operands with fp32 accumulation), so this only
+    Linear runs on the bf16x3 wgmma kernels, DCN / attention on fp16 operands with fp32 accumulation), so this only
     matters for library ops a caller wraps around the model; "strict" (default) keeps them at full fp32 like the
     reference's CPU path — TF32 costs 3-7e-3 over ~60 layers on O(1) activations (DESIGN.md §2) — "tf32" restores
     PyTorch's own default."""
@@ -83,7 +83,7 @@ class Encoder(nn.Module):
         self.layers = nn.ModuleList(layers)
 
     def forward(self, x, last_out="f32"):
-        """All nine convs run on the tcgen05 implicit-GEMM kernel (stride 2 via TMA element strides) with LeakyReLU
+        """All nine convs run on the wgmma implicit-GEMM kernel (stride 2 via TMA element strides) with LeakyReLU
         fused and the bf16 split operand handed from epilogue to the next conv; the group-wise concatenation of
         e2fgvi.py:103-108 is expressed as two TMA sources, never materialised.  ``last_out="both"`` also returns the
         bf16 (hi, lo) split of the features (operand of the propagation convs and of SoftSplit)."""
@@ -291,7 +291,7 @@ class InpaintGenerator(BaseNetwork):
         return self._decode(enc_feat), pred_flows
 
     def _decode(self, x):
-        """tanh(self.decoder(x)) (e2fgvi.py:143-150, :262) with the convs on the tcgen05 kernel, LeakyReLU(0.2) fused, and
+        """tanh(self.decoder(x)) (e2fgvi.py:143-150, :262) with the convs on the wgmma kernel, LeakyReLU(0.2) fused, and
         tanh + the NCHW store fused into the output conv."""
         d = self.decoder
         y = ops.conv3x3([ops.upsample2x_split(x)], d[0].conv.weight, d[0].conv.bias, negative_slope=0.2, out="split")

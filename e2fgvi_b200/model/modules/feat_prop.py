@@ -2,8 +2,8 @@
 
 ``SecondOrderDeformableAlignment`` keeps the reference's parameter names (``weight``, ``bias``,
 ``conv_offset.{0,2,4,6}``) and attributes (stride/padding/dilation/groups/deform_groups) but its DCN is the
-fused sm_100a kernel (``ops.deform_align_fused``): 10*tanh + flow add + sigmoid + bilinear sampling + im2col +
-tcgen05 GEMM + bias in one launch, no column buffer.  ``BidirectionalPropagation`` restates the recurrence,
+fused sm_90a kernel (``ops.deform_align_fused``): 10*tanh + flow add + sigmoid + bilinear sampling + im2col +
+wgmma GEMM + bias in one launch, no column buffer.  ``BidirectionalPropagation`` restates the recurrence,
 including the two reference quirks that trained weights depend on (SURVEY §7): the flow index is ``i-1`` for BOTH
 sweep directions (feat_prop.py:94-103) and the caller passes (forward, backward) flows into
 (flows_backward, flows_forward) (e2fgvi.py:249-250).

@@ -39,7 +39,7 @@ class SPyNetBasicModule(nn.Module):
         self.basic_module = nn.Sequential(*[_ConvHolder(ci, co) for ci, co in _LEVEL_CONVS])
 
     def forward(self, tensor_input):
-        """Five 7x7 convs on the tcgen05 implicit-GEMM kernel, ReLU fused (LeakyReLU with slope 0), the bf16 split
+        """Five 7x7 convs on the wgmma implicit-GEMM kernel, ReLU fused (LeakyReLU with slope 0), the bf16 split
         operand handed from conv to conv.  Activations with <= 32 channels (the 8-channel input, the 32- and
         16-channel intermediates) travel in the row-gapped layout so their convs use window-packed K: 7 / 28 / 14 K
         chunks per tile instead of 49 taps zero-padded to 64 channels."""

@@ -56,7 +56,7 @@ class _timed:
 def _need_cuda(*ts):
     for t in ts:
         if t is not None and not t.is_cuda:
-            raise RuntimeError("e2fgvi_b200 kernels need CUDA tensors on a B200 (sm_100a); there is no CPU fallback")
+            raise RuntimeError("e2fgvi_b200 kernels need CUDA tensors on an H100 (sm_90a); there is no CPU fallback")
 
 
 def _is_cl(x):
@@ -761,7 +761,7 @@ def _packed_conv_weight(weight, src_channels, groups, rows_cin=0):
 def conv3x3(sources, weight, bias=None, groups=1, negative_slope=1.0, residual=None, out="f32", stride=1,
             padding=None, out_lead=0):
     """``leaky_relu(F.conv2d(torch.cat(sources, 1) [group-wise for groups > 1], weight, bias, 1, 1, 1, groups),
-    negative_slope) (+ residual)`` as one tcgen05 implicit-GEMM launch; the cat is never built.
+    negative_slope) (+ residual)`` as one wgmma implicit-GEMM launch; the cat is never built.
 
     Also serves square k x k kernels (k = 3, 7) with stride 1 / 2 (``padding`` defaults to k // 2): the stride-2
     encoder convs and SPyNet's 7x7 convs (negative_slope = 0 is ReLU).

@@ -1,4 +1,4 @@
-/* e2fgvi_b200 — C ABI of the sm_100a hot-path kernels behind E2FGVI's InpaintGenerator.forward.
+/* e2fgvi_b200 — C ABI of the sm_90a hot-path kernels behind E2FGVI's InpaintGenerator.forward.
  *
  * The reference (MCG-NKU/E2FGVI) is pure Python and has no C ABI of its own; each entry point below replaces
  * one operator boundary of the reference and cites it.  A reference maintainer binds these with ctypes (see
@@ -42,7 +42,7 @@ extern "C" {
 #define E2F_PAD_ZEROS 0
 #define E2F_PAD_BORDER 1
 
-/* Library / build identification: "e2fgvi_b200 <version> sm_100a". */
+/* Library / build identification: "e2fgvi_b200 <version> sm_90a". */
 const char* e2f_version(void);
 /* Thread-local message describing the last failing call on this thread ("" if none). */
 const char* e2f_last_error(void);
@@ -66,7 +66,7 @@ int e2f_flow_warp_nchw(const float* x, const float* flow, float* out, int n, int
 int e2f_dcn_pack_weight(const float* w, void* w_packed_f16, int cout, int cin, int deform_groups, void* stream);
 
 /* modulated_deform_conv2d — replaces mmcv.ops.modulated_deform_conv2d as called at feat_prop.py:55-58
- * (3x3, stride 1, padding 1, dilation 1, groups 1).  Sampling + im2col are fused into the tcgen05 GEMM; no
+ * (3x3, stride 1, padding 1, dilation 1, groups 1).  Sampling + im2col are fused into the wgmma GEMM; no
  * column buffer is materialised.
  *   x        fp16, [N][H][W][Cin] (x_layout = E2F_X_NHWC) or group-major (E2F_X_GROUPED)     offset [N][H][W][2*9*dg] fp32, channel (g*9+tap)*2 + {0:dy, 1:dx}
  *   mask     [N][H][W][9*dg] fp32 (already sigmoid-ed), channel g*9+tap
@@ -190,7 +190,7 @@ int e2f_linear_bf16x3(const void* a_hi, const void* a_lo, const void* w_hi, cons
                       const float* residual, void* out, int m, int n, int k, int out_dtype, int tile_hint,
                       void* stream);
 
-/* 3x3 / stride 1 / pad 1 convolution (nn.Conv2d at e2fgvi.py:75-94,143-150; feat_prop.py:20-28,73-77) as a tcgen05
+/* 3x3 / stride 1 / pad 1 convolution (nn.Conv2d at e2fgvi.py:75-94,143-150; feat_prop.py:20-28,73-77) as a wgmma
  * implicit GEMM with fp32-level accuracy (bf16 3-term split, like e2f_linear_bf16x3):
  *   out = leaky_relu(conv(cat(src_0 .. src_{nsrc-1}, channel dim), W) + bias, slope) (+ residual)
  * without materialising the concatenation or an im2col buffer (TMA boxes with zero-filled out-of-bounds = padding).

@@ -21,7 +21,7 @@ def test_header_and_binding_agree(lib):
 
 
 def test_version_and_error_string(lib):
-    assert b"sm_100a" in lib.e2f_version()
+    assert b"sm_90a" in lib.e2f_version()
     assert isinstance(lib.e2f_last_error(), bytes)
 
 

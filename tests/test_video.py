@@ -12,7 +12,7 @@ import torch
 
 from e2fgvi_b200 import video as V
 from e2fgvi_b200.synth import synth_state_dict, synth_video
-from oracle import reference_loader, restate, restate_video as RV
+from oracle import restate, restate_video as RV
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
@@ -66,13 +66,31 @@ def test_oracle_driver_vs_reference_test_py(name):
     assert d.max() <= 1 and (d > 0).mean() < 1e-4
 
 
-@pytest.mark.skipif(not reference_loader.available(), reason="/root/reference only exists in the build container")
 def test_oracle_driver_bit_exact_with_reference_network():
-    model, family, wseed, frames, masks, kw, g = _case("video_hq_numref")
-    mine = importlib.import_module("e2fgvi_b200.model." + model).InpaintGenerator()
-    ref = reference_loader.reference_generator(hq=True)
-    ref.load_state_dict(synth_state_dict(mine, family, wseed), strict=True)
-    comp = RV.finalize(RV.inpaint_video(lambda x, l: ref(x, l), frames, masks, **kw))
+    """restate_video fed with the reference network's output for each of its calls reproduces test.py's output bit for
+    bit.  The composition reads a window's prediction only at the masked pixels of its local frames, and only as
+    uint8((p + 1) / 2 * 255) (test.py:168-169); the stored data are those uint8 values of the reference output, in call
+    order, and the prediction handed to the driver is the float that quantises back to each of them."""
+    *_, frames, masks, kw, g = _case("video_hq_numref")
+    q = torch.from_numpy(np.load(os.path.join(GOLDEN, "video_hq_numref_reference_net.npz"))["pred_u8"].astype(np.float32))
+    n, h, w = masks.shape
+    sched = RV.window_schedule(n, **kw)
+    used = 0
+
+    def hook(wi, pred):
+        nonlocal used
+        nb = sched[wi][1]
+        sel = torch.from_numpy(masks[nb] != 0)
+        k = int(sel.sum()) * 3
+        p = torch.zeros(len(nb), h, w, 3)
+        p[sel] = ((q[used:used + k] + 0.5) / 255 * 2 - 1).view(-1, 3)
+        used += k
+        out = torch.zeros_like(pred)
+        out[:len(nb), :, :h, :w] = p.permute(0, 3, 1, 2)
+        return out
+    comp = RV.finalize(RV.inpaint_video(lambda x, l: (torch.zeros(x.shape[1], 3, x.shape[3], x.shape[4]), None),
+                                        frames, masks, pred_hook=hook, **kw))
+    assert used == q.numel()
     assert np.array_equal(comp, g["comp"])
 
 

@@ -1,5 +1,5 @@
 """Markdown table of bench.py's per-kernel rooflines (live CUDA-event timing inside the timed region).
-    python tools/kernel_table.py profiles/r02/bench_runNN.json [workload]"""
+    python tools/kernel_table.py <bench JSON line file> [workload]"""
 import json
 import sys
 
