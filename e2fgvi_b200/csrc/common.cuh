@@ -122,104 +122,83 @@ __device__ __forceinline__ void wgmma_wait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
-// D[64 x n] (+)= A[64 x 16] . B[n x 16]^T, A and B K-major in shared memory, issued by a whole warpgroup.  Accumulator
-// fragment of thread t (warp w = (t / 32) % 4, lane l): d[4j + {0,1}] = row 16w + l/4, columns 8j + 2(l%4) + {0,1};
-// d[4j + {2,3}] = the same columns of row 16w + l/4 + 8.  acc = 0 overwrites D.
-__device__ __forceinline__ void wgmma_n16_bf16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(adesc), "l"(bdesc), "r"(acc));
+// D[64 x N] (+)= A[64 x 16] . B[N x 16]^T, A and B K-major in shared memory, issued by a whole warpgroup as ONE
+// m64nNk16 instruction.  Accumulator fragment of thread t (warp w = (t / 32) % 4, lane l): d[4j + {0,1}] = row 16w + l/4,
+// columns 8j + 2(l%4) + {0,1}; d[4j + {2,3}] = the same columns of row 16w + l/4 + 8.  acc = 0 overwrites D.
+// Every instruction reads its whole 2 KB A tile from shared memory, so one full-width instruction instead of several
+// 64-column ones cuts the A traffic: m64n64k16 alone needs 128 B/clk of shared memory at the tensor pipe's rate, all an
+// SM has; m64n128k16 needs 96 and m64n256k16 80.  B rows are contiguous 128-byte K rows (8-row groups 1024 B apart).
+//
+// Operand lists: E2F_WR<c> names accumulator registers 8c .. 8c + 7 in the PTX string, E2F_WD<n>(i) binds d[i .. i + n).
+#define E2F_WR0 "%0, %1, %2, %3, %4, %5, %6, %7"
+#define E2F_WR1 ", %8, %9, %10, %11, %12, %13, %14, %15"
+#define E2F_WR2 ", %16, %17, %18, %19, %20, %21, %22, %23"
+#define E2F_WR3 ", %24, %25, %26, %27, %28, %29, %30, %31"
+#define E2F_WR4 ", %32, %33, %34, %35, %36, %37, %38, %39"
+#define E2F_WR5 ", %40, %41, %42, %43, %44, %45, %46, %47"
+#define E2F_WR6 ", %48, %49, %50, %51, %52, %53, %54, %55"
+#define E2F_WR7 ", %56, %57, %58, %59, %60, %61, %62, %63"
+#define E2F_WR8 ", %64, %65, %66, %67, %68, %69, %70, %71"
+#define E2F_WR9 ", %72, %73, %74, %75, %76, %77, %78, %79"
+#define E2F_WR10 ", %80, %81, %82, %83, %84, %85, %86, %87"
+#define E2F_WR11 ", %88, %89, %90, %91, %92, %93, %94, %95"
+#define E2F_WR12 ", %96, %97, %98, %99, %100, %101, %102, %103"
+#define E2F_WR13 ", %104, %105, %106, %107, %108, %109, %110, %111"
+#define E2F_WR14 ", %112, %113, %114, %115, %116, %117, %118, %119"
+#define E2F_WR15 ", %120, %121, %122, %123, %124, %125, %126, %127"
+#define E2F_WD8(i) "+f"(d[(i)]), "+f"(d[(i) + 1]), "+f"(d[(i) + 2]), "+f"(d[(i) + 3]), \
+                   "+f"(d[(i) + 4]), "+f"(d[(i) + 5]), "+f"(d[(i) + 6]), "+f"(d[(i) + 7])
+#define E2F_WD16(i) E2F_WD8(i), E2F_WD8((i) + 8)
+#define E2F_WD32(i) E2F_WD16(i), E2F_WD16((i) + 16)
+#define E2F_WD64(i) E2F_WD32(i), E2F_WD32((i) + 32)
+
+// one specialisation per (N, f16) the kernels use; any other width fails to compile
+template <int N, bool F16>
+struct WgmmaSS;
+// IA / IB / IP: operand numbers of the A descriptor, the B descriptor and the accumulate flag (N/2, N/2 + 1, N/2 + 2)
+#define E2F_WGMMA_SS(N, F16, TY, REGS, IA, IB, IP, ...)                                                              \
+  template <>                                                                                                       \
+  struct WgmmaSS<N, F16> {                                                                                          \
+    static __device__ __forceinline__ void run(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {            \
+      asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %" IP ", 0;\n"                                                 \
+                   "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32." TY "." TY " {" REGS "}, %" IA ", %" IB         \
+                   ", p, 1, 1, 0, 0;\n}\n"                                                                          \
+                   : __VA_ARGS__                                                                                    \
+                   : "l"(adesc), "l"(bdesc), "r"(acc));                                                             \
+    }                                                                                                               \
+  };
+E2F_WGMMA_SS(32, false, "bf16", E2F_WR0 E2F_WR1, "16", "17", "18", E2F_WD16(0))
+E2F_WGMMA_SS(48, false, "bf16", E2F_WR0 E2F_WR1 E2F_WR2, "24", "25", "26", E2F_WD16(0), E2F_WD8(16))
+E2F_WGMMA_SS(64, false, "bf16", E2F_WR0 E2F_WR1 E2F_WR2 E2F_WR3, "32", "33", "34", E2F_WD32(0))
+E2F_WGMMA_SS(96, false, "bf16", E2F_WR0 E2F_WR1 E2F_WR2 E2F_WR3 E2F_WR4 E2F_WR5, "48", "49", "50", E2F_WD32(0),
+             E2F_WD16(32))
+E2F_WGMMA_SS(112, false, "bf16", E2F_WR0 E2F_WR1 E2F_WR2 E2F_WR3 E2F_WR4 E2F_WR5 E2F_WR6, "56", "57", "58",
+             E2F_WD32(0), E2F_WD16(32), E2F_WD8(48))
+E2F_WGMMA_SS(128, false, "bf16", E2F_WR0 E2F_WR1 E2F_WR2 E2F_WR3 E2F_WR4 E2F_WR5 E2F_WR6 E2F_WR7, "64", "65", "66",
+             E2F_WD64(0))
+E2F_WGMMA_SS(224, false, "bf16",
+             E2F_WR0 E2F_WR1 E2F_WR2 E2F_WR3 E2F_WR4 E2F_WR5 E2F_WR6 E2F_WR7 E2F_WR8 E2F_WR9 E2F_WR10 E2F_WR11 E2F_WR12
+                 E2F_WR13,
+             "112", "113", "114", E2F_WD64(0), E2F_WD32(64), E2F_WD16(96))
+E2F_WGMMA_SS(256, false, "bf16",
+             E2F_WR0 E2F_WR1 E2F_WR2 E2F_WR3 E2F_WR4 E2F_WR5 E2F_WR6 E2F_WR7 E2F_WR8 E2F_WR9 E2F_WR10 E2F_WR11 E2F_WR12
+                 E2F_WR13 E2F_WR14 E2F_WR15,
+             "128", "129", "130", E2F_WD64(0), E2F_WD64(64))
+E2F_WGMMA_SS(64, true, "f16", E2F_WR0 E2F_WR1 E2F_WR2 E2F_WR3, "32", "33", "34", E2F_WD32(0))
+E2F_WGMMA_SS(128, true, "f16", E2F_WR0 E2F_WR1 E2F_WR2 E2F_WR3 E2F_WR4 E2F_WR5 E2F_WR6 E2F_WR7, "64", "65", "66",
+             E2F_WD64(0))
+
+template <int N, bool F16>
+__device__ __forceinline__ void wgmma_ss(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  WgmmaSS<N, F16>::run(d, adesc, bdesc, acc);
 }
-__device__ __forceinline__ void wgmma_n16_f16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(adesc), "l"(bdesc), "r"(acc));
-}
-__device__ __forceinline__ void wgmma_n32_bf16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(adesc), "l"(bdesc), "r"(acc));
-}
-__device__ __forceinline__ void wgmma_n32_f16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(adesc), "l"(bdesc), "r"(acc));
-}
-__device__ __forceinline__ void wgmma_n64_bf16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(adesc), "l"(bdesc), "r"(acc));
-}
-__device__ __forceinline__ void wgmma_n64_f16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(adesc), "l"(bdesc), "r"(acc));
-}
+// register-A variant (A fragment in registers, B transposed = MN-major in shared memory)
 __device__ __forceinline__ void wgmma_n64_f16_rs_tb(float* d, const uint32_t (&a)[4], uint64_t bdesc, uint32_t acc) {
   asm volatile(
       "{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {" E2F_WR0 E2F_WR1 E2F_WR2 E2F_WR3 "}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n}\n"
+      : E2F_WD32(0)
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(acc));
-}
-
-// n = N (multiple of 16) as blocks of 64 / 32 / 16 columns; the B rows of the next block start n*128 bytes further
-template <int N, bool F16>
-__device__ __forceinline__ void wgmma_ss(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
-  static_assert(N % 16 == 0 && N > 0, "wgmma N");
-  if constexpr (N >= 64) {
-    if constexpr (F16) wgmma_n64_f16(d, adesc, bdesc, acc);
-    else wgmma_n64_bf16(d, adesc, bdesc, acc);
-    if constexpr (N > 64) wgmma_ss<N - 64, F16>(d + 32, adesc, gmma_desc_adv(bdesc, 64 * 128), acc);
-  } else if constexpr (N >= 32) {
-    if constexpr (F16) wgmma_n32_f16(d, adesc, bdesc, acc);
-    else wgmma_n32_bf16(d, adesc, bdesc, acc);
-    if constexpr (N > 32) wgmma_ss<N - 32, F16>(d + 16, adesc, gmma_desc_adv(bdesc, 32 * 128), acc);
-  } else {
-    if constexpr (F16) wgmma_n16_f16(d, adesc, bdesc, acc);
-    else wgmma_n16_bf16(d, adesc, bdesc, acc);
-  }
-}
-
-// Accumulator staging: a warpgroup's fragments written to a [rows][N] fp32 shared-memory tile so that a thread can
-// read a whole row (the row-per-thread epilogues).  16-byte chunk c of row r sits at chunk c ^ (r & 7): row-parallel
-// 16-byte reads by 8 consecutive rows hit 8 different bank groups.
-__device__ __forceinline__ uint32_t acc_stage_offset(uint32_t row, uint32_t col, uint32_t n) {
-  return row * n * 4u + ((((col >> 2) ^ (row & 7u))) << 4) + (col & 3u) * 4u;
-}
-template <int N>
-__device__ __forceinline__ void acc_stage_store(uint32_t stage_smem, const float* d, int row0, int lane) {
-  // row0: first row of the calling warp's 16-row slice
-  const int r = row0 + (lane >> 2), c = 2 * (lane & 3);
-#pragma unroll
-  for (int j = 0; j < N / 8; ++j) {
-    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(stage_smem + acc_stage_offset(r, 8 * j + c, N)),
-                 "f"(d[4 * j]), "f"(d[4 * j + 1]) : "memory");
-    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(stage_smem + acc_stage_offset(r + 8, 8 * j + c, N)),
-                 "f"(d[4 * j + 2]), "f"(d[4 * j + 3]) : "memory");
-  }
-}
-// 32 consecutive columns [col0, col0 + 32) of row r (col0 % 32 == 0)
-__device__ __forceinline__ void acc_stage_load32(uint32_t stage_smem, uint32_t r, uint32_t col0, uint32_t n,
-                                                 uint32_t (&v)[32]) {
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
-                 : "=r"(v[4 * i]), "=r"(v[4 * i + 1]), "=r"(v[4 * i + 2]), "=r"(v[4 * i + 3])
-                 : "r"(stage_smem + acc_stage_offset(r, col0 + 4 * i, n))
-                 : "memory");
 }
 
 // ----------------------------------------------------------------------------- misc

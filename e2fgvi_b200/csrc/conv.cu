@@ -19,7 +19,7 @@
 //  * epilogue: + bias, LeakyReLU(slope), optional residual add, fp32 NHWC store and/or the bf16 (hi, lo) split of
 //    the result — dense NHWC or row-gapped for a following window-packed conv (the zero gaps are written here).
 // Pipeline = gemm.cu: persistent CTAs, TMA warp + two consumer warpgroups (64 accumulator rows each, fp32 in registers);
-// a finished accumulator is staged through shared memory so that the epilogue can work row-per-thread.
+// each warp's epilogue reads its own accumulator fragments (no CTA-wide staging tile, so the pipeline gets that room).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cstdlib>
@@ -32,7 +32,7 @@ namespace conv {
 constexpr int BM = 128, BK = 64;
 constexpr int TILE_H = 8, TILE_W = 16;                  // 8 x 16 output pixels = 128 GEMM rows
 constexpr int A_TILE = BM * BK * 2;
-constexpr int EPI_WARPS = 8;                             // two consumer warpgroups; in the epilogue two warps per 32 rows, half of the columns each
+constexpr int EPI_WARPS = 8;                             // two consumer warpgroups; in the epilogue each warp stores its 16 accumulator rows
 constexpr int MAX_COUT = 512;                            // bias staged in shared memory once per CTA
 constexpr int EPI_STAGE = 2048;                          // per epilogue warp: 32 rows x 64 bytes store-transposition buffer
 constexpr int THREADS = (EPI_WARPS + 1) * 32;                // + the TMA warp
@@ -44,11 +44,10 @@ constexpr int MAX_SRC = 4;
 template <int BN>
 struct Cfg {
   static constexpr int W_TILE = BN * BK * 2;
-  static constexpr int STAGE = 2 * A_TILE + 2 * W_TILE;   // 64 KB (BN=128) / 48 KB (BN=64) / 40 KB (BN=32)
-  static constexpr int ACC_STAGE = BM * BN * 4;           // fp32 accumulator tile staged for the epilogue
-  // as many stages as fit next to the accumulator staging in the 227 KB a CTA may use
-  static constexpr int STAGES = (BN >= 96) ? 2 : (BN == 64) ? 3 : 4;
-  static constexpr int SMEM = STAGES * STAGE + 256 + MAX_COUT * 4 + EPI_WARPS * EPI_STAGE + ACC_STAGE + 1024;
+  static constexpr int STAGE = 2 * A_TILE + 2 * W_TILE;   // 64 KB (BN=128) / 56 KB (BN=96) / 48 KB (BN=64) / 40 KB (BN=32)
+  // as many stages as fit in the 227 KB a CTA may use: 211 / 168 / 211 / 219 KB
+  static constexpr int STAGES = (BN >= 96) ? 3 : (BN == 64) ? 4 : 5;
+  static constexpr int SMEM = STAGES * STAGE + 256 + MAX_COUT * 4 + EPI_WARPS * EPI_STAGE + 1024;
 };
 
 struct Maps {
@@ -123,22 +122,29 @@ __device__ __forceinline__ TileCoord decode_tile(int tile, const Params& p, int 
   return t;
 }
 
-// Epilogue of one 128-pixel x BN-channel tile for the calling thread's accumulator row `r`: + bias, LeakyReLU, optional
-// residual, fp32 and/or bf16-split NHWC stores.  TW = tile width in pixels (row r is pixel (y0 + r / TW, x0 + r % TW));
-// acc_smem = the accumulator tile staged in shared memory (acc_stage_store layout).
-// The calling warp handles the 32-column chunks [c_begin, c_end) of the tile.  bias_s = the layer's bias in SHARED
-// memory (zeros when the layer has none): per-channel __ldg's would queue behind the epilogue's own stores.
+// Epilogue of the calling warp's 16 accumulator rows [row0, row0 + 16) x all BN channels of one 128-pixel tile, read
+// straight from the wgmma fragments `acc`: + bias, LeakyReLU, optional residual, fp32 and/or bf16-split NHWC stores.
+// TW = tile width in pixels (row R is pixel (y0 + R / TW, x0 + R % TW)).  bias_s = the layer's bias in SHARED memory
+// (zeros when the layer has none): per-channel __ldg's would queue behind the epilogue's own stores.
 //
-// Stores are STAGED through `stage` (2 KB of shared memory per epilogue warp): with thread = pixel, a direct 16-byte store
-// per thread hits 32 different 128-byte lines per instruction (pixels are Cout * 2 or 4 bytes apart), ~125 cycles each,
-// which made the epilogue the bottleneck of the layers with a short main loop.  Each warp instead transposes its
-// 32 rows x 64 bytes through a conflict-free XOR-swizzled buffer so that 4 consecutive lanes write one pixel's 64
-// contiguous bytes (8 lines per instruction).  Chunks that are not 32 full, 16-byte-aligned channels take the direct path.
+// Everything goes through `stage`, 2 KB of shared memory private to the warp, one 32-channel chunk at a time:
+//  1. fragments -> [16 rows][32 fp32], 16-byte chunk q of row a at q ^ (a & 7): each lane quad holds 8 channels of rows a
+//     and a + 8, and the 8 rows of one store instruction hit 8 different bank groups;
+//  2. read back row-wise: lane = (row lane % 16, channels 16 (lane / 16) .. + 16 of the chunk), the thread = pixel form
+//     in which bias, residual and bias map are 16-byte loads;
+//  3. coalesced stores: with thread = pixel, a direct 16-byte store per thread hits 32 different 128-byte lines per
+//     instruction (pixels are Cout * 2 or 4 bytes apart), ~125 cycles each.  The results instead go to 64-byte buffer
+//     rows through a conflict-free XOR swizzle (fp32: row `lane` = its 16 channels; split: row p = the 32 hi channels of
+//     pixel row p, row 16 + p = the 32 lo channels), and 4 consecutive lanes then store one buffer row: 64 contiguous
+//     bytes of one pixel.
+// Chunks that are not 32 full, 16-byte-aligned channels take the direct path.
 template <int BN>
-__device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& t, uint32_t acc_smem, int r, int cog,
-                                              const float* __restrict__ bias_s, int c_begin, int c_end,
-                                              uint8_t* __restrict__ stage, const int TW, const int TH) {
-  const int lane = r & 31;
+__device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& t, const float* acc, int row0, int cog,
+                                              const float* __restrict__ bias_s, uint8_t* __restrict__ stage, const int TW,
+                                              const int TH) {
+  const int lane = threadIdx.x & 31;
+  const int hf = lane >> 4;                            // which 16 channels of a 32-channel chunk this lane handles
+  const int r = row0 + (lane & 15);                    // this lane's accumulator row
   // accumulator row R -> GEMM-grid pixel (gy, gx) -> output pixel (Y, X) of the out_H x out_W image
   auto map_row = [&](int R, int& Y, int& X) -> bool {
     const int ly = R / TW, gy = t.y0 + ly, gx = t.x0 + (R - ly * TW);
@@ -148,21 +154,41 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
   };
   int y, x;                                            // this thread's OUTPUT pixel
   const bool pix_ok = map_row(r, y, x);
-  const size_t pix = static_cast<size_t>(t.n) * p.out_nstride + static_cast<size_t>(y) * p.out_W + x;        // fp32 out, residual
-  const size_t opix = static_cast<size_t>(t.n) * p.osp_nstride + static_cast<size_t>(y) * p.out_pitch + p.out_lead + x;   // split outputs
-  const size_t mpix = static_cast<size_t>(y) * p.out_W + x;                                         // bias map
+  // pixel indices of this thread's output pixel, computed where used (the fp32 accumulator fills most registers)
+  auto pix = [&] { return static_cast<size_t>(t.n) * p.out_nstride + static_cast<size_t>(y) * p.out_W + x; };          // fp32 out, residual
+  auto opix = [&] { return static_cast<size_t>(t.n) * p.osp_nstride + static_cast<size_t>(y) * p.out_pitch + p.out_lead + x; };  // split outputs
+  auto mpix = [&] { return static_cast<size_t>(y) * p.out_W + x; };                                    // bias map
   const int co_end = (t.g + 1) * cog;               // exclusive end of this group's output channels
   const bool vec_ok = (p.Cout & 3) == 0;            // 16-byte aligned channel groups
-#pragma unroll 1
-  for (int c = c_begin; c < c_end; ++c) {
-    uint32_t v[32];
-    acc_stage_load32(acc_smem, r, c * 32, BN, v);
-    const int co = t.co0 + c * 32;
-    if (vec_ok && co + 32 <= co_end) {
-      // ------------------------------------------------------------ staged, coalesced stores (warp-uniform branch)
-      float f[32];
+  const uint32_t sbase = smem_u32(stage);
+#pragma unroll                                      // compile-time fragment indices: acc stays in registers
+  for (int c = 0; c < BN / 32; ++c) {
+    // ---------------------------------------------------------------- 1 + 2: fragments -> row-wise values
+    __syncwarp();                                   // the previous chunk's stores have read the buffer
+    const int qa = lane >> 2, qc = (lane & 3) >> 1, qo = (lane & 1) * 8;
 #pragma unroll
-      for (int g4 = 0; g4 < 8; ++g4) {
+    for (int jj = 0; jj < 4; ++jj) {
+      const int j = 4 * c + jj;                     // columns 8j + 2 (lane % 4) + {0, 1} of rows qa, qa + 8
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(sbase + sw128_offset(qa, 2 * jj + qc) + qo),
+                   "f"(acc[4 * j]), "f"(acc[4 * j + 1]) : "memory");
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(sbase + sw128_offset(qa + 8, 2 * jj + qc) + qo),
+                   "f"(acc[4 * j + 2]), "f"(acc[4 * j + 3]) : "memory");
+    }
+    __syncwarp();
+    uint32_t v[16];
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+      asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
+                   : "=r"(v[4 * q]), "=r"(v[4 * q + 1]), "=r"(v[4 * q + 2]), "=r"(v[4 * q + 3])
+                   : "r"(sbase + sw128_offset(lane & 15, 4 * hf + q))
+                   : "memory");
+    __syncwarp();                                   // every lane has its values before the buffer is reused
+    const int co_chunk = t.co0 + c * 32, co = co_chunk + 16 * hf;
+    if (vec_ok && co_chunk + 32 <= co_end) {
+      // ------------------------------------------------------------ 3: staged, coalesced stores (warp-uniform branch)
+      float f[16];
+#pragma unroll
+      for (int g4 = 0; g4 < 4; ++g4) {
         const float4 b = *reinterpret_cast<const float4*>(bias_s + co + g4 * 4);
         const float bb[4] = {b.x, b.y, b.z, b.w};
 #pragma unroll
@@ -172,91 +198,88 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
         }
       }
       if (p.residual && pix_ok) {
-        const float4* r4 = reinterpret_cast<const float4*>(p.residual + pix * p.Cout + co);
+        const float4* r4 = reinterpret_cast<const float4*>(p.residual + pix() * p.Cout + co);
 #pragma unroll
-        for (int g4 = 0; g4 < 8; ++g4) {
+        for (int g4 = 0; g4 < 4; ++g4) {
           const float4 ra = __ldg(r4 + g4);
           f[g4 * 4] += ra.x; f[g4 * 4 + 1] += ra.y; f[g4 * 4 + 2] += ra.z; f[g4 * 4 + 3] += ra.w;
         }
       }
       if (p.bias_map && pix_ok) {
-        const float4* m4 = reinterpret_cast<const float4*>(p.bias_map + mpix * p.Cout + co);
+        const float4* m4 = reinterpret_cast<const float4*>(p.bias_map + mpix() * p.Cout + co);
 #pragma unroll
-        for (int g4 = 0; g4 < 8; ++g4) {
+        for (int g4 = 0; g4 < 4; ++g4) {
           const float4 ra = __ldg(m4 + g4);
           f[g4 * 4] += ra.x; f[g4 * 4 + 1] += ra.y; f[g4 * 4 + 2] += ra.z; f[g4 * 4 + 3] += ra.w;
         }
       }
-      // write side: row = lane, logical 16-byte chunk cc at physical chunk cc ^ ((lane >> 1) & 3); read side: lanes
-      // 4k..4k+3 fetch the 4 chunks of row j*8 + k.  Both sides touch 8 distinct bank groups per quarter-warp.
-      const uint32_t wbase = smem_u32(stage) + lane * 64, wsw = (lane >> 1) & 3;
-      const int sub = lane & 3, prow = lane >> 2, rbase = r - lane;
-      auto st_chunk = [&](int cc, uint32_t a, uint32_t b, uint32_t c2, uint32_t d) {
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(wbase + ((cc ^ wsw) << 4)), "r"(a), "r"(b), "r"(c2), "r"(d)
+      // logical 16-byte chunk cc of buffer row rr sits at physical chunk cc ^ ((rr >> 1) & 3); on the read side lanes
+      // 4k..4k+3 fetch the 4 chunks of buffer row jr*8 + k.  Both sides touch 8 distinct bank groups per quarter-warp.
+      const int sub = lane & 3, prow = lane >> 2;
+      auto st_chunk = [&](int rr, int cc, uint32_t a, uint32_t b, uint32_t c2, uint32_t d) {
+        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(sbase + rr * 64 + ((cc ^ ((rr >> 1) & 3)) << 4)),
+                     "r"(a), "r"(b), "r"(c2), "r"(d)
                      : "memory");
       };
       auto ld_chunk = [&](int rr) {
         uint4 u;
         asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
                      : "=r"(u.x), "=r"(u.y), "=r"(u.z), "=r"(u.w)
-                     : "r"(smem_u32(stage) + rr * 64 + ((sub ^ ((rr >> 1) & 3)) << 4))
+                     : "r"(sbase + rr * 64 + ((sub ^ ((rr >> 1) & 3)) << 4))
                      : "memory");
         return u;
       };
-      if (p.out) {
+      if (p.out) {                                  // buffer row lane = its 16 fp32 channels: row rr is accumulator row
+                                                    // row0 + rr % 16, channels 16 (rr / 16) .. + 16 of the chunk
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {                 // 16 fp32 channels = 64 bytes per row and pass
+        for (int cc = 0; cc < 4; ++cc)
+          st_chunk(lane, cc, __float_as_uint(f[cc * 4]), __float_as_uint(f[cc * 4 + 1]), __float_as_uint(f[cc * 4 + 2]),
+                   __float_as_uint(f[cc * 4 + 3]));
+        __syncwarp();
 #pragma unroll
-          for (int cc = 0; cc < 4; ++cc)
-            st_chunk(cc, __float_as_uint(f[h * 16 + cc * 4]), __float_as_uint(f[h * 16 + cc * 4 + 1]),
-                     __float_as_uint(f[h * 16 + cc * 4 + 2]), __float_as_uint(f[h * 16 + cc * 4 + 3]));
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int rr = j * 8 + prow, R = rbase + rr;
-            int yy, xx;
-            const bool ok = map_row(R, yy, xx);
-            const uint4 u = ld_chunk(rr);
-            if (ok)
-              *reinterpret_cast<uint4*>(p.out + (static_cast<size_t>(t.n) * p.out_nstride + static_cast<size_t>(yy) * p.out_W + xx) * p.Cout +
-                                        co + h * 16 + sub * 4) = u;
-          }
-          __syncwarp();
+        for (int jr = 0; jr < 4; ++jr) {
+          const int rr = jr * 8 + prow;
+          int yy, xx;
+          const bool ok = map_row(row0 + (rr & 15), yy, xx);
+          const uint4 u = ld_chunk(rr);
+          if (ok)
+            *reinterpret_cast<uint4*>(p.out + (static_cast<size_t>(t.n) * p.out_nstride + static_cast<size_t>(yy) * p.out_W + xx) * p.Cout +
+                                      co_chunk + 16 * (rr >> 4) + sub * 4) = u;
         }
+        __syncwarp();
       }
-      if (p.out_hi) {
-        uint32_t hp[16], lp[16];                      // packed bf16 pairs
+      if (p.out_hi) {                               // buffer rows [0, 16): 32 bf16 hi channels per pixel row, [16, 32): lo
+        uint32_t hp[8], lp[8];                      // packed bf16 pairs
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
+        for (int i = 0; i < 8; ++i) {
           const __nv_bfloat162 hb = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
-          const float2 hf = __bfloat1622float2(hb);
-          const __nv_bfloat162 lb = __floats2bfloat162_rn(f[2 * i] - hf.x, f[2 * i + 1] - hf.y);
+          const float2 hfl = __bfloat1622float2(hb);
+          const __nv_bfloat162 lb = __floats2bfloat162_rn(f[2 * i] - hfl.x, f[2 * i + 1] - hfl.y);
           hp[i] = *reinterpret_cast<const uint32_t*>(&hb);
           lp[i] = *reinterpret_cast<const uint32_t*>(&lb);
         }
+        const int pr = lane & 15;                   // this lane's pixel row; its 16 channels are chunks 2 hf, 2 hf + 1
+        st_chunk(pr, 2 * hf, hp[0], hp[1], hp[2], hp[3]);
+        st_chunk(pr, 2 * hf + 1, hp[4], hp[5], hp[6], hp[7]);
+        st_chunk(16 + pr, 2 * hf, lp[0], lp[1], lp[2], lp[3]);
+        st_chunk(16 + pr, 2 * hf + 1, lp[4], lp[5], lp[6], lp[7]);
+        __syncwarp();
 #pragma unroll
-        for (int part = 0; part < 2; ++part) {        // 32 bf16 channels = 64 bytes per row: hi, then lo
-          const uint32_t* src = part ? lp : hp;
-          __nv_bfloat16* dst = part ? p.out_lo : p.out_hi;
-#pragma unroll
-          for (int cc = 0; cc < 4; ++cc) st_chunk(cc, src[cc * 4], src[cc * 4 + 1], src[cc * 4 + 2], src[cc * 4 + 3]);
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int rr = j * 8 + prow, R = rbase + rr;
-            int yy, xx;
-            const bool ok = map_row(R, yy, xx);
-            const uint4 u = ld_chunk(rr);
-            if (ok)
-              *reinterpret_cast<uint4*>(dst + (static_cast<size_t>(t.n) * p.osp_nstride + static_cast<size_t>(yy) * p.out_pitch + p.out_lead + xx) *
-                                              p.Cout + co + sub * 8) = u;
-          }
-          __syncwarp();
+        for (int jr = 0; jr < 4; ++jr) {
+          const int rr = jr * 8 + prow;
+          int yy, xx;
+          const bool ok = map_row(row0 + (rr & 15), yy, xx);
+          const uint4 u = ld_chunk(rr);
+          __nv_bfloat16* dst = rr < 16 ? p.out_hi : p.out_lo;
+          if (ok)
+            *reinterpret_cast<uint4*>(dst + (static_cast<size_t>(t.n) * p.osp_nstride + static_cast<size_t>(yy) * p.out_pitch + p.out_lead + xx) *
+                                            p.Cout + co_chunk + sub * 8) = u;
         }
+        __syncwarp();
       }
     } else if (pix_ok && co < co_end) {
 #pragma unroll
-      for (int g8 = 0; g8 < 4; ++g8) {              // 8 output channels at a time
+      for (int g8 = 0; g8 < 2; ++g8) {              // 8 output channels at a time
         const int cb = co + g8 * 8;
         if (vec_ok && cb + 8 <= co_end) {
           float f[8];
@@ -268,19 +291,19 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
             f[i] = a > 0.f ? a : a * p.slope;
           }
           if (p.residual) {
-            const float4* r4 = reinterpret_cast<const float4*>(p.residual + pix * p.Cout + cb);
+            const float4* r4 = reinterpret_cast<const float4*>(p.residual + pix() * p.Cout + cb);
             const float4 ra = __ldg(r4), rb = __ldg(r4 + 1);
             f[0] += ra.x; f[1] += ra.y; f[2] += ra.z; f[3] += ra.w;
             f[4] += rb.x; f[5] += rb.y; f[6] += rb.z; f[7] += rb.w;
           }
           if (p.bias_map) {
-            const float4* r4 = reinterpret_cast<const float4*>(p.bias_map + mpix * p.Cout + cb);
+            const float4* r4 = reinterpret_cast<const float4*>(p.bias_map + mpix() * p.Cout + cb);
             const float4 ra = __ldg(r4), rb = __ldg(r4 + 1);
             f[0] += ra.x; f[1] += ra.y; f[2] += ra.z; f[3] += ra.w;
             f[4] += rb.x; f[5] += rb.y; f[6] += rb.z; f[7] += rb.w;
           }
           if (p.out) {
-            float4* d4 = reinterpret_cast<float4*>(p.out + pix * p.Cout + cb);
+            float4* d4 = reinterpret_cast<float4*>(p.out + pix() * p.Cout + cb);
             d4[0] = make_float4(f[0], f[1], f[2], f[3]);
             d4[1] = make_float4(f[4], f[5], f[6], f[7]);
           }
@@ -289,13 +312,13 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
               const __nv_bfloat162 hb = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
-              const float2 hf = __bfloat1622float2(hb);
-              const __nv_bfloat162 lb = __floats2bfloat162_rn(f[2 * i] - hf.x, f[2 * i + 1] - hf.y);
+              const float2 hfl = __bfloat1622float2(hb);
+              const __nv_bfloat162 lb = __floats2bfloat162_rn(f[2 * i] - hfl.x, f[2 * i + 1] - hfl.y);
               hp[i] = *reinterpret_cast<const uint32_t*>(&hb);
               lp[i] = *reinterpret_cast<const uint32_t*>(&lb);
             }
-            *reinterpret_cast<uint4*>(p.out_hi + opix * p.Cout + cb) = make_uint4(hp[0], hp[1], hp[2], hp[3]);
-            *reinterpret_cast<uint4*>(p.out_lo + opix * p.Cout + cb) = make_uint4(lp[0], lp[1], lp[2], lp[3]);
+            *reinterpret_cast<uint4*>(p.out_hi + opix() * p.Cout + cb) = make_uint4(hp[0], hp[1], hp[2], hp[3]);
+            *reinterpret_cast<uint4*>(p.out_lo + opix() * p.Cout + cb) = make_uint4(lp[0], lp[1], lp[2], lp[3]);
           }
         } else if (cb < co_end) {
 #pragma unroll
@@ -303,19 +326,19 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
             if (cb + i < co_end) {
               float a = __uint_as_float(v[g8 * 8 + i]) + bias_s[cb + i];
               a = a > 0.f ? a : a * p.slope;
-              if (p.residual) a += __ldg(p.residual + pix * p.Cout + cb + i);
-              if (p.bias_map) a += __ldg(p.bias_map + mpix * p.Cout + cb + i);
+              if (p.residual) a += __ldg(p.residual + pix() * p.Cout + cb + i);
+              if (p.bias_map) a += __ldg(p.bias_map + mpix() * p.Cout + cb + i);
               if (p.epi_flags & EPI_TANH) a = tanhf(a);
               if (p.out) {
                 if (p.epi_flags & EPI_NCHW)   // thread = pixel: consecutive lanes write consecutive x of one channel plane
                   p.out[((static_cast<size_t>(t.n) * p.Cout + cb + i) * p.out_H + y) * p.out_W + x] = a;
                 else
-                  p.out[pix * p.Cout + cb + i] = a;
+                  p.out[pix() * p.Cout + cb + i] = a;
               }
               if (p.out_hi) {
                 const __nv_bfloat16 hb = __float2bfloat16_rn(a);
-                p.out_hi[opix * p.Cout + cb + i] = hb;
-                p.out_lo[opix * p.Cout + cb + i] = __float2bfloat16_rn(a - __bfloat162float(hb));
+                p.out_hi[opix() * p.Cout + cb + i] = hb;
+                p.out_lo[opix() * p.Cout + cb + i] = __float2bfloat16_rn(a - __bfloat162float(hb));
               }
             }
           }
@@ -324,17 +347,18 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
     }
   }
   // row-gapped split output: the pixel at x == 0 also writes the zero gap in front of its row, the very last pixel
-  // the zero tail (once per pixel: only the first N tile of group 0 does it; Cout % 8 == 0 is checked by the API)
-  if (p.out_hi && p.out_lead && pix_ok && t.co0 == 0 && c_begin == 0) {
+  // the zero tail (once per pixel: only the first-half lane of the first N tile of group 0 does it; Cout % 8 == 0 is
+  // checked by the API)
+  if (p.out_hi && p.out_lead && pix_ok && t.co0 == 0 && hf == 0) {
     const uint4 z = make_uint4(0, 0, 0, 0);
     if (x == 0) {
-      uint4* zh = reinterpret_cast<uint4*>(p.out_hi + (opix - p.out_lead) * p.Cout);
-      uint4* zl = reinterpret_cast<uint4*>(p.out_lo + (opix - p.out_lead) * p.Cout);
+      uint4* zh = reinterpret_cast<uint4*>(p.out_hi + (opix() - p.out_lead) * p.Cout);
+      uint4* zl = reinterpret_cast<uint4*>(p.out_lo + (opix() - p.out_lead) * p.Cout);
       for (int i = 0; i < p.out_lead * p.Cout / 8; ++i) zh[i] = zl[i] = z;
     }
     if (x == p.out_W - 1 && y == p.out_H - 1 && t.n == p.N - 1) {
-      uint4* zh = reinterpret_cast<uint4*>(p.out_hi + (opix + 1) * p.Cout);
-      uint4* zl = reinterpret_cast<uint4*>(p.out_lo + (opix + 1) * p.Cout);
+      uint4* zh = reinterpret_cast<uint4*>(p.out_hi + (opix() + 1) * p.Cout);
+      uint4* zl = reinterpret_cast<uint4*>(p.out_lo + (opix() + 1) * p.Cout);
       for (int i = 0; i < p.out_tail * p.Cout / 8; ++i) zh[i] = zl[i] = z;
     }
   }
@@ -349,7 +373,6 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_kernel(const __grid_consta
   uint64_t* empty = full + STAGES;
   float* bias_s = reinterpret_cast<float*>(smem + STAGES * STAGE + 256);
   uint8_t* epi_stage = smem + STAGES * STAGE + 256 + MAX_COUT * 4;
-  const uint32_t acc_smem = smem_u32(epi_stage + EPI_WARPS * EPI_STAGE);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   for (int i = tid; i < MAX_COUT; i += blockDim.x) bias_s[i] = (p.bias && i < p.Cout) ? __ldg(p.bias + i) : 0.f;
@@ -429,10 +452,6 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_kernel(const __grid_consta
     const uint64_t d_al0 = gmma_desc_adv(d_ah0, A_TILE);
     const uint64_t d_wh0 = gmma_desc_sw128(smem_u32(smem) + 2 * A_TILE, 16, 1024);
     const uint64_t d_wl0 = gmma_desc_adv(d_wh0, W_TILE);
-    // epilogue: warp wq reads rows 64 wg + 32 (wq & 1) + lane, the first or second half of the 32-column chunks
-    constexpr int NCH = BN / 32;
-    const int c_split = (NCH + 1) / 2;
-    const int c_begin = (wq >> 1) ? c_split : 0, c_end = (wq >> 1) ? NCH : c_split;
     uint8_t* my_stage = epi_stage + warp * EPI_STAGE;
     float acc[BN / 2];
     uint32_t it = 0;
@@ -461,12 +480,8 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_kernel(const __grid_consta
       }
       wgmma_wait<0>();
       if (num_kb > 0 && lane == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
-      acc_stage_store<BN>(acc_smem, acc, wg * 64 + wq * 16, lane);
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // this warpgroup's 64 rows staged
       const TileCoord t = decode_tile<BN>(tile, p, tiles_y, tiles_x, tiles_ng);
-      epilogue_tile<BN>(p, t, acc_smem, wg * 64 + 32 * (wq & 1) + lane, cog, bias_s, c_begin, c_end, my_stage, p.tile_w,
-                        p.tile_h);
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // staging read before the next tile overwrites it
+      epilogue_tile<BN>(p, t, acc, wg * 64 + wq * 16, cog, bias_s, my_stage, p.tile_w, p.tile_h);
     }
   }
 }
@@ -505,13 +520,11 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_halo_kernel(const __grid_c
   uint64_t* w_full = a_empty + HALO_MAX_SLOTS;
   float* bias_s = reinterpret_cast<float*>(ring + nslots * HALO_SLOT + 256);
   uint8_t* epi_stage = ring + nslots * HALO_SLOT + 256 + MAX_COUT * 4;
-  const uint32_t acc_smem = smem_u32(epi_stage + EPI_WARPS * EPI_STAGE);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   for (int i = tid; i < MAX_COUT; i += blockDim.x) bias_s[i] = (p.bias && i < p.Cout) ? __ldg(p.bias + i) : 0.f;
   const int tiles_y = (p.H + HTILE_H - 1) / HTILE_H, tiles_x = (p.W + HTILE_W - 1) / HTILE_W;
   const int num_tiles = p.N * tiles_y * tiles_x;
-  const int pieces = 2 * p.chunks_total;                            // (chunk, hi | lo) halo pieces per tile
 
   if (tid == 0) {
     for (int s = 0; s < nslots; ++s) {
@@ -563,50 +576,54 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_halo_kernel(const __grid_c
     const int wg = warp >> 2, wq = warp & 3;
     const uint64_t d_a0 = gmma_desc_sw128(smem_u32(ring) + wg * 8 * HALO_W * 128, 16, HALO_W * 128);
     const uint64_t d_w0 = gmma_desc_sw128(smem_u32(smem), 16, 1024);
-    constexpr int NCH = BN / 32;
-    const int c_split = (NCH + 1) / 2;
-    const int c_begin = (wq >> 1) ? c_split : 0, c_end = (wq >> 1) ? NCH : c_split;
     uint8_t* my_stage = epi_stage + warp * EPI_STAGE;
     float acc[BN / 2];
     mbar_wait(w_full, 0);
     uint32_t it = 0;
+    const uint32_t wstep = static_cast<uint32_t>(p.chunks_total * 2 * W_TILE) >> 4;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      for (int pc = 0; pc < pieces; ++pc, ++it) {
-        const int slot = it % nslots;
-        const int chunk = pc >> 1, lo = pc & 1;
+      // one chunk = its hi piece, then its lo piece, in straight-line code: a data-dependent branch between the two MMA
+      // sequences makes ptxas serialize every wgmma of the kernel.  Taps are fully unrolled so that the halo shift
+      // (dy*10 + dx pixels) is an immediate, one running 64-bit add per weight slot.
+      for (int chunk = 0; chunk < p.chunks_total; ++chunk) {
+        const uint64_t dw0 = d_w0 + ((chunk * 2 * W_TILE) >> 4);
+        int slot = it % nslots;
         mbar_wait(&a_full[slot], (it / nslots) & 1);
-        // taps fully unrolled so that the halo shift (dy*10 + dx pixels) is an immediate, one running 64-bit add per
-        // weight slot, hi / lo pieces in separate loops
-        const uint64_t da = d_a0 + ((slot * HALO_SLOT) >> 4);
-        uint64_t dw = d_w0 + ((chunk * 2 * W_TILE) >> 4);
-        const uint32_t wstep = static_cast<uint32_t>(p.chunks_total * 2 * W_TILE) >> 4;
+        uint64_t da = d_a0 + ((slot * HALO_SLOT) >> 4);
+        uint64_t dw = dw0;
         wgmma_fence();
-        if (lo) {
 #pragma unroll
-          for (int tap = 0; tap < 9; ++tap, dw += wstep) {
-            const uint64_t dat = da + ((((tap / 3) * HALO_W + tap % 3) * 128) >> 4);
+        for (int tap = 0; tap < 9; ++tap, dw += wstep) {
+          const uint64_t dat = da + ((((tap / 3) * HALO_W + tap % 3) * 128) >> 4);
 #pragma unroll
-            for (int k = 0; k < BK / 16; ++k) wgmma_ss<BN, false>(acc, dat + 2 * k, dw + 2 * k, 1);      // + Al.Wh
-          }
-        } else {
-#pragma unroll
-          for (int tap = 0; tap < 9; ++tap, dw += wstep) {
-            const uint64_t dat = da + ((((tap / 3) * HALO_W + tap % 3) * 128) >> 4);
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              wgmma_ss<BN, false>(acc, dat + 2 * k, dw + (W_TILE >> 4) + 2 * k, (pc | tap | k) != 0);    // Ah.Wl
-              wgmma_ss<BN, false>(acc, dat + 2 * k, dw + 2 * k, 1);                                       // + Ah.Wh
-            }
+          for (int k = 0; k < BK / 16; ++k) {
+            wgmma_ss<BN, false>(acc, dat + 2 * k, dw + (W_TILE >> 4) + 2 * k, (chunk | tap | k) != 0);   // Ah.Wl
+            wgmma_ss<BN, false>(acc, dat + 2 * k, dw + 2 * k, 1);                                         // + Ah.Wh
           }
         }
         wgmma_commit();
-        wgmma_wait<1>();                                  // the previous piece's MMAs are done: release its slot
-        if (pc > 0 && lane == 0) mbar_arrive(&a_empty[(it - 1) % nslots]);
+        wgmma_wait<1>();                                  // the previous chunk's lo piece is done: release its slot
+        if (chunk > 0 && lane == 0) mbar_arrive(&a_empty[(it - 1) % nslots]);
+        ++it;
+
+        slot = it % nslots;
+        mbar_wait(&a_full[slot], (it / nslots) & 1);
+        da = d_a0 + ((slot * HALO_SLOT) >> 4);
+        dw = dw0;
+        wgmma_fence();
+#pragma unroll
+        for (int tap = 0; tap < 9; ++tap, dw += wstep) {
+          const uint64_t dat = da + ((((tap / 3) * HALO_W + tap % 3) * 128) >> 4);
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k) wgmma_ss<BN, false>(acc, dat + 2 * k, dw + 2 * k, 1);        // + Al.Wh
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                                  // this chunk's hi piece is done: release its slot
+        if (lane == 0) mbar_arrive(&a_empty[(it - 1) % nslots]);
+        ++it;
       }
       wgmma_wait<0>();
-      if (pieces > 0 && lane == 0) mbar_arrive(&a_empty[(it - 1) % nslots]);
-      acc_stage_store<BN>(acc_smem, acc, wg * 64 + wq * 16, lane);
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+      if (p.chunks_total > 0 && lane == 0) mbar_arrive(&a_empty[(it - 1) % nslots]);
       TileCoord t;
       t.x0 = (tile % tiles_x) * HTILE_W;
       t.y0 = ((tile / tiles_x) % tiles_y) * HTILE_H;
@@ -614,9 +631,7 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_halo_kernel(const __grid_c
       t.g = 0;
       t.co0 = 0;
       t.ph = t.oy = t.ox = 0;
-      epilogue_tile<BN>(p, t, acc_smem, wg * 64 + 32 * (wq & 1) + lane, p.Cout, bias_s, c_begin, c_end, my_stage, HTILE_W,
-                        HTILE_H);
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+      epilogue_tile<BN>(p, t, acc, wg * 64 + wq * 16, p.Cout, bias_s, my_stage, HTILE_W, HTILE_H);
     }
   }
 }
@@ -815,7 +830,7 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
       const char* e = getenv("E2F_CONV_HALO");
       return !(e && e[0] == '0');
     }();
-    const int room = SMEM_LIMIT - 1024 - 256 - MAX_COUT * 4 - halo_w_bytes(bn, chunks_all) - EPI_WARPS * EPI_STAGE - BM * bn * 4;
+    const int room = SMEM_LIMIT - 1024 - 256 - MAX_COUT * 4 - halo_w_bytes(bn, chunks_all) - EPI_WARPS * EPI_STAGE;
     if (enabled && room >= 3 * HALO_SLOT) halo_slots = room / HALO_SLOT < HALO_MAX_SLOTS ? room / HALO_SLOT : HALO_MAX_SLOTS;
   }
   const cuuint32_t estr4[4] = {1, static_cast<cuuint32_t>(stride), static_cast<cuuint32_t>(stride), 1};
@@ -896,8 +911,7 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
       return -2;
     }
     const int hgrid = htiles < num_sms() ? static_cast<int>(htiles) : num_sms();
-    const int hsmem = 1024 + halo_w_bytes(bn, chunks_all) + halo_slots * HALO_SLOT + 256 + MAX_COUT * 4 + EPI_WARPS * EPI_STAGE +
-                      BM * bn * 4;
+    const int hsmem = 1024 + halo_w_bytes(bn, chunks_all) + halo_slots * HALO_SLOT + 256 + MAX_COUT * 4 + EPI_WARPS * EPI_STAGE;
     if (bn == 32)
       conv3x3_halo_kernel<32><<<hgrid, THREADS, hsmem, stream>>>(maps, p, halo_slots);
     else

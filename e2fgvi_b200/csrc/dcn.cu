@@ -76,7 +76,20 @@ dcn_kernel(const __grid_constant__ CUtensorMap tmap_w, const __half* __restrict_
   if (warp == TMA_WARP && lane == 0) tma_prefetch_desc(&tmap_w);
   __syncthreads();
 
-  if (warp < PRODUCER_WARPS) {
+  // the TMA warp's branch comes first: with the sampler / MMA warps in the `if` branch and the TMA warp in an `else if`,
+  // ptxas serializes every wgmma of the kernel (advisory C7518, WG.DP in divergent path)
+  if (warp == TMA_WARP) {
+    // ------------------------------------------------------------------ B producer: packed weight via TMA
+    if (elect_one()) {   // one thread, chosen by elect.sync: ptxas then emits bare UTCHMMA / UTMALDG (no per-instruction ELECT loop)
+      for (int j = 0; j < NUM_KB; ++j) {
+        const int stage = j % STAGES;
+        const uint32_t phase = (j / STAGES) & 1;
+        mbar_wait(&empty[stage], phase ^ 1);
+        mbar_arrive_expect_tx(&full_b[stage], B_BYTES);
+        tma_load_2d(smem_u32(sB + stage * B_BYTES), &tmap_w, &full_b[stage], j * BLOCK_K, 0);
+      }
+    }
+  } else {
     // ------------------------------------------------------------------ A producer: sampler + im2col
     const int r = tid >> 1, s0 = 2 * (tid & 1);          // row, first of this thread's two sample points
     const long long m = static_cast<long long>(blockIdx.x) * BLOCK_M + r;
@@ -227,17 +240,6 @@ dcn_kernel(const __grid_constant__ CUtensorMap tmap_w, const __half* __restrict_
         } else {
           *reinterpret_cast<uint32_t*>(out + om * COUT + col) = pack_half2(f0, f1);
         }
-      }
-    }
-  } else if (warp == TMA_WARP) {
-    // ------------------------------------------------------------------ B producer: packed weight via TMA
-    if (elect_one()) {   // one thread, chosen by elect.sync: ptxas then emits bare UTCHMMA / UTMALDG (no per-instruction ELECT loop)
-      for (int j = 0; j < NUM_KB; ++j) {
-        const int stage = j % STAGES;
-        const uint32_t phase = (j / STAGES) & 1;
-        mbar_wait(&empty[stage], phase ^ 1);
-        mbar_arrive_expect_tx(&full_b[stage], B_BYTES);
-        tma_load_2d(smem_u32(sB + stage * B_BYTES), &tmap_w, &full_b[stage], j * BLOCK_K, 0);
       }
     }
   }

@@ -222,7 +222,7 @@ __global__ void __launch_bounds__(THREADS, 1) focal_attn_kernel(const __grid_con
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < HD / 16; ++k)
-        wgmma_n64_f16(s, (k < 4 ? dq0 : dq1) + 2 * (k & 3), dk + (k < 4 ? 0 : (KATOM >> 4)) + 2 * (k & 3), k != 0);
+        wgmma_ss<64, true>(s, (k < 4 ? dq0 : dq1) + 2 * (k & 3), dk + (k < 4 ? 0 : (KATOM >> 4)) + 2 * (k & 3), k != 0);
       wgmma_commit();
       wgmma_wait<0>();
       __syncwarp();
