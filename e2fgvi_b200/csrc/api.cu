@@ -264,13 +264,8 @@ int e2f_linear_bf16x3(const void* a_hi, const void* a_lo, const void* w_hi, cons
   if (tile_hint != 0 && tile_hint != 128 && tile_hint != 256) { set_error("e2f_linear_bf16x3: tile_hint %d", tile_hint); return E2F_ERR_BAD_ARG; }
   if (k % 8 || n % (out_dtype == E2F_F16 ? 8 : 4)) { set_error("e2f_linear_bf16x3: K %% 8 and N %% %d must be 0 (k=%d n=%d)", out_dtype == E2F_F16 ? 8 : 4, k, n); return E2F_ERR_UNSUPPORTED; }
   if (!aligned(a_hi, 16) || !aligned(a_lo, 16) || !aligned(w_hi, 16) || !aligned(w_lo, 16) || !aligned(out, 16) || (residual && !aligned(residual, 16))) { set_error("e2f_linear_bf16x3: 16-byte alignment required"); return E2F_ERR_ALIGNMENT; }
-  int bn = tile_hint;
-  if (bn == 0) {
-    // 256-wide tiles re-read A half as often; 128-wide ones only when they save more than ~15% of padded columns
-    const int t128 = (n + 127) / 128, t256 = (n + 255) / 256;
-    bn = (n < 512 || t128 * 115 < t256 * 200) ? 128 : 256;
-  }
-  return finish(launch_linear_bf16x3(a_hi, a_lo, w_hi, w_lo, bias, residual, out, m, n, k, out_dtype, bn, static_cast<cudaStream_t>(stream)), "e2f_linear_bf16x3");
+  // every tile_hint runs the ping-pong kernel's 128 x 128 tiles
+  return finish(launch_linear_bf16x3(a_hi, a_lo, w_hi, w_lo, bias, residual, out, m, n, k, out_dtype, static_cast<cudaStream_t>(stream)), "e2f_linear_bf16x3");
 }
 
 int e2f_conv2d_rows_bf16x3(int nsrc, const void* const* src_hi, const void* const* src_lo, const int* src_channels,

@@ -18,7 +18,7 @@
 //    kernel width are zero; what those positions read is finite data of the same buffer.
 //  * epilogue: + bias, LeakyReLU(slope), optional residual add, fp32 NHWC store and/or the bf16 (hi, lo) split of
 //    the result — dense NHWC or row-gapped for a following window-packed conv (the zero gaps are written here).
-// Pipeline = gemm.cu: persistent CTAs, TMA warp + two consumer warpgroups (64 accumulator rows each, fp32 in registers);
+// Pipeline: persistent CTAs, TMA warp + two consumer warpgroups (64 accumulator rows each, fp32 in registers);
 // each warp's epilogue reads its own accumulator fragments (no CTA-wide staging tile, so the pipeline gets that room).
 #include <cuda.h>
 #include <cuda_bf16.h>

@@ -70,8 +70,7 @@ int launch_t2t_fold(const float* tok, const float* bias, float* img, int bt, int
 
 int launch_split_bf16(const float* x, void* hi, void* lo, long long n, cudaStream_t stream);
 int launch_linear_bf16x3(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, const float* bias,
-                         const float* residual, void* out, int m, int n, int k, int out_dtype, int block_n,
-                         cudaStream_t stream);
+                         const float* residual, void* out, int m, int n, int k, int out_dtype, cudaStream_t stream);
 
 // Optional generalised geometry of the implicit-GEMM conv ("gather conv", see conv.cu Params): explicit tap offsets,
 // output phases and tile shape.  nullptr = the plain k x k / stride / pad conv.

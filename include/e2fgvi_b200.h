@@ -185,7 +185,8 @@ int e2f_split_bf16(const float* x, void* hi_bf16, void* lo_bf16, int64_t n, void
  * with fp32 accumulation (relative error ~2^-17; TF32 would be 2^-11).
  *   a_hi/a_lo [M][K] bf16, w_hi/w_lo [N][K] bf16 (from e2f_split_bf16), bias [N] fp32 or NULL,
  *   residual [M][N] fp32 or NULL, out [M][N] fp32 (E2F_F32) or fp16 (E2F_F16).
- *   K % 8 == 0; N % 4 == 0 (fp32 out) / N % 8 == 0 (fp16 out).  tile_hint: 0 = auto, 128 or 256 = N tile. */
+ *   K % 8 == 0; N % 4 == 0 (fp32 out) / N % 8 == 0 (fp16 out).  tile_hint: 0, 128 or 256; every value runs the
+ *   same 128 x 128 tile kernel (kept so that callers written for the former choice of N tile stay valid). */
 int e2f_linear_bf16x3(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, const float* bias,
                       const float* residual, void* out, int m, int n, int k, int out_dtype, int tile_hint,
                       void* stream);
