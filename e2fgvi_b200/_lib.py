@@ -66,6 +66,8 @@ SIGNATURES = {
     "e2f_video_compose": (_i, [_fp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "e2f_video_blend": (_i, [_vp, _vp, _vp, _fp, _i, _c.c_int64, _vp]),
     "e2f_video_finalize": (_i, [_fp, _vp, _c.c_int64, _vp]),
+    "e2f_video_resize_bicubic": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "e2f_video_prepare_masks": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "e2f_launch_count": (_c.c_int64, []),
 }
 

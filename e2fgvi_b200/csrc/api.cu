@@ -474,4 +474,34 @@ int e2f_video_finalize(const float* comp, uint8_t* out, int64_t count, void* str
   return finish(launch_video_finalize(comp, out, static_cast<long long>(count), static_cast<cudaStream_t>(stream)), "e2f_video_finalize");
 }
 
+// widest frame the bicubic resize takes: one input row is staged in shared memory
+static const int kResizeMaxWidth = 65536;
+
+int e2f_video_resize_bicubic(const uint8_t* src, uint8_t* dst, uint8_t* scratch, const int* xtab, int xtaps,
+                             const int* ytab, int ytaps, int n, int h, int w, int h2, int w2, void* stream) {
+  const char* who = "e2f_video_resize_bicubic";
+  if (!src || !dst) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if (n < 0 || h <= 0 || w <= 0 || h2 <= 0 || w2 <= 0 || w > kResizeMaxWidth || w2 > kResizeMaxWidth ||
+      static_cast<long long>(n) * (h > h2 ? h : h2) > 0x7fffffffLL) {
+    set_error("%s: bad shape n=%d %dx%d -> %dx%d (widths up to %d)", who, n, h, w, h2, w2, kResizeMaxWidth);
+    return E2F_ERR_BAD_ARG;
+  }
+  const bool horiz = w2 != w, vert = h2 != h;
+  if (horiz && (!xtab || xtaps <= 0)) { set_error("%s: width changes but xtab is null or xtaps=%d", who, xtaps); return E2F_ERR_BAD_ARG; }
+  if (vert && (!ytab || ytaps <= 0)) { set_error("%s: height changes but ytab is null or ytaps=%d", who, ytaps); return E2F_ERR_BAD_ARG; }
+  if (horiz && vert && !scratch) { set_error("%s: null scratch (both passes run)", who); return E2F_ERR_BAD_ARG; }
+  return finish(launch_video_resize_bicubic(src, dst, scratch, xtab, xtaps, ytab, ytaps, n, h, w, h2, w2, static_cast<cudaStream_t>(stream)), who);
+}
+
+int e2f_video_prepare_masks(const uint8_t* src, uint8_t* dst, const int* rows, const int* cols, int n, int hm, int wm,
+                            int h, int w, void* stream) {
+  const char* who = "e2f_video_prepare_masks";
+  if (!src || !dst || !rows || !cols) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if (n < 0 || hm <= 0 || wm <= 0 || h <= 0 || w <= 0 || (h + 31) / 32 > 65535) {
+    set_error("%s: bad shape n=%d %dx%d -> %dx%d", who, n, hm, wm, h, w);
+    return E2F_ERR_BAD_ARG;
+  }
+  return finish(launch_video_prepare_masks(src, dst, rows, cols, n, hm, wm, h, w, static_cast<cudaStream_t>(stream)), who);
+}
+
 }  // extern "C"

@@ -115,5 +115,9 @@ int launch_video_compose(const float* pred, const uint8_t* frames, const uint8_t
 int launch_video_blend(const uint8_t* img, const int* ids, const int* first, float* comp, int n_local,
                        long long frame_elems, cudaStream_t stream);
 int launch_video_finalize(const float* comp, uint8_t* out, long long count, cudaStream_t stream);
+int launch_video_resize_bicubic(const uint8_t* src, uint8_t* dst, uint8_t* scratch, const int* xtab, int xtaps,
+                                const int* ytab, int ytaps, int n, int h, int w, int h2, int w2, cudaStream_t stream);
+int launch_video_prepare_masks(const uint8_t* src, uint8_t* dst, const int* rows, const int* cols, int n, int hm,
+                               int wm, int h, int w, cudaStream_t stream);
 
 }  // namespace e2f

@@ -13,14 +13,25 @@ Windows are independent units of work (only the final blend is ordered), so
   ``all_gather`` exchanges them (uint8: 4x smaller than the fp32 predictions, SURVEY §8(e)), and every rank blends in
   schedule order.
 
+The script's front end (``resize_frames``, test.py:98-103, and ``read_mask``, :56-70) runs here too, as two byte-exact
+kernels: ``prepare_inputs`` turns decoded frames and mask planes at any size into the ``(frames, masks)`` pair
+``VideoInpainter`` takes, equal bit for bit to what test.py derives with Pillow and OpenCV.  The resample tables are
+Pillow's (checked against Pillow 12.2's ``Image.resize``; the reference pins Pillow 9.0.1, whose 8-bit resample is
+believed to be the same but is not checked here).  The horizontal pass always runs first, as in Pillow 9; recent releases
+(12.2 among them) run the vertical pass first for an image more than 100 times taller than wide, which a video frame is not.
+
 There is no CPU path: the kernels raise on CPU tensors.
 """
+import functools
+
+import numpy as np
 import torch
 
 from . import _lib
 from .ops import _need_cuda, _stream
 
 MOD_H, MOD_W = 60, 108          # test.py:157-158
+RESAMPLE_BITS = 22              # Pillow's 8-bit resample precision (libImaging/Resample.c)
 
 
 def get_ref_index(f, neighbor_ids, length, ref_length=10, num_ref=-1):
@@ -178,3 +189,166 @@ class VideoInpainter:
                 seen[i] = True
         assert all(seen), "every frame is a neighbour of some window (test.py:147-150)"
         return finalize(comp)
+
+
+# ----------------------------------------------------------------------------------------------- the front end
+def _cubic(x, a=-0.5):
+    x = abs(x)
+    if x < 1.0:
+        return ((a + 2.0) * x - (a + 3.0)) * x * x + 1
+    if x < 2.0:
+        return (((x - 5) * x + 8) * x - 4) * a
+    return 0.0
+
+
+@functools.lru_cache(maxsize=None)
+def bicubic_coeffs(n_in, n_out):
+    """Pillow's fixed-point BICUBIC filter for one axis ``n_in -> n_out``: a tuple of ``(first, (k_0, ..., k_{count-1}))``
+    per output index, the output being ``clamp((2^21 + sum_j k_j * in[first + j]) >> 22, 0, 255)``.  Double precision,
+    in the order of operations of Pillow's ``precompute_coeffs`` / ``normalize_coeffs_8bpc``."""
+    scale = n_in / n_out
+    fs = max(scale, 1.0)
+    support = 2.0 * fs
+    ss = 1.0 / fs
+    out = []
+    for i in range(n_out):
+        center = (i + 0.5) * scale
+        first = max(int(center - support + 0.5), 0)
+        count = min(int(center + support + 0.5), n_in) - first
+        w = [_cubic((j + first - center + 0.5) * ss) for j in range(count)]
+        total = 0.0
+        for v in w:
+            total += v
+        if total != 0.0:
+            w = [v / total for v in w]
+        one = 1 << RESAMPLE_BITS
+        out.append((first, tuple(int(v * one + 0.5) if v >= 0 else int(v * one - 0.5) for v in w)))
+    return tuple(out)
+
+
+@functools.lru_cache(maxsize=None)
+def nearest_index(n_in, n_out):
+    """Pillow's NEAREST source index per output index for one axis: ``v`` starts at half a step and is advanced by the
+    step in sequence (Pillow's affine scaler), not computed in closed form."""
+    step = n_in / n_out
+    v = step * 0.5
+    out = []
+    for _ in range(n_out):
+        out.append(int(v))
+        v += step
+    assert 0 <= out[0] and out[-1] < n_in, (n_in, n_out)
+    return tuple(out)
+
+
+def bicubic_table(n_in, n_out):
+    """``bicubic_coeffs`` as the kernel's int32 table ``[n_out][2 + taps]`` (first, count, k_0 .. k_{taps-1}, zero
+    padded) and ``taps``."""
+    coeffs = bicubic_coeffs(n_in, n_out)
+    taps = max(len(k) for _, k in coeffs)
+    tab = np.zeros((n_out, 2 + taps), dtype=np.int32)
+    for i, (first, k) in enumerate(coeffs):
+        tab[i, 0], tab[i, 1] = first, len(k)
+        tab[i, 2:2 + len(k)] = k
+    return tab, taps
+
+
+_DEVICE_TABLES = {}
+
+
+def _device_table(kind, n_in, n_out, device):
+    key = (kind, n_in, n_out, device)
+    if key not in _DEVICE_TABLES:
+        if kind == "bicubic":
+            tab, taps = bicubic_table(n_in, n_out)
+        else:
+            tab, taps = np.asarray(nearest_index(n_in, n_out), dtype=np.int32), 1
+        _DEVICE_TABLES[key] = (torch.from_numpy(tab).to(device), taps)
+    return _DEVICE_TABLES[key]
+
+
+def _size(size):
+    w, h = (int(v) for v in size)
+    if w <= 0 or h <= 0:
+        raise ValueError(f"size must be (width, height) > 0, got {size}")
+    return w, h
+
+
+def resize_frames(frames, size):
+    """``[Image.fromarray(f).resize(size) for f in frames]`` (test.py:98-103): uint8 RGB (N,H,W,3) on the GPU ->
+    (N,H',W',3) with ``size = (W', H')`` as in PIL, Pillow's BICUBIC, bit for bit."""
+    _need_cuda(frames)
+    if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[-1] != 3:
+        raise ValueError(f"frames must be (N,H,W,3) uint8, got {tuple(frames.shape)} {frames.dtype}")
+    w2, h2 = _size(size)
+    frames = frames.contiguous()
+    n, h, w, _ = frames.shape
+    dev = frames.device
+    out = torch.empty((n, h2, w2, 3), dtype=torch.uint8, device=dev)
+    xtab, xtaps = _device_table("bicubic", w, w2, dev) if w2 != w else (None, 0)
+    ytab, ytaps = _device_table("bicubic", h, h2, dev) if h2 != h else (None, 0)
+    scratch = torch.empty((n, h, w2, 3), dtype=torch.uint8, device=dev) if w2 != w and h2 != h else None
+    ptr = lambda t: None if t is None else t.data_ptr()
+    st = _lib.load().e2f_video_resize_bicubic(frames.data_ptr(), out.data_ptr(), ptr(scratch), ptr(xtab), xtaps,
+                                              ptr(ytab), ytaps, n, h, w, h2, w2, _stream())
+    _lib.check(st, "e2f_video_resize_bicubic")
+    return out
+
+
+def prepare_masks(masks, size):
+    """The body of test.py's ``read_mask`` after decoding: 'L' planes (N,Hm,Wm) uint8 on the GPU -> (N,H',W') uint8 in
+    {0,1}: NEAREST resize to ``size = (W', H')``, ``> 0``, ``cv2.dilate`` with a 3x3 cross 4 times."""
+    _need_cuda(masks)
+    if masks.dtype != torch.uint8 or masks.dim() != 3:
+        raise ValueError(f"masks must be (N,H,W) uint8, got {tuple(masks.shape)} {masks.dtype}")
+    w2, h2 = _size(size)
+    masks = masks.contiguous()
+    n, hm, wm = masks.shape
+    dev = masks.device
+    out = torch.empty((n, h2, w2), dtype=torch.uint8, device=dev)
+    rows, _ = _device_table("nearest", hm, h2, dev)
+    cols, _ = _device_table("nearest", wm, w2, dev)
+    st = _lib.load().e2f_video_prepare_masks(masks.data_ptr(), out.data_ptr(), rows.data_ptr(), cols.data_ptr(), n, hm,
+                                             wm, h2, w2, _stream())
+    _lib.check(st, "e2f_video_prepare_masks")
+    return out
+
+
+def _as_uint8(x, device):
+    t = torch.from_numpy(np.ascontiguousarray(x)) if isinstance(x, np.ndarray) else x
+    if t.dtype != torch.uint8:
+        raise TypeError(f"expected uint8, got {t.dtype}")
+    return t.to(device, non_blocking=True)
+
+
+def prepare_inputs(frames, masks, size=None, device=None):
+    """Decoded frames and masks -> the ``(frames, masks)`` pair ``VideoInpainter`` takes, as test.py:129-140 makes
+    them.  ``frames`` (N,H,W,3) uint8 RGB; ``masks`` the 'L' planes, as one (M,Hm,Wm) uint8 array or a sequence of
+    (Hm,Wm) planes (their sizes may differ).  Frames are resized to ``size = (W, H)`` (Pillow BICUBIC) only when
+    ``size`` is given; masks are always brought to the frames' size (NEAREST, ``> 0``, 4x cross dilation).  Extra
+    masks are ignored, as test.py ignores them; fewer masks than frames raise IndexError, where test.py does.
+    Host inputs are uploaded once; the results live on ``device`` (default: the current CUDA device)."""
+    if device is None:
+        device = frames.device if isinstance(frames, torch.Tensor) and frames.is_cuda else \
+            torch.device("cuda", torch.cuda.current_device())
+    n = len(frames)
+    if len(masks) < n:
+        raise IndexError(f"{len(masks)} masks for {n} frames (test.py indexes a mask per frame)")
+    frames = _as_uint8(frames, device)
+    if frames.dim() != 4 or frames.shape[-1] != 3:
+        raise ValueError(f"frames must be (N,H,W,3), got {tuple(frames.shape)}")
+    if size is not None:
+        frames = resize_frames(frames, size)
+    h, w = frames.shape[1:3]
+    if isinstance(masks, (np.ndarray, torch.Tensor)):
+        out = prepare_masks(_as_uint8(masks[:n], device), (w, h))
+    else:
+        planes = [_as_uint8(m, device) for m in masks[:n]]
+        out = torch.empty((n, h, w), dtype=torch.uint8, device=device)
+        i = 0
+        while i < n:                                    # runs of same-size planes -> one launch each
+            j = i + 1
+            while j < n and planes[j].shape == planes[i].shape:
+                j += 1
+            out[i:j] = prepare_masks(torch.stack(planes[i:j]), (w, h))
+            i = j
+    return frames, out

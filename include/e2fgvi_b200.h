@@ -389,6 +389,34 @@ int e2f_video_blend(const uint8_t* img, const int* ids, const int* first, float*
                     void* stream);
 int e2f_video_finalize(const float* comp, uint8_t* out, int64_t count, void* stream);
 
+/* Video front end — the frame resize and mask preparation of test.py:56-70,98-103, once per video.  Device buffers;
+ * `src` and `dst` must not overlap.
+ *
+ *   e2f_video_resize_bicubic : PIL `Image.resize((w2, h2))` of n uint8 RGB frames [n][h][w][3] -> dst [n][h2][w2][3]
+ *       with Pillow's default BICUBIC filter.  A pass whose size is unchanged is skipped; with both unchanged dst is a
+ *       copy.  Horizontal pass first, into a uint8 intermediate (`scratch` [n][h][w2][3], needed only when both passes
+ *       run; otherwise it may be NULL), then the vertical pass.  Each output byte of a pass is
+ *           clamp((2^21 + sum_{j < count} k_j * in[first + j]) >> 22, 0, 255)
+ *       in int32 with an arithmetic shift, `in` running along the pass's axis (per channel).  The per-axis table is
+ *       int32 [n_out][2 + taps]: first, count, k_0 .. k_{taps-1} (0 <= first, first + count <= n_in, count <= taps).
+ *       Pillow's tables, per axis with scale = n_in / n_out in double precision:
+ *           fs = max(scale, 1), support = 2 fs, ss = 1 / fs; for output i: center = (i + 0.5) scale,
+ *           first = max((int)(center - support + 0.5), 0), count = min((int)(center + support + 0.5), n_in) - first,
+ *           w_j = cubic((j + first - center + 0.5) ss) for j < count, w_j /= sum(w) if sum(w) != 0,
+ *           k_j = (int)(w_j 2^22 + 0.5) if w_j >= 0 else (int)(w_j 2^22 - 0.5);
+ *           cubic(x), a = -0.5: |x| < 1: ((a + 2)|x| - (a + 3))|x|^2 + 1;  |x| < 2: (((|x| - 5)|x| + 8)|x| - 4) a;  else 0.
+ *       xtab / ytab may be NULL when their axis is unchanged.  Widths up to 65536.
+ *   e2f_video_prepare_masks  : read_mask after decoding: src [n][hm][wm] uint8 (the 'L' plane) -> dst [n][h][w] in
+ *       {0, 1}: m[y][x] = src[rows[y]][cols[x]] > 0 (NEAREST), then dst = 1 iff some m within L1 distance <= 4 inside
+ *       the frame is 1 (cv2.dilate with a 3x3 MORPH_CROSS, iterations=4).  rows / cols are int32 source indices,
+ *       Pillow's NEAREST: v = (n_in / n_out) * 0.5, then for each i: idx[i] = (int)v; v += n_in / n_out (in
+ *       sequence, double precision).
+ * The arithmetic is integer / exact: results are bit-identical to Pillow's 8-bit resample and to OpenCV's dilate. */
+int e2f_video_resize_bicubic(const uint8_t* src, uint8_t* dst, uint8_t* scratch, const int* xtab, int xtaps,
+                             const int* ytab, int ytaps, int n, int h, int w, int h2, int w2, void* stream);
+int e2f_video_prepare_masks(const uint8_t* src, uint8_t* dst, const int* rows, const int* cols, int n, int hm, int wm,
+                            int h, int w, void* stream);
+
 /* Number of kernel launches issued through this library since load (all threads); used by bench.py's
  * "gpu_launches" accounting. */
 int64_t e2f_launch_count(void);
