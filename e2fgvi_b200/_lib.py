@@ -68,6 +68,13 @@ SIGNATURES = {
     "e2f_video_finalize": (_i, [_fp, _vp, _c.c_int64, _vp]),
     "e2f_video_resize_bicubic": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "e2f_video_prepare_masks": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "e2f_conv3d_bf16x3": (_i, [_vp, _vp, _i, _vp, _vp, _fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _c.POINTER(_i), _i,
+                               _vp]),
+    "e2f_i3d_stem_elems": (_c.c_int64, [_i, _i, _i, _i]),
+    "e2f_i3d_stem_pack": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "e2f_i3d_stem_conv": (_i, [_vp, _vp, _vp, _vp, _fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "e2f_maxpool3d": (_i, [_fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _c.POINTER(_i), _c.POINTER(_i), _c.POINTER(_i), _vp]),
+    "e2f_mean_thw": (_i, [_fp, _fp, _i, _i, _i, _i, _i, _vp]),
     "e2f_launch_count": (_c.c_int64, []),
 }
 

@@ -504,4 +504,81 @@ int e2f_video_prepare_masks(const uint8_t* src, uint8_t* dst, const int* rows, c
   return finish(launch_video_prepare_masks(src, dst, rows, cols, n, hm, wm, h, w, static_cast<cudaStream_t>(stream)), who);
 }
 
+// ----------------------------------------------------------------------------- I3D (VFID)
+static bool pad_ok(const int* pad, int k, int t, int h, int w) {
+  const int sz[3] = {t, h, w};
+  for (int a = 0; a < 3; ++a)
+    if (pad[2 * a] < 0 || pad[2 * a + 1] < 0 || pad[2 * a] >= k || pad[2 * a + 1] >= k ||
+        sz[a] + pad[2 * a] + pad[2 * a + 1] < k)
+      return false;
+  return true;
+}
+
+int e2f_conv3d_bf16x3(const void* src_hi, const void* src_lo, int cin, const void* w_hi, const void* w_lo, const float* bias,
+                      float* out, void* out_hi, void* out_lo, int out_cs, int b, int t, int h, int w, int cout, int ksize,
+                      const int* pad, int relu, void* stream) {
+  const char* who = "e2f_conv3d_bf16x3";
+  if (!src_hi || !src_lo || !w_hi || !w_lo || !pad) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if ((!out && !out_hi) || (!out_hi) != (!out_lo)) { set_error("%s: need out and/or both of out_hi/out_lo", who); return E2F_ERR_BAD_ARG; }
+  if (b < 0 || t <= 0 || h <= 0 || w <= 0 || cin <= 0 || cout <= 0 || cout > 512) { set_error("%s: bad shape b=%d t=%d h=%d w=%d cin=%d cout=%d", who, b, t, h, w, cin, cout); return E2F_ERR_BAD_ARG; }
+  if (cin % 8 || cout % 8 || out_cs < cout || out_cs % 8) { set_error("%s: cin, cout and out_cs must be multiples of 8 with out_cs >= cout (cin=%d cout=%d out_cs=%d)", who, cin, cout, out_cs); return E2F_ERR_UNSUPPORTED; }
+  if (ksize != 1 && ksize != 3) { set_error("%s: ksize=%d (1 or 3)", who, ksize); return E2F_ERR_UNSUPPORTED; }
+  if (!pad_ok(pad, ksize, t, h, w)) { set_error("%s: padding must be 0..ksize-1 per side and leave a non-empty output", who); return E2F_ERR_BAD_ARG; }
+  if (relu != 0 && relu != 1) { set_error("%s: relu=%d", who, relu); return E2F_ERR_BAD_ARG; }
+  if (!aligned(src_hi, 16) || !aligned(src_lo, 16) || !aligned(w_hi, 16) || !aligned(w_lo, 16) || (out && !aligned(out, 16)) ||
+      (out_hi && (!aligned(out_hi, 16) || !aligned(out_lo, 16))) || (bias && !aligned(bias, 16))) { set_error("%s: alignment (16 bytes)", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_conv3d(src_hi, src_lo, cin, 0, w_hi, w_lo, bias, out, out_hi, out_lo, out_cs, b, t, h, w, cout, ksize, 1,
+                              pad, relu ? 0.f : 1.f, static_cast<cudaStream_t>(stream)), who);
+}
+
+int64_t e2f_i3d_stem_elems(int b, int t, int h, int w) {
+  if (b < 0 || t <= 0 || h <= 0 || w <= 0) return E2F_ERR_BAD_ARG;
+  return static_cast<int64_t>(i3d_stem_elems(b, t, h, w));
+}
+
+int e2f_i3d_stem_pack(const void* x, int x_u8, void* hi, void* lo, int b, int t, int h, int w, void* stream) {
+  const char* who = "e2f_i3d_stem_pack";
+  if (!x || !hi || !lo) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if (b < 0 || t <= 0 || h <= 0 || w <= 0 || (x_u8 != 0 && x_u8 != 1)) { set_error("%s: bad shape b=%d t=%d h=%d w=%d x_u8=%d", who, b, t, h, w, x_u8); return E2F_ERR_BAD_ARG; }
+  if (!aligned(hi, 16) || !aligned(lo, 16) || (!x_u8 && !aligned(x, 4))) { set_error("%s: alignment", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_i3d_stem_pack(x, x_u8, hi, lo, b, t, h, w, static_cast<cudaStream_t>(stream)), who);
+}
+
+int e2f_i3d_stem_conv(const void* hi, const void* lo, const void* w_hi, const void* w_lo, const float* bias, float* out,
+                      void* out_hi, void* out_lo, int out_cs, int b, int t, int h, int w, int cout, void* stream) {
+  const char* who = "e2f_i3d_stem_conv";
+  if (!hi || !lo || !w_hi || !w_lo) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if ((!out && !out_hi) || (!out_hi) != (!out_lo)) { set_error("%s: need out and/or both of out_hi/out_lo", who); return E2F_ERR_BAD_ARG; }
+  if (b < 0 || t <= 0 || h <= 0 || w <= 0 || cout <= 0 || cout > 512 || cout % 8 || out_cs < cout || out_cs % 8) { set_error("%s: bad shape b=%d t=%d h=%d w=%d cout=%d out_cs=%d", who, b, t, h, w, cout, out_cs); return E2F_ERR_BAD_ARG; }
+  if (!aligned(hi, 16) || !aligned(lo, 16) || !aligned(w_hi, 16) || !aligned(w_lo, 16) || (out && !aligned(out, 16)) ||
+      (out_hi && (!aligned(out_hi, 16) || !aligned(out_lo, 16))) || (bias && !aligned(bias, 16))) { set_error("%s: alignment (16 bytes)", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_i3d_stem_conv(hi, lo, w_hi, w_lo, bias, out, out_hi, out_lo, out_cs, b, t, h, w, cout,
+                                     static_cast<cudaStream_t>(stream)), who);
+}
+
+int e2f_maxpool3d(const float* x, float* out, void* out_hi, void* out_lo, int b, int t, int h, int w, int c, const int* ksize,
+                  const int* stride, const int* pad, void* stream) {
+  const char* who = "e2f_maxpool3d";
+  if (!x || !ksize || !stride || !pad) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if ((!out && !out_hi) || (!out_hi) != (!out_lo)) { set_error("%s: need out and/or both of out_hi/out_lo", who); return E2F_ERR_BAD_ARG; }
+  if (b < 0 || t <= 0 || h <= 0 || w <= 0 || c <= 0 || c % 4 || (out_hi && c % 8)) { set_error("%s: bad shape b=%d t=%d h=%d w=%d c=%d", who, b, t, h, w, c); return E2F_ERR_BAD_ARG; }
+  const int sz[3] = {t, h, w};
+  for (int a = 0; a < 3; ++a) {
+    if (ksize[a] < 1 || ksize[a] > 3 || stride[a] < 1 || stride[a] > 2 || pad[2 * a] < 0 || pad[2 * a + 1] < 0 ||
+        pad[2 * a] >= ksize[a] || pad[2 * a + 1] >= ksize[a] || sz[a] + pad[2 * a] + pad[2 * a + 1] < ksize[a]) {
+      set_error("%s: unsupported window on axis %d (k=%d s=%d pad=%d,%d)", who, a, ksize[a], stride[a], pad[2 * a], pad[2 * a + 1]);
+      return E2F_ERR_UNSUPPORTED;
+    }
+  }
+  if (!aligned(x, 16) || (out && !aligned(out, 16)) || (out_hi && (!aligned(out_hi, 16) || !aligned(out_lo, 16)))) { set_error("%s: alignment (16 bytes)", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_i3d_maxpool(x, out, out_hi, out_lo, b, t, h, w, c, ksize, stride, pad, static_cast<cudaStream_t>(stream)), who);
+}
+
+int e2f_mean_thw(const float* x, float* out, int b, int t, int h, int w, int c, void* stream) {
+  const char* who = "e2f_mean_thw";
+  if (!x || !out) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if (b < 0 || t <= 0 || h <= 0 || w <= 0 || c <= 0) { set_error("%s: bad shape b=%d t=%d h=%d w=%d c=%d", who, b, t, h, w, c); return E2F_ERR_BAD_ARG; }
+  return finish(launch_i3d_mean(x, out, b, t, h, w, c, static_cast<cudaStream_t>(stream)), who);
+}
+
 }  // extern "C"

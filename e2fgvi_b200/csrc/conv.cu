@@ -23,6 +23,7 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cstdlib>
+#include <cstring>
 #include "common.cuh"
 #include "launch.h"
 
@@ -76,6 +77,12 @@ struct Params {
   long long osp_nstride;   // ... of the split outputs (dense: out_H * out_pitch)
   int8_t tap_dy[64], tap_dx[64];
   uint8_t ph_tap0[10], ph_oy[9], ph_ox[9];
+  // 3-D convs (the T3 instantiations, NDHWC activations): image index n = b * t_out + t over OUTPUT frames.  Dense
+  // sources: tap i also reads frame t + tap_dt[i].  Window-packed source: kt temporal taps, tap k reads frame
+  // t * tstride - tpad + k.  Frames outside [0, T) are zero-filled by the TMA unit (the conv's temporal padding).
+  int t_out, kt, tstride, tpad;
+  int8_t tap_dt[64];
+  int out_cs;              // channels per pixel of the fp32 / split outputs: Cout, or more for a channel slice
   float slope;             // LeakyReLU negative slope (1 = identity)
   int epi_flags;           // EPI_TANH: tanh after the activation; EPI_NCHW: fp32 output stored [N][Cout][out_H][out_W]
   const float* bias;
@@ -93,6 +100,14 @@ __device__ __forceinline__ void tma_load_4d(uint32_t smem_dst, const void* tmap,
   asm volatile(
       "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
       ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
+
+__device__ __forceinline__ void tma_load_5d(uint32_t smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2,
+                                            int c3, int c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
+      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
 }
 
@@ -243,7 +258,7 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
           const bool ok = map_row(row0 + (rr & 15), yy, xx);
           const uint4 u = ld_chunk(rr);
           if (ok)
-            *reinterpret_cast<uint4*>(p.out + (static_cast<size_t>(t.n) * p.out_nstride + static_cast<size_t>(yy) * p.out_W + xx) * p.Cout +
+            *reinterpret_cast<uint4*>(p.out + (static_cast<size_t>(t.n) * p.out_nstride + static_cast<size_t>(yy) * p.out_W + xx) * p.out_cs +
                                       co_chunk + 16 * (rr >> 4) + sub * 4) = u;
         }
         __syncwarp();
@@ -273,7 +288,7 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
           __nv_bfloat16* dst = rr < 16 ? p.out_hi : p.out_lo;
           if (ok)
             *reinterpret_cast<uint4*>(dst + (static_cast<size_t>(t.n) * p.osp_nstride + static_cast<size_t>(yy) * p.out_pitch + p.out_lead + xx) *
-                                            p.Cout + co_chunk + sub * 8) = u;
+                                            p.out_cs + co_chunk + sub * 8) = u;
         }
         __syncwarp();
       }
@@ -303,7 +318,7 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
             f[4] += rb.x; f[5] += rb.y; f[6] += rb.z; f[7] += rb.w;
           }
           if (p.out) {
-            float4* d4 = reinterpret_cast<float4*>(p.out + pix() * p.Cout + cb);
+            float4* d4 = reinterpret_cast<float4*>(p.out + pix() * p.out_cs + cb);
             d4[0] = make_float4(f[0], f[1], f[2], f[3]);
             d4[1] = make_float4(f[4], f[5], f[6], f[7]);
           }
@@ -317,8 +332,8 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
               hp[i] = *reinterpret_cast<const uint32_t*>(&hb);
               lp[i] = *reinterpret_cast<const uint32_t*>(&lb);
             }
-            *reinterpret_cast<uint4*>(p.out_hi + opix() * p.Cout + cb) = make_uint4(hp[0], hp[1], hp[2], hp[3]);
-            *reinterpret_cast<uint4*>(p.out_lo + opix() * p.Cout + cb) = make_uint4(lp[0], lp[1], lp[2], lp[3]);
+            *reinterpret_cast<uint4*>(p.out_hi + opix() * p.out_cs + cb) = make_uint4(hp[0], hp[1], hp[2], hp[3]);
+            *reinterpret_cast<uint4*>(p.out_lo + opix() * p.out_cs + cb) = make_uint4(lp[0], lp[1], lp[2], lp[3]);
           }
         } else if (cb < co_end) {
 #pragma unroll
@@ -333,12 +348,12 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
                 if (p.epi_flags & EPI_NCHW)   // thread = pixel: consecutive lanes write consecutive x of one channel plane
                   p.out[((static_cast<size_t>(t.n) * p.Cout + cb + i) * p.out_H + y) * p.out_W + x] = a;
                 else
-                  p.out[pix() * p.Cout + cb + i] = a;
+                  p.out[pix() * p.out_cs + cb + i] = a;
               }
               if (p.out_hi) {
                 const __nv_bfloat16 hb = __float2bfloat16_rn(a);
-                p.out_hi[opix() * p.Cout + cb + i] = hb;
-                p.out_lo[opix() * p.Cout + cb + i] = __float2bfloat16_rn(a - __bfloat162float(hb));
+                p.out_hi[opix() * p.out_cs + cb + i] = hb;
+                p.out_lo[opix() * p.out_cs + cb + i] = __float2bfloat16_rn(a - __bfloat162float(hb));
               }
             }
           }
@@ -364,7 +379,9 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
   }
 }
 
-template <int BN>
+// T3: 3-D conv over NDHWC sources through 5-D tensor maps {C, W, H, T, B} (see Params::t_out); the 2-D instantiations
+// are unchanged.
+template <int BN, bool T3>
 __global__ void __launch_bounds__(THREADS, 1) conv3x3_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p) {
   constexpr int W_TILE = Cfg<BN>::W_TILE, STAGE = Cfg<BN>::STAGE, STAGES = Cfg<BN>::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -405,6 +422,45 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_kernel(const __grid_consta
         int kb = 0;
         // bytes a stage receives: two A boxes of tile_w * tile_h rows x 128 B (rows beyond stay idle) + [Wh | Wl]
         const uint32_t stage_tx = 2u * static_cast<uint32_t>(p.tile_w * p.tile_h) * 128u + 2u * W_TILE;
+        if constexpr (T3) {
+          const int b = t.n / p.t_out, to = t.n - b * p.t_out;
+          if (p.rows_px) {
+            // window-packed K over (kt, ky, g): kt frames, ky rows, window g of the kernel row
+            for (int k = 0; k < p.kt; ++k) {
+              const int ti = to * p.tstride - p.tpad + k;
+              for (int ky = 0; ky < p.ks; ++ky) {
+                const int yy = t.y0 * p.stride - p.pad + ky;
+                for (int g = 0; g < p.rows_g; ++g, ++kb, ++it) {
+                  const int stage = it % STAGES;
+                  mbar_wait(&empty[stage], ((it / STAGES) & 1) ^ 1);
+                  mbar_arrive_expect_tx(&full[stage], stage_tx);
+                  const uint32_t s0 = smem_u32(smem + stage * STAGE);
+                  const int xi = t.x0 + g * p.rows_px / p.stride;
+                  tma_load_5d(s0, &maps.a_hi[0], &full[stage], 0, xi, yy, ti, b);
+                  tma_load_5d(s0 + A_TILE, &maps.a_lo[0], &full[stage], 0, xi, yy, ti, b);
+                  tma_load_2d(s0 + 2 * A_TILE, &maps.w_hi, &full[stage], kb * BK, t.co0);
+                  tma_load_2d(s0 + 2 * A_TILE + W_TILE, &maps.w_lo, &full[stage], kb * BK, t.co0);
+                }
+              }
+            }
+            continue;
+          }
+          const int ntap = p.ph_tap0[1];
+          for (int tap = 0; tap < ntap; ++tap) {
+            const int yy = t.y0 + p.tap_dy[tap], xx = t.x0 + p.tap_dx[tap], ti = to + p.tap_dt[tap];
+            for (int j = 0; j < p.chunks[0]; ++j, ++kb, ++it) {
+              const int stage = it % STAGES;
+              mbar_wait(&empty[stage], ((it / STAGES) & 1) ^ 1);
+              mbar_arrive_expect_tx(&full[stage], stage_tx);
+              const uint32_t s0 = smem_u32(smem + stage * STAGE);
+              tma_load_5d(s0, &maps.a_hi[0], &full[stage], j * BK, xx, yy, ti, b);
+              tma_load_5d(s0 + A_TILE, &maps.a_lo[0], &full[stage], j * BK, xx, yy, ti, b);
+              tma_load_2d(s0 + 2 * A_TILE, &maps.w_hi, &full[stage], kb * BK, t.co0);
+              tma_load_2d(s0 + 2 * A_TILE + W_TILE, &maps.w_lo, &full[stage], kb * BK, t.co0);
+            }
+          }
+          continue;
+        }
         if (p.rows_px) {
           // window-packed K: chunk (ky, g) = pixels [x*stride - pad + g*PX, +PX) x cin of input row y*stride - pad + ky
           for (int ky = 0; ky < p.ks; ++ky) {
@@ -457,6 +513,7 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_kernel(const __grid_consta
     uint32_t it = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int num_kb = p.ks * p.rows_g;                     // window-packed K
+      if constexpr (T3) num_kb *= p.kt;
       if (!p.rows_px) {
         const int ph = (tile / (tiles_ng * p.groups)) % p.nphase;
         num_kb = (p.ph_tap0[ph + 1] - p.ph_tap0[ph]) * p.chunks_total;
@@ -763,6 +820,7 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
   p.N = n; p.H = h; p.W = w; p.Cout = cout; p.groups = groups; p.nsrc = nsrc;
   p.ks = ks; p.stride = stride; p.pad = pad;
   p.slope = slope; p.bias = bias; p.residual = residual; p.out = out; p.epi_flags = epi_flags;
+  p.out_cs = cout;
   p.out_hi = static_cast<__nv_bfloat16*>(out_hi); p.out_lo = static_cast<__nv_bfloat16*>(out_lo);
   p.chunks_total = 0;
   p.rows_px = p.rows_g = 0;
@@ -886,13 +944,13 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
   static DeviceOnce configured, halo_configured;
   const int dev = current_device();
   if (!device_done(configured, dev)) {
-    cudaError_t e = cudaFuncSetAttribute(conv3x3_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<128>::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(conv3x3_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<128>::SMEM);
     if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(conv3x3_kernel<96>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<96>::SMEM);
+      e = cudaFuncSetAttribute(conv3x3_kernel<96, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<96>::SMEM);
     if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(conv3x3_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64>::SMEM);
+      e = cudaFuncSetAttribute(conv3x3_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64>::SMEM);
     if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(conv3x3_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<32>::SMEM);
+      e = cudaFuncSetAttribute(conv3x3_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<32>::SMEM);
     if (e != cudaSuccess) return static_cast<int>(e);
     device_mark(configured, dev);
   }
@@ -929,13 +987,163 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
   }
   const int grid = tiles < num_sms() ? static_cast<int>(tiles) : num_sms();
   if (bn == 32)
-    conv3x3_kernel<32><<<grid, THREADS, Cfg<32>::SMEM, stream>>>(maps, p);
+    conv3x3_kernel<32, false><<<grid, THREADS, Cfg<32>::SMEM, stream>>>(maps, p);
   else if (bn == 64)
-    conv3x3_kernel<64><<<grid, THREADS, Cfg<64>::SMEM, stream>>>(maps, p);
+    conv3x3_kernel<64, false><<<grid, THREADS, Cfg<64>::SMEM, stream>>>(maps, p);
   else if (bn == 96)
-    conv3x3_kernel<96><<<grid, THREADS, Cfg<96>::SMEM, stream>>>(maps, p);
+    conv3x3_kernel<96, false><<<grid, THREADS, Cfg<96>::SMEM, stream>>>(maps, p);
   else
-    conv3x3_kernel<128><<<grid, THREADS, Cfg<128>::SMEM, stream>>>(maps, p);
+    conv3x3_kernel<128, false><<<grid, THREADS, Cfg<128>::SMEM, stream>>>(maps, p);
+  count_launch();
+  return static_cast<int>(cudaGetLastError());
+}
+
+
+// 3-D conv (I3D's Unit3D, see i3d.cu): the generic kernel's T3 instantiation.  Dense: one NDHWC source [b][t][h][w][cin]
+// (cin % 8 == 0), ks^3 taps, stride 1, per-axis zero padding pad = {t_f, t_b, h_f, h_b, w_f, w_b}.  Window-packed
+// (in_rows = lead > 0): the stem's row-gapped source [b][t][h][pitch][4] whose rows have `lead` zero pixels in front,
+// stride 2 on every axis.  Outputs [b][t_o][h_o][w_o][out_cs] with this conv's channels at the pointers given.
+int launch_conv3d(const void* src_hi, const void* src_lo, int cin, int in_rows, const void* w_hi, const void* w_lo,
+                  const float* bias, float* out, void* out_hi, void* out_lo, int out_cs, int b, int t_in, int h_in,
+                  int w_in, int cout, int ks, int stride, const int* pad, float slope, cudaStream_t stream) {
+  using namespace conv;
+  const int t_o = (t_in + pad[0] + pad[1] - ks) / stride + 1;
+  const int h = (h_in + pad[2] + pad[3] - ks) / stride + 1;
+  const int w = (w_in + pad[4] + pad[5] - ks) / stride + 1;
+  EncodeTiledFn enc = get_encode();
+  if (!enc) {
+    set_error("cuTensorMapEncodeTiled is not available from the driver");
+    return -4;
+  }
+  int tile_w = TILE_W, tile_h = TILE_H;
+  if (w < TILE_W || h < TILE_H) {
+    tile_w = w < TILE_W ? w : TILE_W;
+    tile_h = h < TILE_H ? h : TILE_H;
+  } else if (!in_rows) {                                     // fewest tiles, as launch_conv3x3
+    long long best = static_cast<long long>((h + TILE_H - 1) / TILE_H) * ((w + TILE_W - 1) / TILE_W);
+    for (int tw = 32; tw >= 8; --tw) {
+      const int th = BM / tw;
+      if (th < 4 || th > h || tw > w) continue;
+      const long long cnt = static_cast<long long>((h + th - 1) / th) * ((w + tw - 1) / tw);
+      if (cnt < best) {
+        best = cnt;
+        tile_w = tw;
+        tile_h = th;
+      }
+    }
+  }
+  // the N tile depends on cout alone, so a video's result does not depend on the batch it is computed in
+  const int bn = cout <= 32 ? 32 : (cout <= 64 ? 64 : (cout == 96 ? 96 : 128));
+  const long long n_img = static_cast<long long>(b) * t_o;
+  Maps maps;
+  Params p;
+  memset(&p, 0, sizeof(p));
+  p.N = static_cast<int>(n_img); p.H = h; p.W = w; p.Cout = cout; p.groups = 1; p.nsrc = 1;
+  p.ks = ks; p.stride = stride; p.pad = pad[2];
+  p.t_out = t_o; p.kt = ks; p.tstride = stride; p.tpad = pad[0];
+  p.slope = slope; p.bias = bias; p.out = out; p.out_cs = out_cs;
+  p.out_hi = static_cast<__nv_bfloat16*>(out_hi); p.out_lo = static_cast<__nv_bfloat16*>(out_lo);
+  p.tile_w = tile_w; p.tile_h = tile_h;
+  p.nphase = 1; p.ostep = 1; p.out_H = h; p.out_W = w;
+  p.out_pitch = w;
+  p.out_nstride = p.osp_nstride = static_cast<long long>(h) * w;
+  const int ntaps = in_rows ? 1 : ks * ks * ks;
+  for (int i = 0; i < ntaps; ++i) {
+    p.tap_dt[i] = static_cast<int8_t>(i / (ks * ks) - pad[0]);
+    p.tap_dy[i] = static_cast<int8_t>((i / ks) % ks - pad[2]);
+    p.tap_dx[i] = static_cast<int8_t>(i % ks - pad[4]);
+  }
+  p.ph_tap0[0] = 0; p.ph_tap0[1] = static_cast<uint8_t>(ntaps);
+  const CUtensorMapDataType bf = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  int kpad;
+  if (in_rows) {
+    // 4-channel rows, dimension 1 steps by 2 pixels (16 B) and dimension 0 spans the 16-pixel window; the base is moved
+    // by lead - w_f pixels (even, so 16-byte aligned) so that window xi starts at input column 2 xi - w_f
+    const int lead = in_rows, pitch = conv_rows_pitch(w_in, lead, 4);
+    p.rows_px = BK / 4;
+    p.rows_g = (ks + p.rows_px - 1) / p.rows_px;
+    p.cig[0] = 4; p.chunks[0] = 1; p.chunks_total = 1;
+    const cuuint64_t dims[5] = {BK, static_cast<cuuint64_t>(w), static_cast<cuuint64_t>(h_in), static_cast<cuuint64_t>(t_in),
+                                static_cast<cuuint64_t>(b)};
+    const cuuint64_t strides[4] = {16, static_cast<cuuint64_t>(pitch) * 8, static_cast<cuuint64_t>(h_in) * pitch * 8,
+                                   static_cast<cuuint64_t>(t_in) * h_in * pitch * 8};
+    const cuuint32_t box[5] = {BK, static_cast<cuuint32_t>(tile_w), static_cast<cuuint32_t>(tile_h * stride), 1, 1};
+    const cuuint32_t estr[5] = {1, 1, static_cast<cuuint32_t>(stride), 1, 1};
+    for (int part = 0; part < 2; ++part) {
+      const __nv_bfloat16* base = static_cast<const __nv_bfloat16*>(part ? src_lo : src_hi) + (lead - pad[4]) * 4;
+      CUresult r = enc(part ? &maps.a_lo[0] : &maps.a_hi[0], bf, 5, const_cast<__nv_bfloat16*>(base), dims, strides, box,
+                       estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (r != CUDA_SUCCESS) {
+        set_error("conv3d: cuTensorMapEncodeTiled(row-gapped source) failed with CUresult %d", static_cast<int>(r));
+        return -4;
+      }
+    }
+    kpad = ks * ks * p.rows_g * BK;
+  } else {
+    p.cig[0] = cin; p.chunks[0] = (cin + BK - 1) / BK; p.chunks_total = p.chunks[0];
+    const cuuint64_t dims[5] = {static_cast<cuuint64_t>(cin), static_cast<cuuint64_t>(w_in), static_cast<cuuint64_t>(h_in),
+                                static_cast<cuuint64_t>(t_in), static_cast<cuuint64_t>(b)};
+    const cuuint64_t strides[4] = {static_cast<cuuint64_t>(cin) * 2, static_cast<cuuint64_t>(w_in) * cin * 2,
+                                   static_cast<cuuint64_t>(h_in) * w_in * cin * 2,
+                                   static_cast<cuuint64_t>(t_in) * h_in * w_in * cin * 2};
+    const cuuint32_t box[5] = {BK, static_cast<cuuint32_t>(tile_w), static_cast<cuuint32_t>(tile_h), 1, 1};
+    const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+    for (int part = 0; part < 2; ++part) {
+      CUresult r = enc(part ? &maps.a_lo[0] : &maps.a_hi[0], bf, 5, const_cast<void*>(part ? src_lo : src_hi), dims, strides,
+                       box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (r != CUDA_SUCCESS) {
+        set_error("conv3d: cuTensorMapEncodeTiled(source) failed with CUresult %d (c=%d w=%d h=%d t=%d b=%d)",
+                  static_cast<int>(r), cin, w_in, h_in, t_in, b);
+        return -4;
+      }
+    }
+    kpad = ntaps * p.chunks_total * BK;
+  }
+  {
+    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(kpad), static_cast<cuuint64_t>(cout)};
+    const cuuint64_t strides[1] = {static_cast<cuuint64_t>(kpad) * 2};
+    const cuuint32_t box[2] = {BK, static_cast<cuuint32_t>(bn)};
+    const cuuint32_t estr[2] = {1, 1};
+    for (int part = 0; part < 2; ++part) {
+      CUresult r = enc(part ? &maps.w_lo : &maps.w_hi, bf, 2, const_cast<void*>(part ? w_lo : w_hi), dims, strides, box,
+                       estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (r != CUDA_SUCCESS) {
+        set_error("conv3d: cuTensorMapEncodeTiled(weight) failed with CUresult %d", static_cast<int>(r));
+        return -4;
+      }
+    }
+  }
+  static DeviceOnce configured;
+  const int dev = current_device();
+  if (!device_done(configured, dev)) {
+    cudaError_t e = cudaFuncSetAttribute(conv3x3_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<128>::SMEM);
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(conv3x3_kernel<96, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<96>::SMEM);
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(conv3x3_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64>::SMEM);
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(conv3x3_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<32>::SMEM);
+    if (e != cudaSuccess) return static_cast<int>(e);
+    device_mark(configured, dev);
+  }
+  const long long tiles = n_img * ((h + tile_h - 1) / tile_h) * ((w + tile_w - 1) / tile_w) * ((cout + bn - 1) / bn);
+  if (tiles == 0) return 0;
+  if (tiles > 0x7FFFFFFFLL) {
+    set_error("conv3d: too many tiles");
+    return -2;
+  }
+  const int grid = tiles < num_sms() ? static_cast<int>(tiles) : num_sms();
+  if (bn == 32)
+    conv3x3_kernel<32, true><<<grid, THREADS, Cfg<32>::SMEM, stream>>>(maps, p);
+  else if (bn == 64)
+    conv3x3_kernel<64, true><<<grid, THREADS, Cfg<64>::SMEM, stream>>>(maps, p);
+  else if (bn == 96)
+    conv3x3_kernel<96, true><<<grid, THREADS, Cfg<96>::SMEM, stream>>>(maps, p);
+  else
+    conv3x3_kernel<128, true><<<grid, THREADS, Cfg<128>::SMEM, stream>>>(maps, p);
   count_launch();
   return static_cast<int>(cudaGetLastError());
 }

@@ -101,6 +101,18 @@ int conv_rows_pitch(int w, int lead, int channels);
 int launch_pack_rows(const float* x, void* hi, void* lo, int n, int c, int h, int w, int cin, int lead,
                      cudaStream_t stream);
 
+int launch_conv3d(const void* src_hi, const void* src_lo, int cin, int in_rows, const void* w_hi, const void* w_lo,
+                  const float* bias, float* out, void* out_hi, void* out_lo, int out_cs, int b, int t_in, int h_in,
+                  int w_in, int cout, int ks, int stride, const int* pad, float slope, cudaStream_t stream);
+constexpr int I3D_STEM_TAIL = 16;          // zero pixels after the stem operand's last row (the last window's overrun)
+long long i3d_stem_elems(int b, int t, int h, int w);
+int launch_i3d_stem_pack(const void* x, int x_u8, void* hi, void* lo, int b, int t, int h, int w, cudaStream_t stream);
+int launch_i3d_stem_conv(const void* hi, const void* lo, const void* w_hi, const void* w_lo, const float* bias, float* out,
+                         void* out_hi, void* out_lo, int out_cs, int b, int t, int h, int w, int cout, cudaStream_t stream);
+int launch_i3d_maxpool(const float* x, float* out, void* out_hi, void* out_lo, int b, int t, int h, int w, int c,
+                       const int* k, const int* s, const int* pad, cudaStream_t stream);
+int launch_i3d_mean(const float* x, float* out, int b, int t, int h, int w, int c, cudaStream_t stream);
+
 int launch_spynet_pyramid(const float* frames, float* pyr, int b, int t, int lt, int H, int W, int h, int w, int hu, int wu,
                           const float* mean3, const float* std3, cudaStream_t stream);
 int launch_spynet_level_input(const float* img, const float* prev, void* hi, void* lo, float* flow_up, int b, int lt, int hk,

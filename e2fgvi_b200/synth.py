@@ -140,3 +140,40 @@ def synth_video(n, h, w, seed=0):
         x0 = int((w - ww) * (i / max(n - 1, 1)))
         masks[i, y0:y0 + hh, x0:x0 + ww] = 1
     return frames, masks
+
+
+def synth_i3d_state_dict(seed=0):
+    """A full ``InceptionI3d`` state dict (the reference's 344 keys, CPU) with deterministic synthetic values: conv
+    weights N(0, 2 / fan_in) (He), so activations stay O(1) through the 57 ReLU layers; BatchNorm weight 1 + N(0, 0.1),
+    bias N(0, 0.1), running mean N(0, 0.1) and running var 1 + U(-0.3, 0.3), so that the host-side folding is exercised;
+    ``num_batches_tracked`` kept; the classifier's conv weight and bias N(0, 0.02)."""
+    from .i3d import InceptionI3d
+    out = {}
+    for key, t in InceptionI3d().state_dict().items():
+        shape = tuple(t.shape)
+        g = _gen(seed, "i3d:" + key)
+        leaf = key.rsplit(".", 1)[-1]
+        if not t.is_floating_point():
+            out[key] = t.detach().clone()
+        elif key.startswith("logits."):
+            out[key] = _normal(shape, 0.02, g)
+        elif ".conv3d." in key:
+            out[key] = _normal(shape, math.sqrt(2.0 / _fan_in(shape)), g)
+        elif leaf == "weight":
+            out[key] = 1.0 + _normal(shape, 0.1, g)
+        elif leaf in ("bias", "running_mean"):
+            out[key] = _normal(shape, 0.1, g)
+        elif leaf == "running_var":
+            out[key] = 1.0 + torch.empty(shape).uniform_(-0.3, 0.3, generator=g)
+        else:
+            raise KeyError(f"no synthetic rule for {key}")
+    return out
+
+
+def synth_activations(n, d, seed=0):
+    """(n, d) float64 synthetic activation rows for Fréchet-distance checks: non-negative and correlated, like I3D's
+    post-ReLU feature means."""
+    g = _gen(seed, f"activations:{n}:{d}")
+    mix = torch.randn((d, d), generator=g, dtype=torch.float64) / math.sqrt(d)
+    z = torch.randn((n, d), generator=g, dtype=torch.float64)
+    return (z @ mix + 0.5).clamp_(min=0).numpy()

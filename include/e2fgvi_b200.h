@@ -417,6 +417,43 @@ int e2f_video_resize_bicubic(const uint8_t* src, uint8_t* dst, uint8_t* scratch,
 int e2f_video_prepare_masks(const uint8_t* src, uint8_t* dst, const int* rows, const int* cols, int n, int hm, int wm,
                             int h, int w, void* stream);
 
+/* I3D — the InceptionI3d feature extractor behind evaluate.py's VFID (reference core/metrics.py:154-570).  NDHWC
+ * activations [B][T][H][W][C] contiguous; every conv runs as a wgmma implicit GEMM with the bf16 three-term split (the
+ * accuracy contract of e2f_conv2d_bf16x3: fp32-level results, fp32 accumulation).
+ *
+ * "Same" padding (the reference's compute_pad) per axis of size s, kernel k, stride st:
+ *     pad = max(k - st, 0) if s % st == 0 else max(k - s % st, 0);  front = pad / 2, back = pad - front;
+ *     output size = (s + pad - k) / st + 1 = ceil(s / st).
+ * `pad` arguments are host int[6] = {t_front, t_back, h_front, h_back, w_front, w_back}.
+ *
+ *   e2f_conv3d_bf16x3 : out = act(conv3d(x, W) + bias), ksize^3 taps (ksize 1 or 3), stride 1, zero padding `pad`
+ *       (each side < ksize); act = ReLU (relu = 1) or identity.  x = (src_hi, src_lo) bf16 [b][t][h][w][cin],
+ *       cin % 8 == 0.  W = (w_hi, w_lo) bf16 [cout][taps][ceil(cin / 64) * 64], taps in (kt, ky, kx) order, zero
+ *       columns past cin; bias fp32 [cout] or NULL.  Outputs: fp32 `out` and/or the bf16 (hi, lo) split of the result,
+ *       each [b][t_o][h_o][w_o][out_cs] with this conv's cout channels at the given pointers: a channel slice of a wider
+ *       tensor (pointer = base + channel offset; offsets multiples of 8, 16-byte aligned).  cout, out_cs % 8 == 0.
+ *   e2f_i3d_stem_elems / e2f_i3d_stem_pack / e2f_i3d_stem_conv : Conv3d_1a_7x7, 3 -> cout, 7x7x7, stride 2, same
+ *       padding on every axis.  The packed operand is (hi, lo) bf16 of e2f_i3d_stem_elems(b, t, h, w) elements each,
+ *       rows [b][t][h][pitch][4] with `lead` zero pixels in front of each row (lead = the smallest value >= both w
+ *       paddings with lead - w_front even; pitch = lead + w rounded up to even), then 16 zero pixels.  stem_pack reads
+ *       x as uint8 RGB frames [b][t][h][w][3] (x_u8 = 1; value u / 255.0f in fp32) or as the reference's fp32 input
+ *       [b][3][t][h][w] (x_u8 = 0).  stem_conv: weight [cout][7 kt][7 ky][64], chunk = 16 pixels x 4 channels of one
+ *       input row (kx < 7, channel < 3; zeros elsewhere); outputs as e2f_conv3d_bf16x3; the activation is ReLU.
+ *   e2f_maxpool3d : MaxPool3dSamePadding: x fp32 [b][t][h][w][c] -> max over each window of the ZERO-padded input
+ *       (F.pad's zeros take part in the max), windows ksize[3] <= 3 with stride[3] <= 2 and padding `pad`; fp32 `out`
+ *       and/or its bf16 split, dense [b][t_o][h_o][w_o][c].  c % 4 == 0 (% 8 with a split output).  Bit-exact.
+ *   e2f_mean_thw : out[b][c] = x.mean(W).mean(H).mean(T) of fp32 [b][t][h][w][c], in that order, deterministic. */
+int e2f_conv3d_bf16x3(const void* src_hi, const void* src_lo, int cin, const void* w_hi, const void* w_lo, const float* bias,
+                      float* out, void* out_hi, void* out_lo, int out_cs, int b, int t, int h, int w, int cout, int ksize,
+                      const int* pad, int relu, void* stream);
+int64_t e2f_i3d_stem_elems(int b, int t, int h, int w);
+int e2f_i3d_stem_pack(const void* x, int x_u8, void* hi, void* lo, int b, int t, int h, int w, void* stream);
+int e2f_i3d_stem_conv(const void* hi, const void* lo, const void* w_hi, const void* w_lo, const float* bias, float* out,
+                      void* out_hi, void* out_lo, int out_cs, int b, int t, int h, int w, int cout, void* stream);
+int e2f_maxpool3d(const float* x, float* out, void* out_hi, void* out_lo, int b, int t, int h, int w, int c, const int* ksize,
+                  const int* stride, const int* pad, void* stream);
+int e2f_mean_thw(const float* x, float* out, int b, int t, int h, int w, int c, void* stream);
+
 /* Number of kernel launches issued through this library since load (all threads); used by bench.py's
  * "gpu_launches" accounting. */
 int64_t e2f_launch_count(void);
