@@ -75,6 +75,8 @@ SIGNATURES = {
     "e2f_i3d_stem_conv": (_i, [_vp, _vp, _vp, _vp, _fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "e2f_maxpool3d": (_i, [_fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _c.POINTER(_i), _c.POINTER(_i), _c.POINTER(_i), _vp]),
     "e2f_mean_thw": (_i, [_fp, _fp, _i, _i, _i, _i, _i, _vp]),
+    "e2f_frame_metrics_work_elems": (_c.c_int64, [_i, _i, _i, _i, _i]),
+    "e2f_frame_metrics": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _c.c_double, _vp]),
     "e2f_launch_count": (_c.c_int64, []),
 }
 

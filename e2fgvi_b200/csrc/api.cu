@@ -581,4 +581,39 @@ int e2f_mean_thw(const float* x, float* out, int b, int t, int h, int w, int c, 
   return finish(launch_i3d_mean(x, out, b, t, h, w, c, static_cast<cudaStream_t>(stream)), who);
 }
 
+// ----------------------------------------------------------------------------- PSNR / SSIM (evaluate.py)
+static constexpr size_t kMetricsMaxSmem = 227 * 1024;   // sm_90 opt-in shared memory per block, static included
+
+// win = 0 asks for the SSE alone
+static long long metrics_ctas(int n, int h, int w, int c, int win) {
+  return static_cast<long long>(n) * (win ? frame_metrics_tiles(w, win) : frame_sse_blocks(h, w, c));
+}
+
+static bool metrics_shape_ok(const char* who, int n, int h, int w, int c, int win) {
+  if (n < 1 || h < 1 || w < 1 || c < 1 || c > 4) { set_error("%s: bad shape n=%d h=%d w=%d c=%d (n >= 1, 1 <= c <= 4)", who, n, h, w, c); return false; }
+  if (win != 0 && (win < 3 || !(win & 1) || win > h || win > w)) { set_error("%s: win=%d must be 0 (SSE only) or odd, >= 3 and <= min(h, w) = %d", who, win, h < w ? h : w); return false; }
+  if (metrics_ctas(n, h, w, c, win) > 0x7fffffffLL) { set_error("%s: n=%d frames of %dx%dx%d are too many for one call", who, n, h, w, c); return false; }
+  return true;
+}
+
+int64_t e2f_frame_metrics_work_elems(int n, int h, int w, int c, int win) {
+  if (!metrics_shape_ok("e2f_frame_metrics_work_elems", n, h, w, c, win)) return E2F_ERR_BAD_ARG;
+  return static_cast<int64_t>(metrics_ctas(n, h, w, c, win)) * (win ? 1 + c : 1);
+}
+
+int e2f_frame_metrics(const void* a, int a_u8, const void* b, int b_u8, double* sse, double* ssim, double* work, int n,
+                      int h, int w, int c, int win, double data_range, void* stream) {
+  const char* who = "e2f_frame_metrics";
+  if (!a || !b || !sse || (win && !ssim)) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if ((a_u8 != 0 && a_u8 != 1) || (b_u8 != 0 && b_u8 != 1)) { set_error("%s: a_u8=%d b_u8=%d (0 = fp32, 1 = uint8)", who, a_u8, b_u8); return E2F_ERR_BAD_ARG; }
+  if (!metrics_shape_ok(who, n, h, w, c, win)) return E2F_ERR_BAD_ARG;
+  if (!(data_range > 0.0) || data_range > 1e300) { set_error("%s: data_range=%g must be > 0 and finite", who, data_range); return E2F_ERR_BAD_ARG; }
+  if (!work) { set_error("%s: null workspace (e2f_frame_metrics_work_elems doubles needed)", who); return E2F_ERR_BAD_ARG; }
+  if (win && frame_metrics_smem(c, win) > kMetricsMaxSmem) { set_error("%s: win=%d with c=%d needs %zu bytes of shared memory (at most %zu)", who, win, c, frame_metrics_smem(c, win), kMetricsMaxSmem); return E2F_ERR_UNSUPPORTED; }
+  if ((!a_u8 && !aligned(a, 4)) || (!b_u8 && !aligned(b, 4)) || !aligned(sse, 8) || (ssim && !aligned(ssim, 8)) || !aligned(work, 8)) { set_error("%s: alignment (fp32 operands 4 bytes, outputs and workspace 8)", who); return E2F_ERR_ALIGNMENT; }
+  if (!win) return finish(launch_frame_sse(a, a_u8, b, b_u8, sse, work, n, h, w, c, static_cast<cudaStream_t>(stream)), who);
+  return finish(launch_frame_metrics(a, a_u8, b, b_u8, sse, ssim, work, n, h, w, c, win, data_range,
+                                     static_cast<cudaStream_t>(stream)), who);
+}
+
 }  // extern "C"

@@ -113,6 +113,14 @@ int launch_i3d_maxpool(const float* x, float* out, void* out_hi, void* out_lo, i
                        const int* k, const int* s, const int* pad, cudaStream_t stream);
 int launch_i3d_mean(const float* x, float* out, int b, int t, int h, int w, int c, cudaStream_t stream);
 
+int frame_metrics_tiles(int w, int win);
+size_t frame_metrics_smem(int c, int win);            // all of the kernel's shared memory (dynamic; no static)
+long long frame_sse_blocks(int h, int w, int c);
+int launch_frame_sse(const void* a, int a_u8, const void* b, int b_u8, double* sse, double* work, int n, int h, int w,
+                     int c, cudaStream_t stream);
+int launch_frame_metrics(const void* a, int a_u8, const void* b, int b_u8, double* sse, double* ssim, double* work,
+                         int n, int h, int w, int c, int win, double data_range, cudaStream_t stream);
+
 int launch_spynet_pyramid(const float* frames, float* pyr, int b, int t, int lt, int H, int W, int h, int w, int hu, int wu,
                           const float* mean3, const float* std3, cudaStream_t stream);
 int launch_spynet_level_input(const float* img, const float* prev, void* hi, void* lo, float* flow_up, int b, int lt, int hk,

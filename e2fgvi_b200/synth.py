@@ -177,3 +177,52 @@ def synth_activations(n, d, seed=0):
     mix = torch.randn((d, d), generator=g, dtype=torch.float64) / math.sqrt(d)
     z = torch.randn((n, d), generator=g, dtype=torch.float64)
     return (z @ mix + 0.5).clamp_(min=0).numpy()
+
+
+def synth_composite_pair(h, w, c, seed, holes=True):
+    """A uint8 frame and an evaluate.py-like composite: multiples of 1/4, equal to the frame outside the holes."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    ori = rng.integers(0, 256, (h, w, c), dtype=np.uint8)
+    comp = ori.astype(np.float32)
+    if holes:
+        y0, x0 = h // 4, w // 3
+        quarters = rng.integers(0, 255 * 4 + 1, (h // 2, w // 3, c)).astype(np.float32) / 4
+        comp[y0:y0 + h // 2, x0:x0 + w // 3] = quarters
+    return ori, comp
+
+
+def write_eval_dataset(root, videos, size=(54, 96), drop_mask=None):
+    """A DAVIS-layout dataset as evaluate.py reads it: R/davis/{test.json, JPEGImages/<v>.zip, test_masks/<v>/%05d.png}.
+    Zip members are PNG (lossless: decoding does not depend on the OpenCV build); masks are at frame size and, as
+    DAVIS's, palette images (index 1 = hole, colour (128, 0, 0)); the holes are the top quarter of ``synth_video``'s
+rectangles.  ``videos``: name -> frame count; video k comes from
+    ``synth_video(n, *size, seed=40 + k)``.  Returns R and {name: (frames, masks)}."""
+    import json
+    import os
+    import zipfile
+    import cv2
+    import numpy as np
+    from PIL import Image
+    data = os.path.join(root, "davis")
+    os.makedirs(os.path.join(data, "JPEGImages"))
+    with open(os.path.join(data, "test.json"), "w") as f:
+        json.dump(videos, f)
+    out = {}
+    for k, (name, n) in enumerate(videos.items()):
+        frames, masks = synth_video(n, *size, seed=40 + k)
+        for m in masks:                                   # the top quarter of each rectangle: small goldens
+            rows = np.nonzero(m.any(1))[0]
+            m[rows[0] + (len(rows) + 3) // 4:] = 0
+        with zipfile.ZipFile(os.path.join(data, "JPEGImages", f"{name}.zip"), "w") as z:
+            for i in range(n):
+                z.writestr(f"{i:05d}.png", cv2.imencode(".png", cv2.cvtColor(frames[i], cv2.COLOR_RGB2BGR))[1].tobytes())
+        mdir = os.path.join(data, "test_masks", name)
+        os.makedirs(mdir)
+        for i in range(n):
+            if (name, i) != drop_mask:
+                im = Image.fromarray(masks[i], mode="P")
+                im.putpalette([0, 0, 0, 128, 0, 0] + [0] * 762)
+                im.save(os.path.join(mdir, f"{i:05d}.png"))
+        out[name] = (frames, masks)
+    return root, out

@@ -140,8 +140,14 @@ class VideoInpainter:
                                  "test.py:45-46 lets get_ref_index reach video_length when num_ref != -1)")
         return sched
 
-    @torch.no_grad()
     def __call__(self, frames, masks, device=None):
+        return finalize(self.composite(frames, masks, device))
+
+    @torch.no_grad()
+    def composite(self, frames, masks, device=None):
+        """The blended composite before test.py:195's uint8 truncation: (N,H,W,3) float32 on the GPU.  A frame that
+        several windows touch holds their 0.5/0.5 float32 blend (at most three windows with the default stride, so
+        every value is a multiple of 1/4); evaluate.py computes PSNR and SSIM on this, VFID on its truncation."""
         device = torch.device(device) if device is not None else (
             frames.device if frames.is_cuda else torch.device("cuda", torch.cuda.current_device()))
         if frames.dtype != torch.uint8 or masks.dtype != torch.uint8:
@@ -188,7 +194,7 @@ class VideoInpainter:
             for i in nb:
                 seen[i] = True
         assert all(seen), "every frame is a neighbour of some window (test.py:147-150)"
-        return finalize(comp)
+        return comp
 
 
 # ----------------------------------------------------------------------------------------------- the front end

@@ -454,6 +454,27 @@ int e2f_maxpool3d(const float* x, float* out, void* out_hi, void* out_lo, int b,
                   const int* stride, const int* pad, void* stream);
 int e2f_mean_thw(const float* x, float* out, int b, int t, int h, int w, int c, void* stream);
 
+/* Per-frame PSNR and SSIM inputs of evaluate.py (reference core/metrics.py:20-54).  `a` and `b` are device images
+ * [n][h][w][c], each uint8 (flag 1) or fp32 (flag 0).  Per frame f:
+ *   sse[f]  = sum over the frame of (a - b)^2 in fp64;
+ *   ssim[f] = skimage 0.16.2 compare_ssim(a[f], b[f], data_range, multichannel=True, win_size=win) with the uniform
+ *             window and sample covariance: per channel, with u = (window sum) / win^2 of x, y, x^2, y^2, xy,
+ *             k = win^2 / (win^2 - 1), C1 = (0.01 data_range)^2, C2 = (0.03 data_range)^2,
+ *                 S = (2 ux uy + C1) (2 k (uxy - ux uy) + C2) / ((ux^2 + uy^2 + C1) (k (uxx - ux^2) + k (uyy - uy^2) + C2)),
+ *             averaged over the (h - win + 1) x (w - win + 1) windows inside the frame (skimage's crop of (win - 1) / 2
+ *             removes exactly the windows that touch its reflect padding), then over the channels.
+ * For uint8 operands and for values that are multiples of 1/4 (evaluate.py's blended composite) every window sum and
+ * every SSE is exact in fp64 (multiples of 1/16 below 2^43, 1080p included), so the SSE is exact and the box means are
+ * correctly rounded.  Deterministic: per-CTA partials are added in a fixed order, no atomics.
+ * win = 0 computes the SSE alone (any h, w >= 1; `ssim` may be NULL and is not written).
+ * `work` is a device workspace of e2f_frame_metrics_work_elems(n, h, w, c, win) doubles (negative = bad arguments);
+ * sse / ssim are device fp64 [n].  Requires n >= 1, 1 <= c <= 4, win = 0 or odd with 3 <= win <= min(h, w),
+ * data_range > 0; the window's shared memory, 80 c (win + 255) + 320 c bytes, must fit 227 KB (win <= 709 at c = 3,
+ * win <= 467 at c = 4; E2F_ERR_UNSUPPORTED otherwise). */
+int64_t e2f_frame_metrics_work_elems(int n, int h, int w, int c, int win);
+int e2f_frame_metrics(const void* a, int a_u8, const void* b, int b_u8, double* sse, double* ssim, double* work, int n,
+                      int h, int w, int c, int win, double data_range, void* stream);
+
 /* Number of kernel launches issued through this library since load (all threads); used by bench.py's
  * "gpu_launches" accounting. */
 int64_t e2f_launch_count(void);
