@@ -77,6 +77,10 @@ SIGNATURES = {
     "e2f_mean_thw": (_i, [_fp, _fp, _i, _i, _i, _i, _i, _vp]),
     "e2f_frame_metrics_work_elems": (_c.c_int64, [_i, _i, _i, _i, _i]),
     "e2f_frame_metrics": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _c.c_double, _vp]),
+    "e2f_dis_conv3d": (_i, [_vp, _vp, _i, _vp, _vp, _fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "e2f_dis_conv3d_dgrad": (_i, [_vp, _vp, _i, _vp, _vp, _fp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "e2f_dis_conv3d_wgrad_work_elems": (_c.c_int64, [_i, _i, _i, _i, _i, _i, _i]),
+    "e2f_dis_conv3d_wgrad": (_i, [_fp, _vp, _vp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "e2f_launch_count": (_c.c_int64, []),
 }
 

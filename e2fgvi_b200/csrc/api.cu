@@ -616,4 +616,67 @@ int e2f_frame_metrics(const void* a, int a_u8, const void* b, int b_u8, double* 
                                      static_cast<cudaStream_t>(stream)), who);
 }
 
+// ----------------------------------------------------------------------------- Temporal PatchGAN discriminator
+static int dis_out_size(int s, int pad) { return (s + 2 * pad - 5) / 2 + 1; }
+
+static bool dis_shape_ok(const char* who, int b, int t, int h_in, int w_in, int pad) {
+  if (b < 1 || t < 1 || h_in + 2 * pad < 5 || w_in + 2 * pad < 5 || (pad != 1 && pad != 2) || dis_out_size(h_in, pad) < 1 ||
+      dis_out_size(w_in, pad) < 1 || static_cast<long long>(b) * t > 0x7fffffffLL) {
+    set_error("%s: bad shape b=%d t=%d h=%d w=%d pad=%d (a 5x5 window at stride 2 needs h, w >= %d)", who, b, t, h_in, w_in,
+              pad, 5 - 2 * pad);
+    return false;
+  }
+  return true;
+}
+
+int e2f_dis_conv3d(const void* x_hi, const void* x_lo, int cin, const void* w_hi, const void* w_lo, const float* bias,
+                   float* out, void* out_hi, void* out_lo, int b, int t, int h_in, int w_in, int cout, int pad, int leaky,
+                   void* stream) {
+  const char* who = "e2f_dis_conv3d";
+  if (!x_hi || !x_lo || !w_hi || !w_lo) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if ((!out && !out_hi) || (!out_hi) != (!out_lo)) { set_error("%s: need out and/or both of out_hi/out_lo", who); return E2F_ERR_BAD_ARG; }
+  if (!dis_shape_ok(who, b, t, h_in, w_in, pad)) return E2F_ERR_BAD_ARG;
+  if (cin < 8 || cin % 8 || cout < 8 || cout % 8 || cout > 128) { set_error("%s: cin=%d must be a multiple of 8, cout=%d a multiple of 8 <= 128", who, cin, cout); return E2F_ERR_UNSUPPORTED; }
+  if (leaky != 0 && leaky != 1) { set_error("%s: leaky=%d", who, leaky); return E2F_ERR_BAD_ARG; }
+  if (!aligned(x_hi, 16) || !aligned(x_lo, 16) || !aligned(w_hi, 16) || !aligned(w_lo, 16) || (out && !aligned(out, 16)) ||
+      (out_hi && (!aligned(out_hi, 16) || !aligned(out_lo, 16))) || (bias && !aligned(bias, 16))) { set_error("%s: alignment (16 bytes)", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_dis_conv(x_hi, x_lo, cin, w_hi, w_lo, bias, out, out_hi, out_lo, b, t, h_in, w_in, dis_out_size(h_in, pad),
+                                dis_out_size(w_in, pad), cout, pad, 0, leaky ? 0.2f : 1.f, nullptr, 0.f,
+                                static_cast<cudaStream_t>(stream)), who);
+}
+
+int e2f_dis_conv3d_dgrad(const void* dy_hi, const void* dy_lo, int cout, const void* wt_hi, const void* wt_lo, float* dx,
+                         void* dx_hi, void* dx_lo, const void* act, int b, int t, int h_in, int w_in, int cin, int pad,
+                         void* stream) {
+  const char* who = "e2f_dis_conv3d_dgrad";
+  if (!dy_hi || !dy_lo || !wt_hi || !wt_lo) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if ((!dx && !dx_hi) || (!dx_hi) != (!dx_lo)) { set_error("%s: need dx and/or both of dx_hi/dx_lo", who); return E2F_ERR_BAD_ARG; }
+  if (!dis_shape_ok(who, b, t, h_in, w_in, pad)) return E2F_ERR_BAD_ARG;
+  if (cout < 8 || cout % 8 || cin < 8 || cin % 8 || cin > 128) { set_error("%s: cout=%d must be a multiple of 8, cin=%d a multiple of 8 <= 128", who, cout, cin); return E2F_ERR_UNSUPPORTED; }
+  if (!aligned(dy_hi, 16) || !aligned(dy_lo, 16) || !aligned(wt_hi, 16) || !aligned(wt_lo, 16) || (dx && !aligned(dx, 16)) ||
+      (dx_hi && (!aligned(dx_hi, 16) || !aligned(dx_lo, 16))) || (act && !aligned(act, 16))) { set_error("%s: alignment (16 bytes)", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_dis_conv(dy_hi, dy_lo, cout, wt_hi, wt_lo, nullptr, dx, dx_hi, dx_lo, b, t, dis_out_size(h_in, pad),
+                                dis_out_size(w_in, pad), h_in, w_in, cin, pad, 1, 1.f, act, 0.2f,
+                                static_cast<cudaStream_t>(stream)), who);
+}
+
+int64_t e2f_dis_conv3d_wgrad_work_elems(int b, int t, int h_in, int w_in, int cin, int cout, int pad) {
+  if (!dis_shape_ok("e2f_dis_conv3d_wgrad_work_elems", b, t, h_in, w_in, pad)) return E2F_ERR_BAD_ARG;
+  if (cin < 8 || cin % 8 || cin > 512 || cout < 8 || cout % 8 || cout > 512) { set_error("e2f_dis_conv3d_wgrad_work_elems: cin=%d cout=%d (multiples of 8, <= 512)", cin, cout); return E2F_ERR_BAD_ARG; }
+  return static_cast<int64_t>(dis_wgrad_work_elems(b, t, dis_out_size(h_in, pad), dis_out_size(w_in, pad), cout, cin));
+}
+
+int e2f_dis_conv3d_wgrad(const float* dy, const void* x_hi, const void* x_lo, float* dw, float* db, float* work, int b,
+                         int t, int h_in, int w_in, int cin, int cout, int pad, void* stream) {
+  const char* who = "e2f_dis_conv3d_wgrad";
+  if (!dy || !x_hi || !x_lo || !dw) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if (!dis_shape_ok(who, b, t, h_in, w_in, pad)) return E2F_ERR_BAD_ARG;
+  if (cin < 8 || cin % 8 || cin > 512 || cout < 8 || cout % 8 || cout > 512) { set_error("%s: cin=%d cout=%d (multiples of 8, <= 512)", who, cin, cout); return E2F_ERR_BAD_ARG; }
+  if (!work) { set_error("%s: null workspace (e2f_dis_conv3d_wgrad_work_elems floats needed)", who); return E2F_ERR_BAD_ARG; }
+  if (!aligned(dy, 16) || !aligned(x_hi, 16) || !aligned(x_lo, 16) || !aligned(dw, 4) || (db && !aligned(db, 4)) ||
+      !aligned(work, 4)) { set_error("%s: alignment (dy, x_hi, x_lo 16 bytes)", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_dis_wgrad(dy, x_hi, x_lo, dw, db, work, b, t, h_in, w_in, cin, dis_out_size(h_in, pad),
+                                 dis_out_size(w_in, pad), cout, pad, static_cast<cudaStream_t>(stream)), who);
+}
+
 }  // extern "C"

@@ -38,6 +38,7 @@ constexpr int MAX_COUT = 512;                            // bias staged in share
 constexpr int EPI_STAGE = 2048;                          // per epilogue warp: 32 rows x 64 bytes store-transposition buffer
 constexpr int THREADS = (EPI_WARPS + 1) * 32;                // + the TMA warp
 constexpr int MAX_SRC = 4;
+constexpr int MAX_TAPS = 80;                             // the discriminator's 3x5x5 kernels list 75 taps
 
 // N tile: 128 output channels; 64 / 32 for the layers with <= 64 / <= 32 output channels per group (decoder, encoder
 // conv 1, SPyNet, the 3-channel output conv), which would otherwise waste most of every MMA; 96 for the encoder's
@@ -75,13 +76,13 @@ struct Params {
   int nphase, ostep, out_H, out_W;
   long long out_nstride;   // pixels between consecutive images of the fp32 output / residual (dense: out_H * out_W)
   long long osp_nstride;   // ... of the split outputs (dense: out_H * out_pitch)
-  int8_t tap_dy[64], tap_dx[64];
+  int8_t tap_dy[MAX_TAPS], tap_dx[MAX_TAPS];
   uint8_t ph_tap0[10], ph_oy[9], ph_ox[9];
   // 3-D convs (the T3 instantiations, NDHWC activations): image index n = b * t_out + t over OUTPUT frames.  Dense
   // sources: tap i also reads frame t + tap_dt[i].  Window-packed source: kt temporal taps, tap k reads frame
   // t * tstride - tpad + k.  Frames outside [0, T) are zero-filled by the TMA unit (the conv's temporal padding).
   int t_out, kt, tstride, tpad;
-  int8_t tap_dt[64];
+  int8_t tap_dt[MAX_TAPS];
   int out_cs;              // channels per pixel of the fp32 / split outputs: Cout, or more for a channel slice
   float slope;             // LeakyReLU negative slope (1 = identity)
   int epi_flags;           // EPI_TANH: tanh after the activation; EPI_NCHW: fp32 output stored [N][Cout][out_H][out_W]
@@ -91,6 +92,11 @@ struct Params {
   float* out;              // NHWC fp32 or null
   __nv_bfloat16* out_hi;   // NHWC bf16 split of the result (operand format of the next conv) or null
   __nv_bfloat16* out_lo;
+  // T3 only: derivative of the LeakyReLU(dact_slope) that produced `dact` (bf16 [N][out_H][out_W][Cout], the hi part of
+  // the saved activation).  The result is multiplied by 1 where dact > 0, else by dact_slope (LeakyReLU keeps the sign
+  // of its input, so its output decides).  Null: no multiply.
+  const __nv_bfloat16* dact;
+  float dact_slope;
 };
 
 constexpr int EPI_TANH = 1, EPI_NCHW = 2;     // both only on the element-wise store path (Cout % 4 != 0: the 3-channel output conv)
@@ -153,7 +159,7 @@ __device__ __forceinline__ TileCoord decode_tile(int tile, const Params& p, int 
 //     pixel row p, row 16 + p = the 32 lo channels), and 4 consecutive lanes then store one buffer row: 64 contiguous
 //     bytes of one pixel.
 // Chunks that are not 32 full, 16-byte-aligned channels take the direct path.
-template <int BN>
+template <int BN, bool T3 = false>
 __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& t, const float* acc, int row0, int cog,
                                               const float* __restrict__ bias_s, uint8_t* __restrict__ stage, const int TW,
                                               const int TH) {
@@ -210,6 +216,19 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
         for (int i = 0; i < 4; ++i) {
           const float a = __uint_as_float(v[g4 * 4 + i]) + bb[i];
           f[g4 * 4 + i] = a > 0.f ? a : a * p.slope;
+        }
+      }
+      if constexpr (T3) {
+        if (p.dact && pix_ok) {
+          const uint4* d4 = reinterpret_cast<const uint4*>(p.dact + pix() * p.Cout + co);
+#pragma unroll
+          for (int h8 = 0; h8 < 2; ++h8) {
+            const uint4 u = __ldg(d4 + h8);
+            const __nv_bfloat16* m = reinterpret_cast<const __nv_bfloat16*>(&u);
+#pragma unroll
+            for (int i = 0; i < 8; ++i)
+              if (!(__bfloat162float(m[i]) > 0.f)) f[h8 * 8 + i] *= p.dact_slope;
+          }
         }
       }
       if (p.residual && pix_ok) {
@@ -305,6 +324,15 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
             const float a = __uint_as_float(v[g8 * 8 + i]) + bb[i];
             f[i] = a > 0.f ? a : a * p.slope;
           }
+          if constexpr (T3) {
+            if (p.dact) {
+              const uint4 u = __ldg(reinterpret_cast<const uint4*>(p.dact + pix() * p.Cout + cb));
+              const __nv_bfloat16* m = reinterpret_cast<const __nv_bfloat16*>(&u);
+#pragma unroll
+              for (int i = 0; i < 8; ++i)
+                if (!(__bfloat162float(m[i]) > 0.f)) f[i] *= p.dact_slope;
+            }
+          }
           if (p.residual) {
             const float4* r4 = reinterpret_cast<const float4*>(p.residual + pix() * p.Cout + cb);
             const float4 ra = __ldg(r4), rb = __ldg(r4 + 1);
@@ -341,6 +369,9 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
             if (cb + i < co_end) {
               float a = __uint_as_float(v[g8 * 8 + i]) + bias_s[cb + i];
               a = a > 0.f ? a : a * p.slope;
+              if constexpr (T3) {
+                if (p.dact && !(__bfloat162float(p.dact[pix() * p.Cout + cb + i]) > 0.f)) a *= p.dact_slope;
+              }
               if (p.residual) a += __ldg(p.residual + pix() * p.Cout + cb + i);
               if (p.bias_map) a += __ldg(p.bias_map + mpix() * p.Cout + cb + i);
               if (p.epi_flags & EPI_TANH) a = tanhf(a);
@@ -445,9 +476,11 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_kernel(const __grid_consta
             }
             continue;
           }
-          const int ntap = p.ph_tap0[1];
-          for (int tap = 0; tap < ntap; ++tap) {
-            const int yy = t.y0 + p.tap_dy[tap], xx = t.x0 + p.tap_dx[tap], ti = to + p.tap_dt[tap];
+          // taps of this tile's phase; (y, x) steps by `stride` (the TMA box is traversed with that element stride)
+          const int tap0 = p.ph_tap0[t.ph], tap1 = p.ph_tap0[t.ph + 1];
+          kb = tap0 * p.chunks[0];
+          for (int tap = tap0; tap < tap1; ++tap) {
+            const int yy = t.y0 * p.stride + p.tap_dy[tap], xx = t.x0 * p.stride + p.tap_dx[tap], ti = to + p.tap_dt[tap];
             for (int j = 0; j < p.chunks[0]; ++j, ++kb, ++it) {
               const int stage = it % STAGES;
               mbar_wait(&empty[stage], ((it / STAGES) & 1) ^ 1);
@@ -538,7 +571,7 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_kernel(const __grid_consta
       wgmma_wait<0>();
       if (num_kb > 0 && lane == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
       const TileCoord t = decode_tile<BN>(tile, p, tiles_y, tiles_x, tiles_ng);
-      epilogue_tile<BN>(p, t, acc, wg * 64 + wq * 16, cog, bias_s, my_stage, p.tile_w, p.tile_h);
+      epilogue_tile<BN, T3>(p, t, acc, wg * 64 + wq * 16, cog, bias_s, my_stage, p.tile_w, p.tile_h);
     }
   }
 }
@@ -1142,6 +1175,153 @@ int launch_conv3d(const void* src_hi, const void* src_lo, int cin, int in_rows, 
     conv3x3_kernel<64, true><<<grid, THREADS, Cfg<64>::SMEM, stream>>>(maps, p);
   else if (bn == 96)
     conv3x3_kernel<96, true><<<grid, THREADS, Cfg<96>::SMEM, stream>>>(maps, p);
+  else
+    conv3x3_kernel<128, true><<<grid, THREADS, Cfg<128>::SMEM, stream>>>(maps, p);
+  count_launch();
+  return static_cast<int>(cudaGetLastError());
+}
+
+// Temporal PatchGAN discriminator layers (Conv3d 3x5x5, stride (1, 2, 2), padding (1, pad, pad)): the T3 kernel with a
+// 75-tap table.  One NDHWC source [b][t][h_src][w_src][cin] (cin % 8 == 0; channels past the weight's are ignored).
+//  * forward (transposed = 0): out[b][t][h_out][w_out][cout], h_out = (h_src + 2 pad - 5) / 2 + 1; the source boxes are
+//    traversed with element stride 2 in y and x.  Tap (kt, ky, kx) reads frame t + kt - 1, row 2y + ky - pad, column
+//    2x + kx - pad; weight [cout][75 taps in (kt, ky, kx) order][ceil(cin / 64) * 64].
+//  * input gradient (transposed = 1): the source is dY of the forward conv and the output dX [b][t][h_out][w_out][cout]
+//    (h_out, w_out = the forward's input size).  Output pixel (2gy + oy, 2gx + ox) is phase ph = 2 oy + ox; it gathers
+//    the taps with ky = oy + pad (mod 2), kx = ox + pad (mod 2), reading dY at (t + 1 - kt, gy + (oy + pad - ky) / 2,
+//    gx + (ox + pad - kx) / 2) with stride 1.  Taps are listed phase by phase, each phase in (kt, ky, kx) order, and
+//    the weight [cout][75][ceil(cin / 64) * 64] follows that order.  Rows the forward never read get 0.
+// `dact` (or null): the epilogue multiplies by LeakyReLU(dact_slope)'s derivative at that saved activation.
+int launch_dis_conv(const void* src_hi, const void* src_lo, int cin, const void* w_hi, const void* w_lo, const float* bias,
+                    float* out, void* out_hi, void* out_lo, int b, int t, int h_src, int w_src, int h_out, int w_out,
+                    int cout, int pad, int transposed, float slope, const void* dact, float dact_slope, cudaStream_t stream) {
+  using namespace conv;
+  constexpr int KT = 3, KS = 5;
+  EncodeTiledFn enc = get_encode();
+  if (!enc) {
+    set_error("cuTensorMapEncodeTiled is not available from the driver");
+    return -4;
+  }
+  const int stride = transposed ? 1 : 2;
+  const int h = transposed ? (h_out + 1) / 2 : h_out, w = transposed ? (w_out + 1) / 2 : w_out;   // GEMM grid per phase
+  int tile_w = TILE_W, tile_h = TILE_H;
+  if (w < TILE_W || h < TILE_H) {
+    tile_w = w < TILE_W ? w : TILE_W;
+    tile_h = h < TILE_H ? h : TILE_H;
+  } else {                                                   // fewest tiles, as launch_conv3x3
+    long long best = static_cast<long long>((h + TILE_H - 1) / TILE_H) * ((w + TILE_W - 1) / TILE_W);
+    for (int tw = 32; tw >= 8; --tw) {
+      const int th = BM / tw;
+      if (th < 4 || th > h || tw > w) continue;
+      const long long cnt = static_cast<long long>((h + th - 1) / th) * ((w + tw - 1) / tw);
+      if (cnt < best) {
+        best = cnt;
+        tile_w = tw;
+        tile_h = th;
+      }
+    }
+  }
+  const int bn = cout <= 32 ? 32 : (cout <= 64 ? 64 : 128);
+  const long long n_img = static_cast<long long>(b) * t;
+  Maps maps;
+  Params p;
+  memset(&p, 0, sizeof(p));
+  p.N = static_cast<int>(n_img); p.H = h; p.W = w; p.Cout = cout; p.groups = 1; p.nsrc = 1;
+  p.ks = KS; p.stride = stride; p.pad = pad;
+  p.t_out = t; p.kt = KT; p.tstride = 1; p.tpad = 1;
+  p.slope = slope; p.bias = bias; p.out = out; p.out_cs = cout;
+  p.out_hi = static_cast<__nv_bfloat16*>(out_hi); p.out_lo = static_cast<__nv_bfloat16*>(out_lo);
+  p.dact = static_cast<const __nv_bfloat16*>(dact); p.dact_slope = dact_slope;
+  p.tile_w = tile_w; p.tile_h = tile_h;
+  p.out_H = h_out; p.out_W = w_out; p.out_pitch = w_out;
+  p.out_nstride = p.osp_nstride = static_cast<long long>(h_out) * w_out;
+  int ntaps = 0;
+  if (!transposed) {
+    p.nphase = 1; p.ostep = 1;
+    for (int kt = 0; kt < KT; ++kt)
+      for (int ky = 0; ky < KS; ++ky)
+        for (int kx = 0; kx < KS; ++kx, ++ntaps) {
+          p.tap_dt[ntaps] = static_cast<int8_t>(kt - 1);
+          p.tap_dy[ntaps] = static_cast<int8_t>(ky - pad);
+          p.tap_dx[ntaps] = static_cast<int8_t>(kx - pad);
+        }
+    p.ph_tap0[0] = 0;
+  } else {
+    p.nphase = 4; p.ostep = 2;
+    for (int ph = 0; ph < 4; ++ph) {
+      const int oy = ph >> 1, ox = ph & 1;
+      p.ph_tap0[ph] = static_cast<uint8_t>(ntaps); p.ph_oy[ph] = static_cast<uint8_t>(oy); p.ph_ox[ph] = static_cast<uint8_t>(ox);
+      for (int kt = 0; kt < KT; ++kt)
+        for (int ky = 0; ky < KS; ++ky)
+          for (int kx = 0; kx < KS; ++kx) {
+            if (((oy + pad - ky) & 1) || ((ox + pad - kx) & 1)) continue;
+            p.tap_dt[ntaps] = static_cast<int8_t>(1 - kt);
+            p.tap_dy[ntaps] = static_cast<int8_t>((oy + pad - ky) / 2);
+            p.tap_dx[ntaps] = static_cast<int8_t>((ox + pad - kx) / 2);
+            ++ntaps;
+          }
+    }
+  }
+  p.ph_tap0[p.nphase] = static_cast<uint8_t>(ntaps);
+  const CUtensorMapDataType bf = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  p.cig[0] = cin; p.chunks[0] = (cin + BK - 1) / BK; p.chunks_total = p.chunks[0];
+  {
+    const cuuint64_t dims[5] = {static_cast<cuuint64_t>(cin), static_cast<cuuint64_t>(w_src), static_cast<cuuint64_t>(h_src),
+                                static_cast<cuuint64_t>(t), static_cast<cuuint64_t>(b)};
+    const cuuint64_t strides[4] = {static_cast<cuuint64_t>(cin) * 2, static_cast<cuuint64_t>(w_src) * cin * 2,
+                                   static_cast<cuuint64_t>(h_src) * w_src * cin * 2,
+                                   static_cast<cuuint64_t>(t) * h_src * w_src * cin * 2};
+    const cuuint32_t box[5] = {BK, static_cast<cuuint32_t>(tile_w * stride), static_cast<cuuint32_t>(tile_h * stride), 1, 1};
+    const cuuint32_t estr[5] = {1, static_cast<cuuint32_t>(stride), static_cast<cuuint32_t>(stride), 1, 1};
+    for (int part = 0; part < 2; ++part) {
+      CUresult r = enc(part ? &maps.a_lo[0] : &maps.a_hi[0], bf, 5, const_cast<void*>(part ? src_lo : src_hi), dims, strides,
+                       box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (r != CUDA_SUCCESS) {
+        set_error("dis_conv: cuTensorMapEncodeTiled(source) failed with CUresult %d (c=%d w=%d h=%d t=%d b=%d)",
+                  static_cast<int>(r), cin, w_src, h_src, t, b);
+        return -4;
+      }
+    }
+  }
+  {
+    const int kpad = ntaps * p.chunks_total * BK;
+    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(kpad), static_cast<cuuint64_t>(cout)};
+    const cuuint64_t strides[1] = {static_cast<cuuint64_t>(kpad) * 2};
+    const cuuint32_t box[2] = {BK, static_cast<cuuint32_t>(bn)};
+    const cuuint32_t estr[2] = {1, 1};
+    for (int part = 0; part < 2; ++part) {
+      CUresult r = enc(part ? &maps.w_lo : &maps.w_hi, bf, 2, const_cast<void*>(part ? w_lo : w_hi), dims, strides, box,
+                       estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (r != CUDA_SUCCESS) {
+        set_error("dis_conv: cuTensorMapEncodeTiled(weight) failed with CUresult %d", static_cast<int>(r));
+        return -4;
+      }
+    }
+  }
+  static DeviceOnce configured;
+  const int dev = current_device();
+  if (!device_done(configured, dev)) {
+    cudaError_t e = cudaFuncSetAttribute(conv3x3_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<128>::SMEM);
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(conv3x3_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64>::SMEM);
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(conv3x3_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<32>::SMEM);
+    if (e != cudaSuccess) return static_cast<int>(e);
+    device_mark(configured, dev);
+  }
+  const long long tiles = n_img * ((h + tile_h - 1) / tile_h) * ((w + tile_w - 1) / tile_w) * p.nphase * ((cout + bn - 1) / bn);
+  if (tiles == 0) return 0;
+  if (tiles > 0x7FFFFFFFLL) {
+    set_error("dis_conv: too many tiles");
+    return -2;
+  }
+  const int grid = tiles < num_sms() ? static_cast<int>(tiles) : num_sms();
+  if (bn == 32)
+    conv3x3_kernel<32, true><<<grid, THREADS, Cfg<32>::SMEM, stream>>>(maps, p);
+  else if (bn == 64)
+    conv3x3_kernel<64, true><<<grid, THREADS, Cfg<64>::SMEM, stream>>>(maps, p);
   else
     conv3x3_kernel<128, true><<<grid, THREADS, Cfg<128>::SMEM, stream>>>(maps, p);
   count_launch();

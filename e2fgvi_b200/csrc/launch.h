@@ -104,6 +104,13 @@ int launch_pack_rows(const float* x, void* hi, void* lo, int n, int c, int h, in
 int launch_conv3d(const void* src_hi, const void* src_lo, int cin, int in_rows, const void* w_hi, const void* w_lo,
                   const float* bias, float* out, void* out_hi, void* out_lo, int out_cs, int b, int t_in, int h_in,
                   int w_in, int cout, int ks, int stride, const int* pad, float slope, cudaStream_t stream);
+int launch_dis_conv(const void* src_hi, const void* src_lo, int cin, const void* w_hi, const void* w_lo, const float* bias,
+                    float* out, void* out_hi, void* out_lo, int b, int t, int h_src, int w_src, int h_out, int w_out,
+                    int cout, int pad, int transposed, float slope, const void* dact, float dact_slope, cudaStream_t stream);
+int dis_wgrad_slices(int b, int t, int h_o, int w_o, int cout, int cin);
+long long dis_wgrad_work_elems(int b, int t, int h_o, int w_o, int cout, int cin);
+int launch_dis_wgrad(const float* dy, const void* x_hi, const void* x_lo, float* dw, float* db, float* work, int b, int t,
+                     int h_in, int w_in, int cin, int h_o, int w_o, int cout, int pad, cudaStream_t stream);
 constexpr int I3D_STEM_TAIL = 16;          // zero pixels after the stem operand's last row (the last window's overrun)
 long long i3d_stem_elems(int b, int t, int h, int w);
 int launch_i3d_stem_pack(const void* x, int x_u8, void* hi, void* lo, int b, int t, int h, int w, cudaStream_t stream);

@@ -1301,3 +1301,102 @@ def note_graph_replay(kernel_launches):
 def launch_count():
     """Kernels of this library launched so far: host-side launches (``e2f_launch_count``) + kernels replayed by graphs."""
     return int(_lib.load().e2f_launch_count()) + _GRAPH_REPLAY_LAUNCHES
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Temporal PatchGAN discriminator layers (model/e2fgvi.py:271-344): Conv3d, kernel (3, 5, 5), stride (1, 2, 2), zero
+# padding (1, pad, pad).  Activations are NDHWC; see include/e2fgvi_b200.h for the operand layouts.
+def dis_out_size(s, pad):
+    return (s + 2 * pad - 5) // 2 + 1
+
+
+def dis_dgrad_taps(pad):
+    """Tap order of the input-gradient weight: phase by phase (ph = 2 (y % 2) + x % 2), taps 25 kt + 5 ky + kx with
+    ky = y + pad and kx = x + pad (mod 2) in increasing order."""
+    taps = []
+    for ph in range(4):
+        oy, ox = ph >> 1, ph & 1
+        taps += [25 * kt + 5 * ky + kx for kt in range(3) for ky in range(5) for kx in range(5)
+                 if (oy + pad - ky) % 2 == 0 and (ox + pad - kx) % 2 == 0]
+    return taps
+
+
+def dis_pack_weight(weight, cin_s):
+    """fp32 [cout, cin, 3, 5, 5] -> bf16 (hi, lo) [cout, 75 * ceil(cin_s / 64) * 64] in tap-major K order."""
+    cout, cin = weight.shape[:2]
+    kc = -(-cin_s // 64) * 64
+    p = weight.detach().float().permute(0, 2, 3, 4, 1).reshape(cout, 75, cin)
+    p = torch.nn.functional.pad(p, (0, kc - cin))
+    return split_bf16(p.reshape(cout, 75 * kc))
+
+
+def dis_pack_weight_t(weight, pad, cin_s):
+    """fp32 [cout, cin, 3, 5, 5] -> the input gradient's bf16 (hi, lo) [cin_s, 75 * ceil(cout / 64) * 64]: flipped
+    roles (rows = input channels, zero rows past cin), taps in dis_dgrad_taps(pad) order."""
+    cout, cin = weight.shape[:2]
+    kc = -(-cout // 64) * 64
+    idx = torch.tensor(dis_dgrad_taps(pad), device=weight.device)
+    p = weight.detach().float().permute(1, 2, 3, 4, 0).reshape(cin, 75, cout).index_select(1, idx)
+    p = torch.nn.functional.pad(p, (0, kc - cout, 0, 0, 0, cin_s - cin))
+    return split_bf16(p.reshape(cin_s, 75 * kc))
+
+
+def dis_conv3d(x_hi, x_lo, w_hi, w_lo, bias, cout, pad, leaky):
+    """One discriminator conv on the split operand x [b, t, h, w, cin]: returns (fp32 out, out_hi, out_lo), each
+    [b, t, h_o, w_o, cout], with LeakyReLU(0.2) fused when ``leaky``."""
+    _need_cuda(x_hi, x_lo, w_hi, w_lo, bias)
+    b, t, h, w, cin = x_hi.shape
+    ho, wo = dis_out_size(h, pad), dis_out_size(w, pad)
+    out = torch.empty(b, t, ho, wo, cout, dtype=torch.float32, device=x_hi.device)
+    hi = torch.empty(out.shape, dtype=torch.bfloat16, device=x_hi.device)
+    lo = torch.empty_like(hi)
+    with _timed(f"dis_conv3d_c{cout}", 2.0 * b * t * ho * wo * cout * cin * 75):
+        st = _lib.load().e2f_dis_conv3d(x_hi.data_ptr(), x_lo.data_ptr(), cin, w_hi.data_ptr(), w_lo.data_ptr(),
+                                        None if bias is None else bias.data_ptr(), out.data_ptr(), hi.data_ptr(),
+                                        lo.data_ptr(), b, t, h, w, cout, pad, 1 if leaky else 0, _stream())
+    _lib.check(st, "e2f_dis_conv3d")
+    return out, hi, lo
+
+
+def dis_conv3d_dgrad(dy_hi, dy_lo, wt_hi, wt_lo, act, h_in, w_in, cin_s, pad, split=False):
+    """Input gradient fp32 [b, t, h_in, w_in, cin_s] of a discriminator conv from the split dy [b, t, h_o, w_o, cout];
+    times LeakyReLU(0.2)'s derivative at ``act`` (bf16, the hi part of the layer's input) unless ``act`` is None.
+    Returns (dx, dx_hi, dx_lo); the bf16 split, the next input gradient's operand, only when ``split``."""
+    _need_cuda(dy_hi, dy_lo, wt_hi, wt_lo, act)
+    b, t, _, _, cout = dy_hi.shape
+    dx = torch.empty(b, t, h_in, w_in, cin_s, dtype=torch.float32, device=dy_hi.device)
+    hi = lo = None
+    if split:
+        hi = torch.empty(dx.shape, dtype=torch.bfloat16, device=dx.device)
+        lo = torch.empty_like(hi)
+    with _timed(f"dis_dgrad_c{cin_s}", 2.0 * b * t * dy_hi.shape[2] * dy_hi.shape[3] * cout * cin_s * 75):
+        st = _lib.load().e2f_dis_conv3d_dgrad(dy_hi.data_ptr(), dy_lo.data_ptr(), cout, wt_hi.data_ptr(), wt_lo.data_ptr(),
+                                              dx.data_ptr(), None if hi is None else hi.data_ptr(),
+                                              None if lo is None else lo.data_ptr(),
+                                              None if act is None else act.data_ptr(), b, t, h_in, w_in, cin_s, pad,
+                                              _stream())
+    _lib.check(st, "e2f_dis_conv3d_dgrad")
+    return dx, hi, lo
+
+
+def dis_conv3d_wgrad(dy, x_hi, x_lo, cin, pad, with_bias):
+    """(dW fp32 [cout, cin, 3, 5, 5], db fp32 [cout] or None) of a discriminator conv from dy fp32 [b, t, h_o, w_o,
+    cout] and the forward's split operand x [b, t, h, w, x_cs]: the kernel computes all x_cs channels (the padded
+    ones are zero) and the first ``cin`` are returned."""
+    _need_cuda(dy, x_hi, x_lo)
+    lib = _lib.load()
+    dy = dy.contiguous()
+    b, t, h, w, cs = x_hi.shape
+    cout = dy.shape[-1]
+    elems = lib.e2f_dis_conv3d_wgrad_work_elems(b, t, h, w, cs, cout, pad)
+    if elems < 0:
+        _lib.check(int(elems), "e2f_dis_conv3d_wgrad_work_elems")
+    work = torch.empty(int(elems), dtype=torch.float32, device=dy.device)
+    dw = torch.empty(cout, cs, 3, 5, 5, dtype=torch.float32, device=dy.device)
+    db = torch.empty(cout, dtype=torch.float32, device=dy.device) if with_bias else None
+    with _timed(f"dis_wgrad_c{cout}", 2.0 * dy.numel() * cs * 75):
+        st = lib.e2f_dis_conv3d_wgrad(dy.data_ptr(), x_hi.data_ptr(), x_lo.data_ptr(), dw.data_ptr(),
+                                      None if db is None else db.data_ptr(), work.data_ptr(), b, t, h, w, cs, cout, pad,
+                                      _stream())
+    _lib.check(st, "e2f_dis_conv3d_wgrad")
+    return (dw if cin == cs else dw[:, :cin].contiguous()), db

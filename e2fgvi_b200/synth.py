@@ -226,3 +226,32 @@ rectangles.  ``videos``: name -> frame count; video k comes from
                 im.save(os.path.join(mdir, f"{i:05d}.png"))
         out[name] = (frames, masks)
     return root, out
+
+
+def synth_dis_state_dict(seed=0, use_spectral_norm=True, in_channels=3):
+    """State dict of ``Discriminator(in_channels, use_spectral_norm=...)`` with deterministic values: fan-in-scaled
+    weights (activations stay O(1) through the six layers), small biases, and under spectral norm ``weight_u`` /
+    ``weight_v`` from ten power iterations on the weight."""
+    chans = (in_channels, 32, 64, 128, 128, 128, 128)
+    sd = {}
+    for i in range(6):
+        cout, cin = chans[i + 1], chans[i]
+        shape = (cout, cin, 3, 5, 5)
+        w = _normal(shape, math.sqrt(2.0 / _fan_in(shape)), _gen(seed, f"dis.{i}.w"))
+        p = f"conv.{2 * i}."
+        if i < 5 and use_spectral_norm:
+            sd[p + "weight_orig"] = w
+            # near the top singular pair (as after some training), so that eval()-mode sigma is not arbitrarily small
+            u = _normal((cout,), 1.0, _gen(seed, f"dis.{i}.u")).double()
+            wm = w.double().reshape(cout, -1)
+            for _ in range(10):
+                v = wm.t() @ u
+                v = v / v.norm()
+                u = wm @ v
+                u = u / u.norm()
+            sd[p + "weight_u"] = u.float()
+            sd[p + "weight_v"] = v.float()
+        else:
+            sd[p + "weight"] = w
+            sd[p + "bias"] = _normal((cout,), 0.1, _gen(seed, f"dis.{i}.b"))
+    return sd

@@ -475,6 +475,37 @@ int64_t e2f_frame_metrics_work_elems(int n, int h, int w, int c, int win);
 int e2f_frame_metrics(const void* a, int a_u8, const void* b, int b_u8, double* sse, double* ssim, double* work, int n,
                       int h, int w, int c, int win, double data_range, void* stream);
 
+/* Temporal PatchGAN discriminator (reference model/e2fgvi.py:271-344): Conv3d layers with kernel (3, 5, 5), stride
+ * (1, 2, 2) and zero padding (1, pad, pad), pad 1 or 2.  Activations are NDHWC [b][t][h][w][c]; h_in, w_in are the
+ * layer's INPUT size and h_o = (h_in + 2 pad - 5) / 2 + 1 (w_o likewise) its output size.  Operands are bf16 (hi, lo)
+ * splits with fp32 accumulation (the accuracy contract of e2f_conv2d_bf16x3).  Taps are numbered (kt, ky, kx) with
+ * tap = 25 kt + 5 ky + kx.
+ *   e2f_dis_conv3d : out = act(conv3d(x, W) + bias), act = LeakyReLU(0.2) (leaky = 1) or identity.  x [b][t][h_in][w_in]
+ *       [cin], cin % 8 == 0 (zero-pad the 3-channel image to 8).  W [cout][75 taps][ceil(cin / 64) * 64], zero columns
+ *       past the real input channels; bias fp32 [cout] or NULL.  Outputs: fp32 `out` and/or its split, [b][t][h_o][w_o]
+ *       [cout], cout % 8 == 0, cout <= 128.
+ *   e2f_dis_conv3d_dgrad : input gradient dx [b][t][h_in][w_in][cin] of that conv from dy = (dy_hi, dy_lo)
+ *       [b][t][h_o][w_o][cout], computed as four output phases (y % 2, x % 2).  Phase ph = 2 (y % 2) + (x % 2) uses the
+ *       taps with ky = y + pad and kx = x + pad (mod 2), in increasing tap order; Wt [cin][75][ceil(cout / 64) * 64]
+ *       lists phase 0's taps, then phase 1's, ... with Wt[ci][k][co] = W[co][ci][tap k].  If `act` (bf16 [b][t][h_in]
+ *       [w_in][cin], the hi part of the LeakyReLU(0.2) output that fed the conv) is given, dx is multiplied by that
+ *       LeakyReLU's derivative: 1 where act > 0, else 0.2.  Outputs: fp32 dx and/or its split.  cin % 8 == 0, <= 128.
+ *   e2f_dis_conv3d_wgrad_work_elems / e2f_dis_conv3d_wgrad : dw fp32 [cout][cin][3][5][5] (the torch layout) and, if
+ *       db is not NULL, db fp32 [cout] = the sum of dy over pixels, from dy fp32 [b][t][h_o][w_o][cout] and the forward's
+ *       operand x = (x_hi, x_lo) [b][t][h_in][w_in][cin]; cin, cout % 8 == 0 (channels the forward zero-padded get
+ *       their own, zero-valued, gradient).  wgmma with the bf16 three-term split of dy and x and fp32 accumulation.  K
+ *       (the pixels) is split over CTAs into `work` (device fp32, e2f_dis_conv3d_wgrad_work_elems(...) elements;
+ *       negative = bad arguments) and the slices are added in a fixed order: bit-identical from run to run. */
+int e2f_dis_conv3d(const void* x_hi, const void* x_lo, int cin, const void* w_hi, const void* w_lo, const float* bias,
+                   float* out, void* out_hi, void* out_lo, int b, int t, int h_in, int w_in, int cout, int pad, int leaky,
+                   void* stream);
+int e2f_dis_conv3d_dgrad(const void* dy_hi, const void* dy_lo, int cout, const void* wt_hi, const void* wt_lo, float* dx,
+                         void* dx_hi, void* dx_lo, const void* act, int b, int t, int h_in, int w_in, int cin, int pad,
+                         void* stream);
+int64_t e2f_dis_conv3d_wgrad_work_elems(int b, int t, int h_in, int w_in, int cin, int cout, int pad);
+int e2f_dis_conv3d_wgrad(const float* dy, const void* x_hi, const void* x_lo, float* dw, float* db, float* work, int b,
+                         int t, int h_in, int w_in, int cin, int cout, int pad, void* stream);
+
 /* Number of kernel launches issued through this library since load (all threads); used by bench.py's
  * "gpu_launches" accounting. */
 int64_t e2f_launch_count(void);
