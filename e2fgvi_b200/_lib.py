@@ -55,6 +55,9 @@ SIGNATURES = {
     "e2f_spynet_pyramid": (_i, [_fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _fp, _fp, _vp]),
     "e2f_spynet_level_input": (_i, [_fp, _fp, _vp, _vp, _fp, _i, _i, _i, _i, _i, _vp]),
     "e2f_spynet_final": (_i, [_fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _vp]),
+    "e2f_spynet_pyramid_unit": (_i, [_fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _fp, _fp, _vp]),
+    "e2f_spynet_level_input_backward": (_i, [_fp, _fp, _fp, _fp, _fp, _i, _i, _i, _i, _vp]),
+    "e2f_spynet_final_backward": (_i, [_fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _vp]),
     "e2f_peer_alloc": (_i, [_c.c_size_t, _c.POINTER(_c.c_void_p), _c.c_char_p]),
     "e2f_peer_open": (_i, [_c.c_char_p, _c.POINTER(_c.c_void_p)]),
     "e2f_peer_close": (_i, [_vp]),
@@ -81,6 +84,9 @@ SIGNATURES = {
     "e2f_dis_conv3d_dgrad": (_i, [_vp, _vp, _i, _vp, _vp, _fp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "e2f_dis_conv3d_wgrad_work_elems": (_c.c_int64, [_i, _i, _i, _i, _i, _i, _i]),
     "e2f_dis_conv3d_wgrad": (_i, [_fp, _vp, _vp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "e2f_conv2d_dgrad_bf16x3": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _i, _fp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "e2f_conv2d_wgrad_work_elems": (_c.c_int64, [_i, _i, _i, _i, _i]),
+    "e2f_conv2d_wgrad_bf16x3": (_i, [_fp, _vp, _vp, _i, _fp, _fp, _fp, _i, _i, _i, _i, _i, _vp]),
     "e2f_launch_count": (_c.c_int64, []),
 }
 

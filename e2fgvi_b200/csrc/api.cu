@@ -444,6 +444,33 @@ int e2f_spynet_final(const float* flow, float* flows_forward, float* flows_backw
   return finish(launch_spynet_final(flow, flows_forward, flows_backward, b, l_t, h, w, h_up, w_up, static_cast<cudaStream_t>(stream)), who);
 }
 
+int e2f_spynet_pyramid_unit(const float* frames, float* pyramid, int b, int t, int l_t, int H, int W, int h, int w, int h_up,
+                            int w_up, const float* mean3, const float* std3, void* stream) {
+  const char* who = "e2f_spynet_pyramid_unit";
+  if (!frames || !pyramid || !mean3 || !std3) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if (b < 0 || t <= 0 || l_t <= 0 || l_t > t || H <= 0 || W <= 0 || h <= 1 || w <= 1 || h > H || w > W) { set_error("%s: bad shape b=%d t=%d l_t=%d %dx%d -> %dx%d", who, b, t, l_t, H, W, h, w); return E2F_ERR_BAD_ARG; }
+  if (h_up < h || w_up < w || h_up % 32 || w_up % 32) { set_error("%s: the working size %dx%d must be multiples of 32 >= %dx%d", who, h_up, w_up, h, w); return E2F_ERR_BAD_ARG; }
+  return finish(launch_spynet_pyramid_unit(frames, pyramid, b, t, l_t, H, W, h, w, h_up, w_up, mean3, std3, static_cast<cudaStream_t>(stream)), who);
+}
+
+int e2f_spynet_level_input_backward(const float* d_in, const float* dflow, const float* level_img, const float* flow_up,
+                                    float* dprev, int b, int l_t, int hk, int wk, void* stream) {
+  const char* who = "e2f_spynet_level_input_backward";
+  if (!d_in || !dflow || !level_img || !flow_up || !dprev) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if (b < 0 || l_t < 2 || hk < 2 || wk < 2 || ((hk | wk) & 1)) { set_error("%s: bad shape b=%d l_t=%d %dx%d (even sizes >= 2)", who, b, l_t, hk, wk); return E2F_ERR_BAD_ARG; }
+  if (!aligned(d_in, 4) || !aligned(dflow, 8) || !aligned(flow_up, 8) || !aligned(dprev, 8)) { set_error("%s: alignment (dflow, flow_up, dprev 8 bytes)", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_spynet_level_input_backward(d_in, dflow, level_img, flow_up, dprev, b, l_t, hk, wk, static_cast<cudaStream_t>(stream)), who);
+}
+
+int e2f_spynet_final_backward(const float* d_forward, const float* d_backward, float* dflow, int b, int l_t, int h, int w,
+                              int h_up, int w_up, void* stream) {
+  const char* who = "e2f_spynet_final_backward";
+  if (!d_forward || !d_backward || !dflow) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if (b < 0 || l_t < 2 || h <= 0 || w <= 0 || h_up < h || w_up < w) { set_error("%s: bad shape", who); return E2F_ERR_BAD_ARG; }
+  if (!aligned(dflow, 8)) { set_error("%s: dflow needs 8-byte alignment", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_spynet_final_backward(d_forward, d_backward, dflow, b, l_t, h, w, h_up, w_up, static_cast<cudaStream_t>(stream)), who);
+}
+
 int e2f_video_prepare_clip(const uint8_t* frames, const uint8_t* masks, const int* ids, float* out, int t, int h, int w,
                            int hp, int wp, void* stream) {
   if (!frames || !masks || !ids || !out) { set_error("e2f_video_prepare_clip: null pointer"); return E2F_ERR_BAD_ARG; }
@@ -677,6 +704,47 @@ int e2f_dis_conv3d_wgrad(const float* dy, const void* x_hi, const void* x_lo, fl
       !aligned(work, 4)) { set_error("%s: alignment (dy, x_hi, x_lo 16 bytes)", who); return E2F_ERR_ALIGNMENT; }
   return finish(launch_dis_wgrad(dy, x_hi, x_lo, dw, db, work, b, t, h_in, w_in, cin, dis_out_size(h_in, pad),
                                  dis_out_size(w_in, pad), cout, pad, static_cast<cudaStream_t>(stream)), who);
+}
+
+static bool rows_c(int c) { return c == 4 || c == 8 || c == 16 || c == 32; }
+
+int e2f_conv2d_dgrad_bf16x3(const void* dy_hi, const void* dy_lo, int dy_c, int dy_lead, const void* wt_hi, const void* wt_lo,
+                            const void* act, int act_lead, float* dx, void* dx_hi, void* dx_lo, int dx_lead, int n, int h,
+                            int w, int cin, void* stream) {
+  const char* who = "e2f_conv2d_dgrad_bf16x3";
+  if (!dy_hi || !dy_lo || !wt_hi || !wt_lo) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if ((!dx && !dx_hi) || (!dx_hi) != (!dx_lo)) { set_error("%s: need dx and/or both of dx_hi/dx_lo", who); return E2F_ERR_BAD_ARG; }
+  if (n < 0 || h <= 0 || w <= 0) { set_error("%s: bad shape n=%d h=%d w=%d", who, n, h, w); return E2F_ERR_BAD_ARG; }
+  if (dy_lead != 0 && dy_lead != 3) { set_error("%s: dy_lead=%d (0: dense, 3: row-gapped for the 7x7 / pad 3 conv)", who, dy_lead); return E2F_ERR_BAD_ARG; }
+  if (act_lead < 0 || act_lead > 8 || dx_lead < 0 || dx_lead > 8 || (dx_lead && !dx_hi)) { set_error("%s: act_lead=%d dx_lead=%d (0..8; a row-gapped dx needs the split)", who, act_lead, dx_lead); return E2F_ERR_BAD_ARG; }
+  // row-gapped: the tensor map steps one pixel per row element, a 16-byte multiple from 8 channels on
+  if (dy_lead ? (!rows_c(dy_c) || dy_c < 8) : (dy_c < 8 || dy_c % 8)) { set_error("%s: dy_c=%d (row-gapped: 8, 16 or 32; dense: a multiple of 8)", who, dy_c); return E2F_ERR_UNSUPPORTED; }
+  if (cin < 8 || cin % 8 || cin > 64 || ((dx_lead || act_lead) && !rows_c(cin))) { set_error("%s: cin=%d (a multiple of 8 <= 64; 8, 16 or 32 when dx or act is row-gapped)", who, cin); return E2F_ERR_UNSUPPORTED; }
+  if (!aligned(dy_hi, 16) || !aligned(dy_lo, 16) || !aligned(wt_hi, 16) || !aligned(wt_lo, 16) || (dx && !aligned(dx, 16)) ||
+      (dx_hi && (!aligned(dx_hi, 16) || !aligned(dx_lo, 16))) || (act && !aligned(act, 16))) { set_error("%s: alignment (16 bytes)", who); return E2F_ERR_ALIGNMENT; }
+  if (n == 0) return 0;
+  const void* srch[1] = {dy_hi};
+  const void* srcl[1] = {dy_lo};
+  const int ch[1] = {dy_c};
+  return finish(launch_conv3x3(1, srch, srcl, ch, wt_hi, wt_lo, nullptr, nullptr, dx, dx_hi, dx_lo, n, h, w, cin, 1, 1.f, 7,
+                               1, 3, dy_lead ? 1 : 0, dx_lead, static_cast<cudaStream_t>(stream), nullptr, 0, act, act_lead), who);
+}
+
+int64_t e2f_conv2d_wgrad_work_elems(int n, int h, int w, int cin, int cout) {
+  if (n < 0 || h <= 0 || w <= 0 || cin < 8 || cin % 8 || cin > 512 || cout < 8 || cout % 8 || cout > 512) { set_error("e2f_conv2d_wgrad_work_elems: n=%d %dx%d cin=%d cout=%d (multiples of 8, <= 512)", n, h, w, cin, cout); return E2F_ERR_BAD_ARG; }
+  return static_cast<int64_t>(conv2d_wgrad_work_elems(n, h, w, cin, cout));
+}
+
+int e2f_conv2d_wgrad_bf16x3(const float* dy, const void* x_hi, const void* x_lo, int x_lead, float* dw, float* db, float* work,
+                            int n, int h, int w, int cin, int cout, void* stream) {
+  const char* who = "e2f_conv2d_wgrad_bf16x3";
+  if (!dy || !x_hi || !x_lo || !dw) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if (n < 0 || h <= 0 || w <= 0 || x_lead < 0 || x_lead > 8) { set_error("%s: bad shape n=%d %dx%d x_lead=%d", who, n, h, w, x_lead); return E2F_ERR_BAD_ARG; }
+  if (cin < 8 || cin % 8 || cin > 512 || cout < 8 || cout % 8 || cout > 512 || (x_lead && !rows_c(cin))) { set_error("%s: cin=%d cout=%d (multiples of 8, <= 512; cin 8, 16 or 32 when x is row-gapped)", who, cin, cout); return E2F_ERR_BAD_ARG; }
+  if (!work) { set_error("%s: null workspace (e2f_conv2d_wgrad_work_elems floats needed)", who); return E2F_ERR_BAD_ARG; }
+  if (!aligned(dy, 16) || !aligned(x_hi, 16) || !aligned(x_lo, 16) || !aligned(dw, 4) || (db && !aligned(db, 4)) ||
+      !aligned(work, 4)) { set_error("%s: alignment (dy, x_hi, x_lo 16 bytes)", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_conv2d_wgrad(dy, x_hi, x_lo, x_lead, dw, db, work, n, h, w, cin, cout, static_cast<cudaStream_t>(stream)), who);
 }
 
 }  // extern "C"

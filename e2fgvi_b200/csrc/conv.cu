@@ -92,11 +92,14 @@ struct Params {
   float* out;              // NHWC fp32 or null
   __nv_bfloat16* out_hi;   // NHWC bf16 split of the result (operand format of the next conv) or null
   __nv_bfloat16* out_lo;
-  // T3 only: derivative of the LeakyReLU(dact_slope) that produced `dact` (bf16 [N][out_H][out_W][Cout], the hi part of
-  // the saved activation).  The result is multiplied by 1 where dact > 0, else by dact_slope (LeakyReLU keeps the sign
-  // of its input, so its output decides).  Null: no multiply.
+  // T3 and the DACT instantiations only: derivative of the LeakyReLU(dact_slope) that produced `dact` (bf16, the hi part
+  // of the saved activation, Cout channels per pixel; pixel (n, y, x) at n * dact_nstride + y * dact_pitch + dact_lead
+  // + x: dense or row-gapped).  The result is multiplied by 1 where dact > 0, else by dact_slope (LeakyReLU keeps the
+  // sign of its input, so its output decides).  Null: no multiply.
   const __nv_bfloat16* dact;
   float dact_slope;
+  int dact_pitch, dact_lead;
+  long long dact_nstride;
 };
 
 constexpr int EPI_TANH = 1, EPI_NCHW = 2;     // both only on the element-wise store path (Cout % 4 != 0: the 3-channel output conv)
@@ -159,7 +162,7 @@ __device__ __forceinline__ TileCoord decode_tile(int tile, const Params& p, int 
 //     pixel row p, row 16 + p = the 32 lo channels), and 4 consecutive lanes then store one buffer row: 64 contiguous
 //     bytes of one pixel.
 // Chunks that are not 32 full, 16-byte-aligned channels take the direct path.
-template <int BN, bool T3 = false>
+template <int BN, bool T3 = false, bool DACT = false>
 __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& t, const float* acc, int row0, int cog,
                                               const float* __restrict__ bias_s, uint8_t* __restrict__ stage, const int TW,
                                               const int TH) {
@@ -179,6 +182,7 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
   auto pix = [&] { return static_cast<size_t>(t.n) * p.out_nstride + static_cast<size_t>(y) * p.out_W + x; };          // fp32 out, residual
   auto opix = [&] { return static_cast<size_t>(t.n) * p.osp_nstride + static_cast<size_t>(y) * p.out_pitch + p.out_lead + x; };  // split outputs
   auto mpix = [&] { return static_cast<size_t>(y) * p.out_W + x; };                                    // bias map
+  auto dpix = [&] { return static_cast<size_t>(t.n) * p.dact_nstride + static_cast<size_t>(y) * p.dact_pitch + p.dact_lead + x; };  // dact
   const int co_end = (t.g + 1) * cog;               // exclusive end of this group's output channels
   const bool vec_ok = (p.Cout & 3) == 0;            // 16-byte aligned channel groups
   const uint32_t sbase = smem_u32(stage);
@@ -218,9 +222,9 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
           f[g4 * 4 + i] = a > 0.f ? a : a * p.slope;
         }
       }
-      if constexpr (T3) {
+      if constexpr (T3 || DACT) {
         if (p.dact && pix_ok) {
-          const uint4* d4 = reinterpret_cast<const uint4*>(p.dact + pix() * p.Cout + co);
+          const uint4* d4 = reinterpret_cast<const uint4*>(p.dact + dpix() * p.Cout + co);
 #pragma unroll
           for (int h8 = 0; h8 < 2; ++h8) {
             const uint4 u = __ldg(d4 + h8);
@@ -324,9 +328,9 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
             const float a = __uint_as_float(v[g8 * 8 + i]) + bb[i];
             f[i] = a > 0.f ? a : a * p.slope;
           }
-          if constexpr (T3) {
+          if constexpr (T3 || DACT) {
             if (p.dact) {
-              const uint4 u = __ldg(reinterpret_cast<const uint4*>(p.dact + pix() * p.Cout + cb));
+              const uint4 u = __ldg(reinterpret_cast<const uint4*>(p.dact + dpix() * p.Cout + cb));
               const __nv_bfloat16* m = reinterpret_cast<const __nv_bfloat16*>(&u);
 #pragma unroll
               for (int i = 0; i < 8; ++i)
@@ -369,8 +373,8 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
             if (cb + i < co_end) {
               float a = __uint_as_float(v[g8 * 8 + i]) + bias_s[cb + i];
               a = a > 0.f ? a : a * p.slope;
-              if constexpr (T3) {
-                if (p.dact && !(__bfloat162float(p.dact[pix() * p.Cout + cb + i]) > 0.f)) a *= p.dact_slope;
+              if constexpr (T3 || DACT) {
+                if (p.dact && !(__bfloat162float(p.dact[dpix() * p.Cout + cb + i]) > 0.f)) a *= p.dact_slope;
               }
               if (p.residual) a += __ldg(p.residual + pix() * p.Cout + cb + i);
               if (p.bias_map) a += __ldg(p.bias_map + mpix() * p.Cout + cb + i);
@@ -411,9 +415,10 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
 }
 
 // T3: 3-D conv over NDHWC sources through 5-D tensor maps {C, W, H, T, B} (see Params::t_out); the 2-D instantiations
-// are unchanged.
-template <int BN, bool T3>
-__global__ void __launch_bounds__(THREADS, 1) conv3x3_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p) {
+// are unchanged.  DACT: 2-D, and the epilogue also applies Params::dact (conv3x3_dact_kernel: the input gradients of
+// SPyNet's 7x7 convs); the plain 2-D instantiations compile without that code.
+template <int BN, bool T3, bool DACT>
+__device__ __forceinline__ void conv3x3_body(const Maps& maps, const Params& p) {
   constexpr int W_TILE = Cfg<BN>::W_TILE, STAGE = Cfg<BN>::STAGE, STAGES = Cfg<BN>::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -571,9 +576,19 @@ __global__ void __launch_bounds__(THREADS, 1) conv3x3_kernel(const __grid_consta
       wgmma_wait<0>();
       if (num_kb > 0 && lane == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
       const TileCoord t = decode_tile<BN>(tile, p, tiles_y, tiles_x, tiles_ng);
-      epilogue_tile<BN, T3>(p, t, acc, wg * 64 + wq * 16, cog, bias_s, my_stage, p.tile_w, p.tile_h);
+      epilogue_tile<BN, T3, DACT>(p, t, acc, wg * 64 + wq * 16, cog, bias_s, my_stage, p.tile_w, p.tile_h);
     }
   }
+}
+
+template <int BN, bool T3>
+__global__ void __launch_bounds__(THREADS, 1) conv3x3_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p) {
+  conv3x3_body<BN, T3, false>(maps, p);
+}
+
+template <int BN>
+__global__ void __launch_bounds__(THREADS, 1) conv3x3_dact_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p) {
+  conv3x3_body<BN, false, true>(maps, p);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -791,10 +806,15 @@ int launch_pack_rows(const float* x, void* hi, void* lo, int n, int c, int h, in
 int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_lo, const int* src_channels,
                    const void* w_hi, const void* w_lo, const float* bias, const float* residual, float* out,
                    void* out_hi, void* out_lo, int n, int h_in, int w_in, int cout, int groups, float slope, int ks,
-                   int stride, int pad, int in_rows, int out_lead, cudaStream_t stream, const ConvGeom* geom, int epi_flags) {
+                   int stride, int pad, int in_rows, int out_lead, cudaStream_t stream, const ConvGeom* geom, int epi_flags,
+                   const void* dact, int dact_lead) {
   using namespace conv;
   if (epi_flags && ((cout & 3) == 0 || out_hi || residual || geom)) {
     set_error("conv: tanh / NCHW epilogues are implemented for the element-wise store path (Cout %% 4 != 0, fp32 output only)");
+    return -2;
+  }
+  if (dact && (geom || groups != 1 || cout > 64 || cout % 8)) {
+    set_error("conv: the ReLU-derivative epilogue needs a plain conv, groups 1 and Cout <= 64, Cout %% 8 == 0");
     return -2;
   }
   // GEMM grid = output size of the plain conv, or what the generalised geometry says
@@ -860,6 +880,7 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
   p.out_lead = out_lead;
   p.tile_w = tile_w; p.tile_h = tile_h;
   p.bias_map = nullptr;
+  p.dact = static_cast<const __nv_bfloat16*>(dact); p.dact_slope = 0.f; p.dact_lead = dact_lead;
   if (geom) {
     p.nphase = geom->nphase; p.ostep = geom->ostep; p.out_H = geom->out_h; p.out_W = geom->out_w;
     p.bias_map = geom->bias_map;
@@ -882,6 +903,8 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
     p.out_nstride = p.osp_nstride = geom->out_nstride;
   }
   p.out_tail = out_lead ? conv_rows_tail(out_lead, cout) : 0;
+  p.dact_pitch = dact_lead ? conv_rows_pitch(p.out_W, dact_lead, cout) : p.out_W;
+  p.dact_nstride = static_cast<long long>(p.out_H) * p.dact_pitch;
   for (int i = 0; i < MAX_SRC; ++i) p.cig[i] = p.chunks[i] = 0;
   if (in_rows) {
     // ONE row-gapped source [N][H][w_in + pad][cin] (+ tail): dimension 1 steps by `stride` pixels, dimension 0 spans
@@ -916,7 +939,7 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
   int chunks_all = 0;
   for (int i = 0; i < nsrc; ++i) chunks_all += (src_channels[i] / groups + BK - 1) / BK;
   int halo_slots = 0;
-  if (!geom && !in_rows && ks == 3 && stride == 1 && pad == 1 && groups == 1 && cout <= 64) {
+  if (!geom && !in_rows && !dact && ks == 3 && stride == 1 && pad == 1 && groups == 1 && cout <= 64) {
     static const bool enabled = [] {
       const char* e = getenv("E2F_CONV_HALO");
       return !(e && e[0] == '0');
@@ -1019,6 +1042,22 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
     return -2;
   }
   const int grid = tiles < num_sms() ? static_cast<int>(tiles) : num_sms();
+  if (dact) {
+    static DeviceOnce dact_configured;
+    if (!device_done(dact_configured, dev)) {
+      cudaError_t e = cudaFuncSetAttribute(conv3x3_dact_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64>::SMEM);
+      if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(conv3x3_dact_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<32>::SMEM);
+      if (e != cudaSuccess) return static_cast<int>(e);
+      device_mark(dact_configured, dev);
+    }
+    if (bn == 32)
+      conv3x3_dact_kernel<32><<<grid, THREADS, Cfg<32>::SMEM, stream>>>(maps, p);
+    else
+      conv3x3_dact_kernel<64><<<grid, THREADS, Cfg<64>::SMEM, stream>>>(maps, p);
+    count_launch();
+    return static_cast<int>(cudaGetLastError());
+  }
   if (bn == 32)
     conv3x3_kernel<32, false><<<grid, THREADS, Cfg<32>::SMEM, stream>>>(maps, p);
   else if (bn == 64)
@@ -1232,6 +1271,7 @@ int launch_dis_conv(const void* src_hi, const void* src_lo, int cin, const void*
   p.slope = slope; p.bias = bias; p.out = out; p.out_cs = cout;
   p.out_hi = static_cast<__nv_bfloat16*>(out_hi); p.out_lo = static_cast<__nv_bfloat16*>(out_lo);
   p.dact = static_cast<const __nv_bfloat16*>(dact); p.dact_slope = dact_slope;
+  p.dact_pitch = w_out; p.dact_lead = 0; p.dact_nstride = static_cast<long long>(h_out) * w_out;
   p.tile_w = tile_w; p.tile_h = tile_h;
   p.out_H = h_out; p.out_W = w_out; p.out_pitch = w_out;
   p.out_nstride = p.osp_nstride = static_cast<long long>(h_out) * w_out;

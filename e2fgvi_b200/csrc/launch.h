@@ -92,7 +92,9 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
                    const void* w_hi, const void* w_lo, const float* bias, const float* residual, float* out,
                    void* out_hi, void* out_lo, int n, int h_in, int w_in, int cout, int groups, float slope, int ks,
                    int stride, int pad, int in_rows, int out_lead, cudaStream_t stream, const ConvGeom* geom = nullptr,
-                   int epi_flags = 0);     // 1: tanh, 2: NCHW fp32 output (3-channel output conv only)
+                   int epi_flags = 0,      // 1: tanh, 2: NCHW fp32 output (3-channel output conv only)
+                   const void* dact = nullptr, int dact_lead = 0);   // ReLU derivative at dact (bf16, Cout channels;
+                                                                     // row-gapped with that lead, or dense when 0)
 int launch_conv_kxn(int nsrc, const void* const* src_hi, const void* const* src_lo, const int* src_c, const void* w_hi,
                     const void* w_lo, const float* bias, const float* residual, float* out, void* out_hi, void* out_lo, int n,
                     int h, int w, int cout, int groups, int co_pad, int ks, float slope, int flags, cudaStream_t stream);
@@ -111,6 +113,11 @@ int dis_wgrad_slices(int b, int t, int h_o, int w_o, int cout, int cin);
 long long dis_wgrad_work_elems(int b, int t, int h_o, int w_o, int cout, int cin);
 int launch_dis_wgrad(const float* dy, const void* x_hi, const void* x_lo, float* dw, float* db, float* work, int b, int t,
                      int h_in, int w_in, int cin, int h_o, int w_o, int cout, int pad, cudaStream_t stream);
+// SPyNet's 7x7 / stride 1 / pad 3 convs: weight (+ bias) gradient from dy fp32 [n][h][w][cout] and the forward's operand
+// x (dense [n][h][w][cin], or row-gapped with x_lead > 0).
+long long conv2d_wgrad_work_elems(int n, int h, int w, int cin, int cout);
+int launch_conv2d_wgrad(const float* dy, const void* x_hi, const void* x_lo, int x_lead, float* dw, float* db, float* work,
+                        int n, int h, int w, int cin, int cout, cudaStream_t stream);
 constexpr int I3D_STEM_TAIL = 16;          // zero pixels after the stem operand's last row (the last window's overrun)
 long long i3d_stem_elems(int b, int t, int h, int w);
 int launch_i3d_stem_pack(const void* x, int x_u8, void* hi, void* lo, int b, int t, int h, int w, cudaStream_t stream);
@@ -132,8 +139,14 @@ int launch_spynet_pyramid(const float* frames, float* pyr, int b, int t, int lt,
                           const float* mean3, const float* std3, cudaStream_t stream);
 int launch_spynet_level_input(const float* img, const float* prev, void* hi, void* lo, float* flow_up, int b, int lt, int hk,
                               int wk, int lead, cudaStream_t stream);
+int launch_spynet_pyramid_unit(const float* frames, float* pyr, int b, int t, int lt, int H, int W, int h, int w, int hu,
+                               int wu, const float* mean3, const float* std3, cudaStream_t stream);
 int launch_spynet_final(const float* flow, float* out_fwd, float* out_bwd, int b, int lt, int h, int w, int hu, int wu,
                         cudaStream_t stream);
+int launch_spynet_level_input_backward(const float* d_in, const float* dflow, const float* img, const float* flow_up,
+                                       float* dprev, int b, int lt, int hk, int wk, cudaStream_t stream);
+int launch_spynet_final_backward(const float* d_fwd, const float* d_bwd, float* dflow, int b, int lt, int h, int w, int hu,
+                                 int wu, cudaStream_t stream);
 
 int launch_video_prepare_clip(const uint8_t* frames, const uint8_t* masks, const int* ids, float* out, int t, int h,
                               int w, int hp, int wp, cudaStream_t stream);

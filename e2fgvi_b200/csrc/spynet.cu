@@ -44,9 +44,10 @@ __device__ __forceinline__ Lerp make_lerp(float src, int in) {
   return t;
 }
 
-// frames: (b, t, 3, H, W) fp32 in [-1, 1]; only frames j < l_t of every clip are used.  One CTA = one 32 x 32 block of
-// level 0 of one local frame; 1024 threads, thread = level-0 pixel.  pyr = the six levels back to back, level k holding
-// [n][3][HU >> k][WU >> k] fp32 (n = b * l_t frames, index bi * l_t + j).
+// frames: (b, t, 3, H, W) fp32 in [-1, 1] (UNIT: already in [0, 1], no (x + 1) / 2); only frames j < l_t of every clip
+// are used.  One CTA = one 32 x 32 block of level 0 of one local frame; 1024 threads, thread = level-0 pixel.  pyr = the
+// six levels back to back, level k holding [n][3][HU >> k][WU >> k] fp32 (n = b * l_t frames, index bi * l_t + j).
+template <bool UNIT>
 __global__ void __launch_bounds__(1024) spynet_pyramid_kernel(const float* __restrict__ frames, float* __restrict__ pyr,
                                                               int T, int LT, int H, int W, int h, int w, int HU, int WU,
                                                               const float* __restrict__ mean3, const float* __restrict__ std3) {
@@ -80,11 +81,17 @@ __global__ void __launch_bounds__(1024) spynet_pyramid_kernel(const float* __res
     for (int a = 0; a < 2; ++a) {
 #pragma unroll
       for (int b2 = 0; b2 < 2; ++b2) {
-        // (x + 1) / 2 of e2fgvi.py:247, then the align_corners=True bilinear sample
-        const float v00 = (__ldg(p + static_cast<long long>(dy[a].i0) * W + dx[b2].i0) + 1.f) / 2.f;
-        const float v01 = (__ldg(p + static_cast<long long>(dy[a].i0) * W + dx[b2].i1) + 1.f) / 2.f;
-        const float v10 = (__ldg(p + static_cast<long long>(dy[a].i1) * W + dx[b2].i0) + 1.f) / 2.f;
-        const float v11 = (__ldg(p + static_cast<long long>(dy[a].i1) * W + dx[b2].i1) + 1.f) / 2.f;
+        // (x + 1) / 2 of e2fgvi.py:247 (UNIT: the [0, 1] value as given), then the align_corners=True bilinear sample
+        float v00 = __ldg(p + static_cast<long long>(dy[a].i0) * W + dx[b2].i0);
+        float v01 = __ldg(p + static_cast<long long>(dy[a].i0) * W + dx[b2].i1);
+        float v10 = __ldg(p + static_cast<long long>(dy[a].i1) * W + dx[b2].i0);
+        float v11 = __ldg(p + static_cast<long long>(dy[a].i1) * W + dx[b2].i1);
+        if constexpr (!UNIT) {
+          v00 = (v00 + 1.f) / 2.f;
+          v01 = (v01 + 1.f) / 2.f;
+          v10 = (v10 + 1.f) / 2.f;
+          v11 = (v11 + 1.f) / 2.f;
+        }
         sm[a][b2] = dy[a].l0 * (dx[b2].l0 * v00 + dx[b2].l1 * v01) + dy[a].l1 * (dx[b2].l0 * v10 + dx[b2].l1 * v11);
       }
     }
@@ -208,13 +215,139 @@ __global__ void __launch_bounds__(256) spynet_final_kernel(const float* __restri
   o[static_cast<long long>(h) * w + static_cast<long long>(y) * w + x] = v * (static_cast<float>(h) / static_cast<float>(HU));
 }
 
+// ----------------------------------------------------------------------------------------------------------- backward
+// Pair p's (ref, supp) frame indices (see spynet_level_input_kernel).
+__device__ __forceinline__ int support_frame(int p, int B, int LT) {
+  const int per_dir = B * (LT - 1);
+  const int dir = p / per_dir, q = p - dir * per_dir;
+  const int bi = q / (LT - 1), j = q - bi * (LT - 1);
+  return bi * LT + (dir ? j : j + 1);
+}
+
+// Gradient reaching flow_up at fine pixel (p, y, x): the residual's dflow, the flow_up channels 6..7 of the conv input's
+// gradient d_in, and the border-mode warp's coordinate gradient from channels 3..5, with torch's grid_sampler_2d backward
+// conventions (a coordinate at or beyond the border gets zero gradient in that axis; out-of-range corners read 0).
+__device__ __forceinline__ float2 flow_up_grad(const float* __restrict__ d_in, const float* __restrict__ dflow,
+                                              const float* __restrict__ sp, const float* __restrict__ flow_up, long long pix,
+                                              int y, int x, int hk, int wk) {
+  const float2 fl = __ldg(reinterpret_cast<const float2*>(flow_up) + pix);
+  const float2 df = __ldg(reinterpret_cast<const float2*>(dflow) + pix);
+  const float* d = d_in + pix * 8;
+  float gu = df.x + __ldg(d + 6), gv = df.y + __ldg(d + 7);
+  const float ix = static_cast<float>(x) + fl.x, iy = static_cast<float>(y) + fl.y;
+  const bool in_x = ix > 0.f && ix < static_cast<float>(wk - 1), in_y = iy > 0.f && iy < static_cast<float>(hk - 1);
+  if (in_x || in_y) {
+    const float px = fminf(fmaxf(ix, 0.f), static_cast<float>(wk - 1)), py = fminf(fmaxf(iy, 0.f), static_cast<float>(hk - 1));
+    const float fx0 = floorf(px), fy0 = floorf(py);
+    const float lx = px - fx0, ly = py - fy0;
+    const int x0 = static_cast<int>(fx0), y0 = static_cast<int>(fy0);
+    const bool x1_ok = x0 + 1 < wk, y1_ok = y0 + 1 < hk;
+    const long long plane = static_cast<long long>(hk) * wk;
+    float gix = 0.f, giy = 0.f;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float* s = sp + c * plane;
+      const float g = __ldg(d + 3 + c);
+      const float v00 = __ldg(s + y0 * wk + x0);
+      const float v01 = x1_ok ? __ldg(s + y0 * wk + x0 + 1) : 0.f;
+      const float v10 = y1_ok ? __ldg(s + (y0 + 1) * wk + x0) : 0.f;
+      const float v11 = (x1_ok && y1_ok) ? __ldg(s + (y0 + 1) * wk + x0 + 1) : 0.f;
+      gix = fmaf(g, (1.f - ly) * (v01 - v00) + ly * (v11 - v10), gix);
+      giy = fmaf(g, (1.f - lx) * (v10 - v00) + lx * (v11 - v01), giy);
+    }
+    if (in_x) gu += gix;
+    if (in_y) gv += giy;
+  }
+  return make_float2(gu, gv);
+}
+
+// Adjoint of spynet_level_input_kernel with respect to prev (the coarser level's flow), as a gather: thread = coarse
+// pixel (p, py, px); it visits the fine pixels whose x2 upsample (align_corners=True) reads it, in a fixed order, and adds
+// 2 * weight * flow_up_grad.  No atomics: deterministic.
+__global__ void __launch_bounds__(256) spynet_level_input_backward_kernel(const float* __restrict__ d_in,
+                                                                          const float* __restrict__ dflow,
+                                                                          const float* __restrict__ img,
+                                                                          const float* __restrict__ flow_up,
+                                                                          float* __restrict__ dprev, int P, int B, int LT,
+                                                                          int hk, int wk) {
+  const int hp = hk >> 1, wp = wk >> 1;
+  const long long total = static_cast<long long>(P) * hp * wp;
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int px = static_cast<int>(i % wp), py = static_cast<int>((i / wp) % hp);
+  const int p = static_cast<int>(i / (static_cast<long long>(wp) * hp));
+  const float* sp = img + static_cast<long long>(support_frame(p, B, LT)) * 3 * hk * wk;
+  const float sy = ac_scale(hp, hk), sx = ac_scale(wp, wk);
+  // fine rows / columns whose lerp taps can include py / px: src = y (hp - 1) / (hk - 1) < y / 2
+  const int y_lo = max(0, 2 * py - 3), y_hi = min(hk - 1, 2 * py + 4);
+  const int x_lo = max(0, 2 * px - 3), x_hi = min(wk - 1, 2 * px + 4);
+  float au = 0.f, av = 0.f;
+  for (int y = y_lo; y <= y_hi; ++y) {
+    const Lerp ty = make_lerp(src_index(sy, y, true), hp);
+    const float wy = (ty.i0 == py ? ty.l0 : 0.f) + (ty.i1 == py ? ty.l1 : 0.f);
+    if (wy == 0.f) continue;
+    for (int x = x_lo; x <= x_hi; ++x) {
+      const Lerp tx = make_lerp(src_index(sx, x, true), wp);
+      const float wx = (tx.i0 == px ? tx.l0 : 0.f) + (tx.i1 == px ? tx.l1 : 0.f);
+      if (wx == 0.f) continue;
+      const float2 g = flow_up_grad(d_in, dflow, sp, flow_up, (static_cast<long long>(p) * hk + y) * wk + x, y, x, hk, wk);
+      const float w2 = 2.0f * wy * wx;
+      au = fmaf(w2, g.x, au);
+      av = fmaf(w2, g.y, av);
+    }
+  }
+  reinterpret_cast<float2*>(dprev)[i] = make_float2(au, av);
+}
+
+// Adjoint of spynet_final_kernel: thread = level-5 flow pixel (p, Y, X); gathers, in a fixed order, the output pixels
+// whose align_corners=False resize reads it, times the u / v rescale.
+__global__ void __launch_bounds__(256) spynet_final_backward_kernel(const float* __restrict__ d_fwd, const float* __restrict__ d_bwd,
+                                                                    float* __restrict__ dflow, int P, int h, int w, int HU, int WU) {
+  const long long total = static_cast<long long>(P) * HU * WU;
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int X = static_cast<int>(i % WU), Y = static_cast<int>((i / WU) % HU);
+  const int p = static_cast<int>(i / (static_cast<long long>(WU) * HU));
+  const int half = P / 2;
+  const float* g = p < half ? d_fwd + static_cast<long long>(p) * 2 * h * w : d_bwd + static_cast<long long>(p - half) * 2 * h * w;
+  const float scy = static_cast<float>(HU) / static_cast<float>(h), scx = static_cast<float>(WU) / static_cast<float>(w);
+  // output rows whose source index lies in [Y - 1, Y + 1): the scale HU / h is >= 1
+  const int y_lo = max(0, (Y - 1) * h / HU - 1), y_hi = min(h - 1, ((Y + 1) * h + HU - 1) / HU + 1);
+  const int x_lo = max(0, (X - 1) * w / WU - 1), x_hi = min(w - 1, ((X + 1) * w + WU - 1) / WU + 1);
+  float au = 0.f, av = 0.f;
+  for (int y = y_lo; y <= y_hi; ++y) {
+    const Lerp ty = make_lerp(src_index(scy, y, false), HU);
+    const float wy = (ty.i0 == Y ? ty.l0 : 0.f) + (ty.i1 == Y ? ty.l1 : 0.f);
+    if (wy == 0.f) continue;
+    for (int x = x_lo; x <= x_hi; ++x) {
+      const Lerp tx = make_lerp(src_index(scx, x, false), WU);
+      const float wx = (tx.i0 == X ? tx.l0 : 0.f) + (tx.i1 == X ? tx.l1 : 0.f);
+      if (wx == 0.f) continue;
+      const float wt = wy * wx;
+      au = fmaf(wt, __ldg(g + static_cast<long long>(y) * w + x), au);
+      av = fmaf(wt, __ldg(g + static_cast<long long>(h) * w + static_cast<long long>(y) * w + x), av);
+    }
+  }
+  reinterpret_cast<float2*>(dflow)[i] =
+      make_float2(au * (static_cast<float>(w) / static_cast<float>(WU)), av * (static_cast<float>(h) / static_cast<float>(HU)));
+}
+
 }  // namespace spy
 
 int launch_spynet_pyramid(const float* frames, float* pyr, int b, int t, int lt, int H, int W, int h, int w, int hu, int wu,
                           const float* mean3, const float* std3, cudaStream_t stream) {
   if (b == 0) return 0;
   const dim3 grid((hu / 32) * (wu / 32), b * lt);
-  spy::spynet_pyramid_kernel<<<grid, 1024, 0, stream>>>(frames, pyr, t, lt, H, W, h, w, hu, wu, mean3, std3);
+  spy::spynet_pyramid_kernel<false><<<grid, 1024, 0, stream>>>(frames, pyr, t, lt, H, W, h, w, hu, wu, mean3, std3);
+  count_launch();
+  return static_cast<int>(cudaGetLastError());
+}
+
+int launch_spynet_pyramid_unit(const float* frames, float* pyr, int b, int t, int lt, int H, int W, int h, int w, int hu,
+                               int wu, const float* mean3, const float* std3, cudaStream_t stream) {
+  if (b == 0) return 0;
+  const dim3 grid((hu / 32) * (wu / 32), b * lt);
+  spy::spynet_pyramid_kernel<true><<<grid, 1024, 0, stream>>>(frames, pyr, t, lt, H, W, h, w, hu, wu, mean3, std3);
   count_launch();
   return static_cast<int>(cudaGetLastError());
 }
@@ -237,6 +370,28 @@ int launch_spynet_final(const float* flow, float* out_fwd, float* out_bwd, int b
   if (P == 0) return 0;
   const long long total = static_cast<long long>(P) * h * w;
   spy::spynet_final_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(flow, out_fwd, out_bwd, P, h, w, hu, wu);
+  count_launch();
+  return static_cast<int>(cudaGetLastError());
+}
+
+int launch_spynet_level_input_backward(const float* d_in, const float* dflow, const float* img, const float* flow_up,
+                                       float* dprev, int b, int lt, int hk, int wk, cudaStream_t stream) {
+  const int P = 2 * b * (lt - 1);
+  if (P == 0) return 0;
+  const long long total = static_cast<long long>(P) * (hk / 2) * (wk / 2);
+  spy::spynet_level_input_backward_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(
+      d_in, dflow, img, flow_up, dprev, P, b, lt, hk, wk);
+  count_launch();
+  return static_cast<int>(cudaGetLastError());
+}
+
+int launch_spynet_final_backward(const float* d_fwd, const float* d_bwd, float* dflow, int b, int lt, int h, int w, int hu,
+                                 int wu, cudaStream_t stream) {
+  const int P = 2 * b * (lt - 1);
+  if (P == 0) return 0;
+  const long long total = static_cast<long long>(P) * hu * wu;
+  spy::spynet_final_backward_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(d_fwd, d_bwd, dflow, P, h,
+                                                                                                     w, hu, wu);
   count_launch();
   return static_cast<int>(cudaGetLastError());
 }

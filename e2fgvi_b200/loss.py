@@ -1,6 +1,9 @@
-"""Losses of the reference's trainer (core/loss.py) that the discriminator step needs."""
+"""Losses of the reference's trainer (core/loss.py) that the discriminator step needs, and the flow completion loss
+(model/modules/flow_comp.py)."""
 import torch
 import torch.nn as nn
+
+from .model.modules.flow_comp import FlowCompletionLoss  # noqa: F401
 
 
 class AdversarialLoss(nn.Module):

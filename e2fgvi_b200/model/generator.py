@@ -2,7 +2,8 @@
 
 Contract kept (SURVEY §8(b)): ``InpaintGenerator()`` takes no required args, ``load_state_dict`` of a reference
 checkpoint is strict-compatible (243 entries base / 244 HQ), and
-``forward(masked_frames[b,t,3,H,W], num_local_frames) -> (pred[b*t,3,H,W], (flows_fwd, flows_bwd))``.
+``forward(masked_frames[b,t,3,H,W], num_local_frames) -> (pred[b*t,3,H,W], (flows_fwd, flows_bwd))``, inference-only.
+``forward_bidirect_flow`` has a backward pass into ``update_spynet`` (the flow-completion loss of train.py).
 The constructor never downloads SPyNet weights.
 """
 import contextlib
@@ -162,8 +163,17 @@ class InpaintGenerator(BaseNetwork):
 
     def forward_bidirect_flow(self, masked_local_frames):
         """1/4 bilinear downsample then SPyNet in both directions (e2fgvi.py:210-234); both directions run as
-        one batched SPyNet call (every op inside is batch-independent)."""
+        one batched SPyNet call (every op inside is batch-independent).  masked_local_frames (b, l_t, 3, h, w) in [0, 1].
+
+        Trainable: with grad mode on and some ``update_spynet`` parameter requiring grad, CUDA frames go through the
+        fused SPyNet path with a backward pass (``SPyNet.bidirect_flows``), and the flows carry a ``grad_fn`` into
+        ``update_spynet``: the flow-completion step of train.py (see INTEGRATION "Flow completion").  The flows equal
+        ``forward(masked_frames, l_t)[1]`` bit for bit when masked_local_frames = (masked_frames[:, :l_t] + 1) / 2.
+        Frames that require grad raise ``ValueError`` there (no gradient into the frames)."""
         b, l_t, c, h, w = masked_local_frames.size()
+        if (masked_local_frames.is_cuda and l_t > 1 and torch.is_grad_enabled()
+                and any(p.requires_grad for p in self.update_spynet.parameters())):
+            return self.update_spynet.bidirect_flows(masked_local_frames, l_t, unit=True)
         small = F.interpolate(masked_local_frames.reshape(-1, c, h, w), scale_factor=1 / 4, mode="bilinear",
                               align_corners=True, recompute_scale_factor=True)
         small = small.view(b, l_t, c, h // 4, w // 4)
@@ -191,8 +201,11 @@ class InpaintGenerator(BaseNetwork):
     _warned_grad = False
 
     def forward(self, masked_frames, num_local_frames):
-        """INFERENCE ONLY, CUDA ONLY: the kernels have no backward (outputs carry no grad_fn) and there is no CPU path
-        (the reference's ``train.py`` / CPU use is out of scope, SURVEY §2)."""
+        """INFERENCE ONLY, CUDA ONLY: outputs carry no grad_fn, the flows included, and there is no CPU path.  To train
+        ``update_spynet`` on the flow-completion loss, call ``forward_bidirect_flow`` (it has a backward pass).  The
+        flows of this call stay untracked on purpose: with the trainer's ``gen_loss = gan + flow + hole + valid``, flows
+        that alone tracked gradients would make ``gen_loss.backward()`` silently leave out every image-loss path into
+        ``update_spynet``."""
         # (CPU tensors fail loudly inside the first kernel wrapper: ops._need_cuda, "there is no CPU fallback")
         if torch.is_grad_enabled() and not InpaintGenerator._warned_grad and any(p.requires_grad for p in self.parameters()):
             import warnings
@@ -247,12 +260,14 @@ class InpaintGenerator(BaseNetwork):
                 main = torch.cuda.current_stream()
                 side = self._side_stream(masked_frames.device)
                 side.wait_stream(main)
-                with torch.cuda.stream(side):
+                with torch.cuda.stream(side), torch.no_grad():
                     pred_flows = self.update_spynet.bidirect_flows(masked_frames, l_t)
             else:
-                pred_flows = self.update_spynet.bidirect_flows(masked_frames, l_t)
+                with torch.no_grad():
+                    pred_flows = self.update_spynet.bidirect_flows(masked_frames, l_t)
         else:
-            pred_flows = self.forward_bidirect_flow((masked_frames[:, :l_t] + 1) / 2)
+            with torch.no_grad():
+                pred_flows = self.forward_bidirect_flow((masked_frames[:, :l_t] + 1) / 2)
 
         # encoder output: fp32 (b*t,c,h,w) in NHWC storage + its bf16 (hi, lo) split, both viewed as (b,t,h,w,c)
         enc32, enc_sp = self.encoder(masked_frames.reshape(b * t, ori_c, ori_h, ori_w), last_out="both")

@@ -1201,11 +1201,12 @@ class FlowPyramid:
         self.levels, self.b, self.l_t, self.size, self.up = levels, b, l_t, size, up
 
 
-def spynet_pyramid(masked_frames, num_local_frames, mean, std):
+def spynet_pyramid(masked_frames, num_local_frames, mean, std, unit=False):
     """Everything in front of SPyNet's first level, once per LOCAL FRAME (the reference does it per (ref, supp) pair):
     ``(x + 1) / 2`` and the 1/4 bilinear downsample of e2fgvi.py:210-218,247, the resize to multiples of 32, the
-    normalisation and the five 2x2 average pools of flow_comp.py:95-115,152-158.  masked_frames (b,t,3,H,W) fp32;
-    mean / std: the (1,3,1,1) buffers.  Returns a ``FlowPyramid``: levels[k] = (b*l_t, 3, h_up >> k, w_up >> k) fp32."""
+    normalisation and the five 2x2 average pools of flow_comp.py:95-115,152-158.  masked_frames (b,t,3,H,W) fp32 in
+    [-1, 1], or in [0, 1] with ``unit`` (``e2f_spynet_pyramid_unit``: no ``(x + 1) / 2``); mean / std: the (1,3,1,1)
+    buffers.  Returns a ``FlowPyramid``: levels[k] = (b*l_t, 3, h_up >> k, w_up >> k) fp32."""
     _need_cuda(masked_frames, mean, std)
     b, t, c, H, W = masked_frames.shape
     if c != 3:
@@ -1219,9 +1220,10 @@ def spynet_pyramid(masked_frames, num_local_frames, mean, std):
     sizes = [n * 3 * (hu >> k) * (wu >> k) for k in range(6)]
     buf = torch.empty(sum(sizes), dtype=torch.float32, device=x.device)
     m32, s32 = mean.detach().float().contiguous(), std.detach().float().contiguous()
-    st = _lib.load().e2f_spynet_pyramid(x.data_ptr(), buf.data_ptr(), b, t, l_t, H, W, h, w, hu, wu, m32.data_ptr(),
-                                        s32.data_ptr(), _stream())
-    _lib.check(st, "e2f_spynet_pyramid")
+    fn = "e2f_spynet_pyramid_unit" if unit else "e2f_spynet_pyramid"
+    st = getattr(_lib.load(), fn)(x.data_ptr(), buf.data_ptr(), b, t, l_t, H, W, h, w, hu, wu, m32.data_ptr(),
+                                  s32.data_ptr(), _stream())
+    _lib.check(st, fn)
     levels, off = [], 0
     for k in range(6):
         levels.append(buf[off: off + sizes[k]].view(n, 3, hu >> k, wu >> k))
@@ -1266,6 +1268,140 @@ def spynet_final(flow, pyr):
     st = _lib.load().e2f_spynet_final(flow.data_ptr(), fwd.data_ptr(), bwd.data_ptr(), pyr.b, pyr.l_t, h, w, hu, wu, _stream())
     _lib.check(st, "e2f_spynet_final")
     return fwd, bwd
+
+
+# ---------------------------------------------------------------------------------------------- SPyNet backward
+def spynet_final_backward(d_forward, d_backward, pyr):
+    """Adjoint of ``spynet_final``: d flows_forward / d flows_backward (b, l_t-1, 2, h, w) -> d level-0 flow
+    (P, h_up, w_up, 2) fp32."""
+    _need_cuda(d_forward, d_backward)
+    h, w = pyr.size
+    hu, wu = pyr.up
+    P = 2 * pyr.b * (pyr.l_t - 1)
+    shape = (pyr.b, pyr.l_t - 1, 2, h, w)
+    if tuple(d_forward.shape) != shape or tuple(d_backward.shape) != shape:
+        raise ValueError(f"spynet_final_backward: gradients {tuple(d_forward.shape)} / {tuple(d_backward.shape)} != {shape}")
+    gf, gb = d_forward.contiguous().float(), d_backward.contiguous().float()
+    dflow = torch.empty((P, hu, wu, 2), dtype=torch.float32, device=gf.device)
+    st = _lib.load().e2f_spynet_final_backward(gf.data_ptr(), gb.data_ptr(), dflow.data_ptr(), pyr.b, pyr.l_t, h, w, hu, wu,
+                                               _stream())
+    _lib.check(st, "e2f_spynet_final_backward")
+    return dflow
+
+
+def spynet_level_input_backward(d_in, dflow, pyr, k, flow_up):
+    """Adjoint of ``spynet_level_input`` with respect to the coarser level's flow.  d_in (P, hk, wk, 8) fp32: gradient
+    of the level's conv input (channels 3..7 are read); dflow (P, hk, wk, 2): gradient of the level's output flow;
+    flow_up: what ``spynet_level_input`` returned.  Returns d prev_flow (P, hk/2, wk/2, 2) fp32."""
+    img = pyr.levels[k]
+    _, _, hk, wk = img.shape
+    P = 2 * pyr.b * (pyr.l_t - 1)
+    for name, t, c in (("d_in", d_in, 8), ("dflow", dflow, 2), ("flow_up", flow_up, 2)):
+        if tuple(t.shape) != (P, hk, wk, c) or not t.is_contiguous() or t.dtype != torch.float32:
+            raise ValueError(f"spynet_level_input_backward: {name} {tuple(t.shape)} != {(P, hk, wk, c)} fp32 contiguous")
+    dprev = torch.empty((P, hk // 2, wk // 2, 2), dtype=torch.float32, device=img.device)
+    st = _lib.load().e2f_spynet_level_input_backward(d_in.data_ptr(), dflow.data_ptr(), img.data_ptr(), flow_up.data_ptr(),
+                                                     dprev.data_ptr(), pyr.b, pyr.l_t, hk, wk, _stream())
+    _lib.check(st, "e2f_spynet_level_input_backward")
+    return dprev
+
+
+def conv_dgrad_weight(weight):
+    """The input gradient's weight: fp32 (Cout, Cin, k, k) -> Wt (Cin, Cout, k, k), Wt[ci][co][ky][kx] =
+    W[co][ci][k-1-ky][k-1-kx] (rotated by 180 degrees, in / out swapped)."""
+    return weight.detach().float().flip(2, 3).transpose(0, 1).contiguous()
+
+
+def pack_conv_dgrad_weight(weight, dy_rows_cin=0):
+    """``conv_dgrad_weight`` packed as the forward packs a weight for that dY: window-packed K for a row-gapped dY of
+    ``dy_rows_cin`` channels (``pack_conv_rows_weight``), tap-major 64-channel chunks for a dense one."""
+    wt = conv_dgrad_weight(weight)
+    if dy_rows_cin:
+        return pack_conv_rows_weight(wt, dy_rows_cin)
+    return pack_conv3x3_weight(wt, [weight.shape[0]])
+
+
+def conv2d_dgrad(dy, weight, act=None, out="f32", out_lead=3):
+    """Input gradient of a 7x7 / stride 1 / pad 3 conv (``e2f_conv2d_dgrad_bf16x3``): dy = the gradient of its output
+    as a ``RowsNHWC`` (lead 3) or dense ``SplitNHWC``; weight = the forward's nn.Conv2d weight (Cout, Cin, 7, 7).
+    ``act`` (``RowsNHWC`` / ``SplitNHWC`` with Cin channels, the ReLU output the conv read, or None) multiplies the result
+    by ReLU's derivative.  Returns (dx fp32 (N, H, W, Cin), operand): operand = None (out "f32"), a ``RowsNHWC`` with
+    ``out_lead`` (out "rows") or a ``SplitNHWC`` (out "split") of dx: the next input gradient's dy."""
+    cout, cin, ks, _ = weight.shape
+    if ks != 7 or tuple(weight.shape[2:]) != (7, 7):
+        raise ValueError(f"conv2d_dgrad: 7x7 kernels only, got {tuple(weight.shape)}")
+    rows = isinstance(dy, RowsNHWC)
+    if rows and dy.lead != 3:
+        raise ValueError("conv2d_dgrad: a row-gapped dy needs lead 3")
+    dy_c = dy.cin if rows else dy.hi.shape[-1]
+    if dy.shape[1] != cout:
+        raise ValueError(f"conv2d_dgrad: dy has {dy.shape[1]} channels, the weight {cout} outputs")
+    n, _, h, w = dy.shape
+    _need_cuda(weight, dy.hi)
+    w_hi, w_lo = _derived([weight], ("dgrad", dy_c if rows else 0), lambda: pack_conv_dgrad_weight(weight, dy_c if rows else 0))
+    act_ptr, act_lead = None, 0
+    if act is not None:
+        if act.shape != (n, cin, h, w) or (isinstance(act, RowsNHWC) and act.cin != cin) or (
+                isinstance(act, SplitNHWC) and act.hi.shape[-1] != cin):
+            raise ValueError(f"conv2d_dgrad: act {act.shape} does not match ({n}, {cin}, {h}, {w})")
+        act_ptr, act_lead = act.hi.data_ptr(), (act.lead if isinstance(act, RowsNHWC) else 0)
+    dev = weight.device
+    dx = torch.empty((n, h, w, cin), dtype=torch.float32, device=dev)
+    ohi = olo = None
+    lead = out_lead if out == "rows" else 0
+    if out == "rows":
+        numel = _rows_numel(n, h, w, out_lead, cin)
+        ohi = torch.empty(numel, dtype=torch.bfloat16, device=dev)
+        olo = torch.empty(numel, dtype=torch.bfloat16, device=dev)
+    elif out == "split":
+        ohi = torch.empty((n, h, w, cin), dtype=torch.bfloat16, device=dev)
+        olo = torch.empty((n, h, w, cin), dtype=torch.bfloat16, device=dev)
+    elif out != "f32":
+        raise ValueError("conv2d_dgrad: out must be 'f32', 'rows' or 'split'")
+    with _timed(f"conv2d_dgrad_c{cin}", 2.0 * n * h * w * cout * cin * 49):
+        st = _lib.load().e2f_conv2d_dgrad_bf16x3(dy.hi.data_ptr(), dy.lo.data_ptr(), dy_c, 3 if rows else 0,
+                                                 w_hi.data_ptr(), w_lo.data_ptr(), act_ptr, act_lead, dx.data_ptr(),
+                                                 None if ohi is None else ohi.data_ptr(),
+                                                 None if olo is None else olo.data_ptr(), lead, n, h, w, cin, _stream())
+    _lib.check(st, "e2f_conv2d_dgrad_bf16x3")
+    if out == "rows":
+        return dx, RowsNHWC(ohi, olo, (n, cin, h, w), out_lead, cin)
+    if out == "split":
+        return dx, SplitNHWC(ohi, olo, (n, cin, h, w))
+    return dx, None
+
+
+def conv2d_wgrad(dy, x, cin, with_bias=True):
+    """(dW fp32 (Cout, cin, 7, 7), db fp32 (Cout,) or None) of a 7x7 / stride 1 / pad 3 conv (``e2f_conv2d_wgrad_bf16x3``)
+    from dy fp32 (N, H, W, Cout) (Cout padded to a multiple of 8 here) and the forward's operand x (``RowsNHWC`` or dense
+    ``SplitNHWC``); the first ``cin`` input channels are returned."""
+    n, h, w, cout = dy.shape
+    _need_cuda(dy, x.hi)
+    dy = dy.contiguous().float()
+    cpad = -(-cout // 8) * 8
+    if cpad != cout:
+        dy = torch.nn.functional.pad(dy, (0, cpad - cout))
+    rows = isinstance(x, RowsNHWC)
+    xc = x.cin if rows else x.hi.shape[-1]
+    if x.shape[0] != n or tuple(x.shape[2:]) != (h, w) or cin > xc:
+        raise ValueError(f"conv2d_wgrad: x {x.shape} does not match dy {tuple(dy.shape)} / cin {cin}")
+    lib = _lib.load()
+    elems = lib.e2f_conv2d_wgrad_work_elems(n, h, w, xc, cpad)
+    if elems < 0:
+        _lib.check(int(elems), "e2f_conv2d_wgrad_work_elems")
+    work = torch.empty(int(elems), dtype=torch.float32, device=dy.device)
+    dw = torch.empty(cpad, xc, 7, 7, dtype=torch.float32, device=dy.device)
+    db = torch.empty(cpad, dtype=torch.float32, device=dy.device) if with_bias else None
+    with _timed(f"conv2d_wgrad_c{cout}", 2.0 * n * h * w * cout * xc * 49):
+        st = lib.e2f_conv2d_wgrad_bf16x3(dy.data_ptr(), x.hi.data_ptr(), x.lo.data_ptr(), x.lead if rows else 0,
+                                         dw.data_ptr(), None if db is None else db.data_ptr(), work.data_ptr(), n, h, w, xc,
+                                         cpad, _stream())
+    _lib.check(st, "e2f_conv2d_wgrad_bf16x3")
+    if cpad != cout or cin != xc:
+        dw = dw[:cout, :cin].contiguous()
+    if db is not None and cpad != cout:
+        db = db[:cout].contiguous()
+    return dw, db
 
 
 def attention_flops(B, T, H, W, C, window_size, expand_size, focal_window, use_pooled=True):

@@ -255,3 +255,22 @@ def synth_dis_state_dict(seed=0, use_spectral_norm=True, in_channels=3):
             sd[p + "weight"] = w
             sd[p + "bias"] = _normal((cout,), 0.1, _gen(seed, f"dis.{i}.b"))
     return sd
+
+
+def synth_spynet_state_dict(seed=0, prefix="", flow_scale=1.0):
+    """State dict of a ``SPyNet`` (``prefix`` e.g. "update_spynet." or "fix_spynet.") with deterministic values:
+    fan-in-scaled (He) weights so that activations stay O(1) through each level's five convs, small biases, and the last
+    conv of every level scaled by ``flow_scale`` so that the flows reach several pixels (about 10 at 64x128 for 1.0, 3 for
+    0.25): enough for warps that clamp at the border and for coarse-level flows that move whole pixels."""
+    from .model.modules.flow_comp import _LEVEL_CONVS, _NUM_LEVELS
+    sd = {}
+    for level in range(_NUM_LEVELS):
+        for k, (cin, cout) in enumerate(_LEVEL_CONVS):
+            shape = (cout, cin, 7, 7)
+            std = math.sqrt(2.0 / _fan_in(shape)) * (flow_scale if k == len(_LEVEL_CONVS) - 1 else 1.0)
+            key = f"{prefix}basic_module.{level}.basic_module.{k}.conv."
+            sd[key + "weight"] = _normal(shape, std, _gen(seed, f"spy.{level}.{k}.w"))
+            sd[key + "bias"] = _normal((cout,), 0.05, _gen(seed, f"spy.{level}.{k}.b"))
+    sd[prefix + "mean"] = torch.tensor([0.485, 0.456, 0.406]).view(1, 3, 1, 1)
+    sd[prefix + "std"] = torch.tensor([0.229, 0.224, 0.225]).view(1, 3, 1, 1)
+    return sd

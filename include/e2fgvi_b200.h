@@ -349,6 +349,26 @@ int e2f_spynet_level_input(const float* level_img, const float* prev_flow, void*
 int e2f_spynet_final(const float* flow, float* flows_forward, float* flows_backward, int b, int l_t, int h, int w, int h_up,
                      int w_up, void* stream);
 
+/* Backward of the SPyNet glue (the differentiable InpaintGenerator.forward_bidirect_flow; gradients reach the flows, not
+ * the frames).  Both backward kernels are gathers with a fixed summation order: no atomics, bit-identical from run to run.
+ *   e2f_spynet_pyramid_unit: e2f_spynet_pyramid for frames already in [0, 1] (no (x + 1) / 2), the input that
+ *     forward_bidirect_flow receives.  Same arguments.
+ *   e2f_spynet_level_input_backward: adjoint of e2f_spynet_level_input with respect to prev_flow.  d_in [P][hk][wk][8]
+ *     fp32 is the gradient of the level's conv input (channels 3..5: the warped support image, 6..7: flow_up; 0..2 are
+ *     not read); dflow [P][hk][wk][2] the gradient of the level's output flow (= the residual's); level_img and flow_up
+ *     as the forward used and wrote them.  d flow_up = dflow + d_in[6:8] + the border warp's coordinate gradient of
+ *     d_in[3:6], with torch grid_sampler_2d's backward conventions: a coordinate at or beyond the border (<= 0 or
+ *     >= size - 1) gets zero gradient in that axis.  dprev [P][hk/2][wk/2][2] = 2 * (x2 align_corners=True upsample)^T
+ *     d flow_up.  hk, wk even.
+ *   e2f_spynet_final_backward: adjoint of e2f_spynet_final: d_forward / d_backward (b, l_t - 1, 2, h, w) fp32 ->
+ *     dflow [P][h_up][w_up][2] fp32 (the u / v rescale, then the transposed align_corners=False resize). */
+int e2f_spynet_pyramid_unit(const float* frames, float* pyramid, int b, int t, int l_t, int H, int W, int h, int w, int h_up,
+                            int w_up, const float* mean3, const float* std3, void* stream);
+int e2f_spynet_level_input_backward(const float* d_in, const float* dflow, const float* level_img, const float* flow_up,
+                                    float* dprev, int b, int l_t, int hk, int wk, void* stream);
+int e2f_spynet_final_backward(const float* d_forward, const float* d_backward, float* dflow, int b, int l_t, int h, int w,
+                              int h_up, int w_up, void* stream);
+
 /* Output stitch over NVLink / NVSwitch peer memory (SURVEY 8(e): clips are the sharding unit, the only exchange is the
  * all-gather of the output frames — the multi-GPU form of test.py:168-179 collecting every window's frames into one list).
  * Each rank owns a landing buffer and PUSHES its block of frames into every peer's buffer with DMA copies (copy engines,
@@ -505,6 +525,29 @@ int e2f_dis_conv3d_dgrad(const void* dy_hi, const void* dy_lo, int cout, const v
 int64_t e2f_dis_conv3d_wgrad_work_elems(int b, int t, int h_in, int w_in, int cin, int cout, int pad);
 int e2f_dis_conv3d_wgrad(const float* dy, const void* x_hi, const void* x_lo, float* dw, float* db, float* work, int b,
                          int t, int h_in, int w_in, int cin, int cout, int pad, void* stream);
+
+/* Gradients of SPyNet's 7x7 / stride 1 / pad 3 convs (the forward is e2f_conv2d_rows_bf16x3 with a ReLU after all but
+ * the last conv), bf16 three-term splits with fp32 accumulation.
+ *   e2f_conv2d_dgrad_bf16x3 : input gradient dX[n][h][w][cin] = conv(dY, W rotated by 180 degrees with in / out swapped),
+ *       on the forward's implicit-GEMM kernel.  dY = (dy_hi, dy_lo) with dy_c channels: dense [n][h][w][dy_c] (dy_lead 0,
+ *       dy_c % 8 == 0) or row-gapped with lead 3 (dy_c 8, 16 or 32, window-packed K; see e2f_conv_rows_pitch).  Wt =
+ *       the forward weight W [dy_c'][cin][7][7] as Wt[ci][co][ky][kx] = W[co][ci][6 - ky][6 - kx], packed as
+ *       e2f_conv2d_rows_bf16x3 packs a weight for that dY layout (row-gapped: [cin][7 * G * 64], dense: [cin][49 *
+ *       ceil(dy_c / 64) * 64]).  `act` (bf16 hi part of the ReLU output that fed the conv, cin channels; dense, or
+ *       row-gapped with act_lead > 0) or NULL: dX is multiplied by ReLU's derivative, 1 where act > 0, else 0.  Outputs:
+ *       fp32 dx [n][h][w][cin] and/or its split (dense, or row-gapped with dx_lead > 0: the next input gradient's dY).
+ *       cin % 8 == 0, <= 64 (8, 16 or 32 with a row-gapped act or dx).
+ *   e2f_conv2d_wgrad_work_elems / e2f_conv2d_wgrad_bf16x3 : dw fp32 [cout][cin][7][7] and, if db is not NULL, db fp32
+ *       [cout] = the sum of dy over pixels, from dy fp32 [n][h][w][cout] and the forward's operand x = (x_hi, x_lo):
+ *       dense [n][h][w][cin] (x_lead 0) or row-gapped with x_lead zero pixels per row (cin 8, 16 or 32).  cin, cout % 8 == 0.
+ *       The split-K GEMM of e2f_dis_conv3d_wgrad: `work` holds e2f_conv2d_wgrad_work_elems(...) floats (negative = bad
+ *       arguments) and the slices are added in a fixed order: bit-identical from run to run. */
+int e2f_conv2d_dgrad_bf16x3(const void* dy_hi, const void* dy_lo, int dy_c, int dy_lead, const void* wt_hi, const void* wt_lo,
+                            const void* act, int act_lead, float* dx, void* dx_hi, void* dx_lo, int dx_lead, int n, int h,
+                            int w, int cin, void* stream);
+int64_t e2f_conv2d_wgrad_work_elems(int n, int h, int w, int cin, int cout);
+int e2f_conv2d_wgrad_bf16x3(const float* dy, const void* x_hi, const void* x_lo, int x_lead, float* dw, float* db, float* work,
+                            int n, int h, int w, int cin, int cout, void* stream);
 
 /* Number of kernel launches issued through this library since load (all threads); used by bench.py's
  * "gpu_launches" accounting. */
