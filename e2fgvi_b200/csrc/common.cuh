@@ -201,6 +201,20 @@ __device__ __forceinline__ void wgmma_n64_f16_rs_tb(float* d, const uint32_t (&a
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(acc));
 }
 
+// ----------------------------------------------------------------------------- warp specialisation
+// named barriers (id 0 is __syncthreads); `threads` counts every thread that syncs or arrives
+__device__ __forceinline__ void named_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+// setmaxnreg: a producer warpgroup gives registers back, consumer warpgroups take them (the whole warpgroup executes it)
+template <int REGS>
+__device__ __forceinline__ void regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
+template <int REGS>
+__device__ __forceinline__ void regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS)); }
+
 // ----------------------------------------------------------------------------- misc
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;

@@ -18,8 +18,11 @@
 //    kernel width are zero; what those positions read is finite data of the same buffer.
 //  * epilogue: + bias, LeakyReLU(slope), optional residual add, fp32 NHWC store and/or the bf16 (hi, lo) split of
 //    the result — dense NHWC or row-gapped for a following window-packed conv (the zero gaps are written here).
-// Pipeline: persistent CTAs, TMA warp + two consumer warpgroups (64 accumulator rows each, fp32 in registers);
-// each warp's epilogue reads its own accumulator fragments (no CTA-wide staging tile, so the pipeline gets that room).
+// Pipeline ("ping-pong", as gemm.cu): persistent CTAs; a producer warpgroup whose one thread fills the TMA ring in the
+// CTA's tile order, and two consumer warpgroups that take alternate tiles, each owning a whole 128 x BN tile (two
+// m64nBN halves, fp32 in registers).  Named barriers make them issue their main loops in turn, so one warpgroup's
+// epilogue runs while the other's MMAs keep the tensor pipe busy.  Each warp's epilogue reads its own accumulator
+// fragments (no CTA-wide staging tile, so the pipeline gets that room).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cstdlib>
@@ -33,10 +36,16 @@ namespace conv {
 constexpr int BM = 128, BK = 64;
 constexpr int TILE_H = 8, TILE_W = 16;                  // 8 x 16 output pixels = 128 GEMM rows
 constexpr int A_TILE = BM * BK * 2;
-constexpr int EPI_WARPS = 8;                             // two consumer warpgroups; in the epilogue each warp stores its 16 accumulator rows
+constexpr int EPI_WARPS = 8;                             // two consumer warpgroups; in the epilogue each warp stores 16-row slices
 constexpr int MAX_COUT = 512;                            // bias staged in shared memory once per CTA
 constexpr int EPI_STAGE = 2048;                          // per epilogue warp: 32 rows x 64 bytes store-transposition buffer
-constexpr int THREADS = (EPI_WARPS + 1) * 32;                // + the TMA warp
+constexpr int THREADS = (EPI_WARPS + 4) * 32;            // + the producer warpgroup (one thread issues the TMA loads)
+// register split (setmaxnreg): two m64nBN accumulators (128 fp32 at BN = 128) + the epilogue do not fit the 168
+// registers a 384-thread CTA starts with, so the producer warpgroup gives its share to the consumers: 128 x 40 + 256 x
+// 232 <= 64 K
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+// named barriers (0 is __syncthreads): ORDER_BAR + w = "warpgroup w may issue its next main loop", 256 threads
+constexpr int ORDER_BAR = 1;
 constexpr int MAX_SRC = 4;
 constexpr int MAX_TAPS = 80;                             // the discriminator's 3x5x5 kernels list 75 taps
 
@@ -437,7 +446,7 @@ __device__ __forceinline__ void conv3x3_body(const Maps& maps, const Params& p) 
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], EPI_WARPS);
+      mbar_init(&empty[s], 4);                           // the 4 warps of the warpgroup that consumed the stage
     }
     fence_barrier_init();
     tma_prefetch_desc(&maps.w_hi);
@@ -449,9 +458,10 @@ __device__ __forceinline__ void conv3x3_body(const Maps& maps, const Params& p) 
   }
   __syncthreads();
 
-  if (warp == EPI_WARPS) {
-    // ------------------------------------------------------------------ TMA producer (im2col by coordinates)
-    if (elect_one()) {
+  if (warp >= EPI_WARPS) {
+    // ------------------------------------------------------------------ TMA producer (im2col by coordinates), one ring
+    regs_dec<PRODUCER_REGS>();
+    if (warp == EPI_WARPS && elect_one()) {
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const TileCoord t = decode_tile<BN>(tile, p, tiles_y, tiles_x, tiles_ng);
@@ -539,23 +549,37 @@ __device__ __forceinline__ void conv3x3_body(const Maps& maps, const Params& p) 
       }
     }
   } else {
-    // ------------------------------------------------------------------ consumers: wgmma main loop, then the epilogue
-    // warpgroup wg owns accumulator rows [64 wg, 64 wg + 64); this warpgroup's A rows start 64 * 128 B into the A tiles
+    // ------------------------------------------------------------------ consumers: ping-pong main loop + epilogue
+    regs_inc<CONSUMER_REGS>();
     const int wg = warp >> 2, wq = warp & 3;
-    const uint64_t d_ah0 = gmma_desc_sw128(smem_u32(smem) + wg * 64 * 128, 16, 1024);
+    // stage-0 descriptors; stage s / K step k / the second 64-row half of the A tiles are reached with one 64-bit add
+    const uint64_t d_ah0 = gmma_desc_sw128(smem_u32(smem), 16, 1024);
     const uint64_t d_al0 = gmma_desc_adv(d_ah0, A_TILE);
     const uint64_t d_wh0 = gmma_desc_sw128(smem_u32(smem) + 2 * A_TILE, 16, 1024);
     const uint64_t d_wl0 = gmma_desc_adv(d_wh0, W_TILE);
+    constexpr uint32_t HALF = (64 * 128) >> 4;
     uint8_t* my_stage = epi_stage + warp * EPI_STAGE;
-    float acc[BN / 2];
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    float acc[BN];                                      // rows [0, 64) of the tile, then rows [64, 128)
+    // this CTA's tiles: tile blockIdx.x + i * gridDim.x for i < my_tiles; warpgroup wg takes i = wg, wg + 2, ...
+    const int grid = static_cast<int>(gridDim.x);
+    const int my_tiles = (num_tiles - static_cast<int>(blockIdx.x) + grid - 1) / grid;
+    uint32_t it = 0;                                    // ring position of tile i's first K block
+    for (int i = 0; i < my_tiles; ++i) {
+      const int tile = static_cast<int>(blockIdx.x) + i * grid;
+      // K blocks of this tile: the 9-phase gather conv's phases have different tap counts, so the ring position of a
+      // tile is the sum over all earlier tiles of the CTA, including the other warpgroup's
       int num_kb = p.ks * p.rows_g;                     // window-packed K
       if constexpr (T3) num_kb *= p.kt;
       if (!p.rows_px) {
         const int ph = (tile / (tiles_ng * p.groups)) % p.nphase;
         num_kb = (p.ph_tap0[ph + 1] - p.ph_tap0[ph]) * p.chunks_total;
       }
+      if ((i & 1) != wg) {
+        it += num_kb;
+        continue;
+      }
+      // wait for the turn: the other warpgroup has issued tile i - 1's main loop
+      if (i > 0) named_sync(ORDER_BAR + wg, 256);
       for (int kb = 0; kb < num_kb; ++kb, ++it) {
         const int stage = it % STAGES;
         mbar_wait(&full[stage], (it / STAGES) & 1);
@@ -566,17 +590,28 @@ __device__ __forceinline__ void conv3x3_body(const Maps& maps, const Params& p) 
           const uint64_t dah = d_ah0 + soff + 2 * k, dal = d_al0 + soff + 2 * k;
           const uint64_t dwh = d_wh0 + soff + 2 * k, dwl = d_wl0 + soff + 2 * k;
           wgmma_ss<BN, false>(acc, dal, dwh, (kb | k) != 0);   // small terms first
+          wgmma_ss<BN, false>(acc + BN / 2, dal + HALF, dwh, (kb | k) != 0);
           wgmma_ss<BN, false>(acc, dah, dwl, 1);
+          wgmma_ss<BN, false>(acc + BN / 2, dah + HALF, dwl, 1);
           wgmma_ss<BN, false>(acc, dah, dwh, 1);
+          wgmma_ss<BN, false>(acc + BN / 2, dah + HALF, dwh, 1);
         }
         wgmma_commit();
         wgmma_wait<1>();                                  // the previous K block's MMAs are done: release its stage
         if (kb > 0 && lane == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
       }
+      if (i + 1 < my_tiles) named_arrive(ORDER_BAR + (wg ^ 1), 256);   // the other warpgroup may issue tile i + 1
       wgmma_wait<0>();
       if (num_kb > 0 && lane == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
       const TileCoord t = decode_tile<BN>(tile, p, tiles_y, tiles_x, tiles_ng);
-      epilogue_tile<BN, T3, DACT>(p, t, acc, wg * 64 + wq * 16, cog, bias_s, my_stage, p.tile_w, p.tile_h);
+      // rows wq*16 and 64 + wq*16 through ONE inlined epilogue: the second half is then moved into the first half's
+      // registers.  Two inlined copies spill at BN = 128 (124 bytes at 232 registers); this form spills nothing.
+#pragma unroll 1
+      for (int h = 0; h < 2; ++h) {
+        epilogue_tile<BN, T3, DACT>(p, t, acc, h * 64 + wq * 16, cog, bias_s, my_stage, p.tile_w, p.tile_h);
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) acc[j] = acc[BN / 2 + j];
+      }
     }
   }
 }
@@ -609,11 +644,12 @@ constexpr int HALO_BYTES = HALO_W * HALO_H * BK * 2;     // 23040
 constexpr int HALO_SLOT = 23552;                        // rounded up to the 1024-byte swizzle atom
 constexpr int HALO_MAX_SLOTS = 6;
 constexpr int SMEM_LIMIT = 232448;                      // 227 KB opt-in maximum per CTA
+constexpr int HALO_THREADS = (EPI_WARPS + 1) * 32;      // two consumer warpgroups (64 accumulator rows each) + the TMA warp
 
 __host__ __device__ constexpr int halo_w_bytes(int bn, int chunks_total) { return 9 * chunks_total * 2 * bn * BK * 2; }
 
 template <int BN>
-__global__ void __launch_bounds__(THREADS, 1) conv3x3_halo_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p,
+__global__ void __launch_bounds__(HALO_THREADS, 1) conv3x3_halo_kernel(const __grid_constant__ Maps maps, const __grid_constant__ Params p,
                                                                   const int nslots) {
   constexpr int W_TILE = Cfg<BN>::W_TILE;
   extern __shared__ uint8_t smem_raw[];
@@ -1027,9 +1063,9 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
     const int hgrid = htiles < num_sms() ? static_cast<int>(htiles) : num_sms();
     const int hsmem = 1024 + halo_w_bytes(bn, chunks_all) + halo_slots * HALO_SLOT + 256 + MAX_COUT * 4 + EPI_WARPS * EPI_STAGE;
     if (bn == 32)
-      conv3x3_halo_kernel<32><<<hgrid, THREADS, hsmem, stream>>>(maps, p, halo_slots);
+      conv3x3_halo_kernel<32><<<hgrid, HALO_THREADS, hsmem, stream>>>(maps, p, halo_slots);
     else
-      conv3x3_halo_kernel<64><<<hgrid, THREADS, hsmem, stream>>>(maps, p, halo_slots);
+      conv3x3_halo_kernel<64><<<hgrid, HALO_THREADS, hsmem, stream>>>(maps, p, halo_slots);
     count_launch();
     return static_cast<int>(cudaGetLastError());
   }

@@ -41,17 +41,6 @@ constexpr int SMEM = STAGES * STAGE + CONSUMER_WARPS * EPI_STAGE + 2 * BN * 4 + 
 // EPI_BAR + w = warpgroup w alone, 128 threads
 constexpr int ORDER_BAR = 1, EPI_BAR = 3;
 
-__device__ __forceinline__ void named_sync(int id, int threads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
-}
-__device__ __forceinline__ void named_arrive(int id, int threads) {
-  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
-}
-template <int REGS>
-__device__ __forceinline__ void regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
-template <int REGS>
-__device__ __forceinline__ void regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS)); }
-
 // Epilogue of the calling warp's 16 rows [row0, row0 + 16) x the tile's 128 columns from n0, read from the warp's
 // fragments `acc` of one m64n128 accumulator: out = acc + bias (+ residual), fp32 or fp16.  bias_s = the tile's 128
 // bias values in shared memory (zeros when the layer has none).  Each 32-column chunk goes through `stage`, 2 KB

@@ -38,10 +38,15 @@ SHAPES = [
     ("x dec3 64->32 f32", 64, [64], 240, 432, 32, 1, 3, 1, "f32"),
     ("x dec3 64->8 f32", 64, [64], 240, 432, 8, 1, 3, 1, "f32"),
     ("x dec2 64->64 f32", 64, [64], 240, 432, 64, 1, 3, 1, "f32"),
-]
+    # per-tile fixed cost: same output (64 images at 60 x 108 = 54 tiles of 12 x 10 each), K = 9 cin / 64 blocks per
+    # tile; the intercept of time against K is what a tile costs besides its MMAs (epilogue, pipeline refill).  Not in
+    # the total; the fit uses K <= 72 (at cin 1024 the time leaves the straight line)
+] + [(f"x ksweep {c}->{co}", 64, [c], 60, 108, co, 1, 3, 1, "split") for co in (128, 64) for c in (64, 128, 256, 512, 1024)]
+SWEEP_TILES, SWEEP_MAX_KB = 64 * 54, 72
 only = sys.argv[1] if len(sys.argv) > 1 else ""
 g = torch.Generator(device="cpu").manual_seed(0)
 total = 0.0
+sweep = {}
 for name, n, cins, h, w, cout, groups, ks, stride, out in SHAPES:
     if only and only not in name:
         continue
@@ -66,7 +71,22 @@ for name, n, cins, h, w, cout, groups, ks, stride, out in SHAPES:
         us = e0.elapsed_time(e1) / reps * 1e3
         ho, wo = (h + 2 * (ks // 2) - ks) // stride + 1, (w + 2 * (ks // 2) - ks) // stride + 1
         flops = 2.0 * n * ho * wo * cout * (sum(cins) // groups) * ks * ks
-        total += us if tag or len(variants) == 1 else 0.0
         print(f"CONV {name + tag:30s} {us:9.1f} us  {flops / us / 1e6:8.1f} TFLOP/s")
+        if name.startswith("x ksweep"):
+            if 9 * cins[0] // 64 <= SWEEP_MAX_KB:
+                sweep.setdefault(cout, []).append((9 * cins[0] // 64, us))
+        else:
+            total += us if tag or len(variants) == 1 else 0.0
     del srcs, variants
 print(f"CONV total {total / 1e3:.2f} ms")
+sms = torch.cuda.get_device_properties(dev).multi_processor_count
+for cout, pts in sweep.items():
+    if len(pts) < 2:
+        continue
+    kb = torch.tensor([p[0] for p in pts], dtype=torch.float64)
+    us = torch.tensor([p[1] for p in pts], dtype=torch.float64)
+    slope = float(((kb - kb.mean()) * (us - us.mean())).sum() / ((kb - kb.mean()) ** 2).sum())
+    icpt = float(us.mean() - slope * kb.mean())
+    per_cta = SWEEP_TILES / sms                        # tiles per persistent CTA
+    print(f"CONV ksweep Cout {cout}: {icpt:.1f} us + {slope:.2f} us per K block of every tile; per tile "
+          f"{icpt / per_cta:.2f} us fixed + {slope / per_cta:.3f} us per K block ({per_cta:.1f} tiles per CTA)")
