@@ -26,111 +26,23 @@ Reachability (dispatch as of this file): conv3x3_halo_kernel<64> is never chosen
 fewer than three halo slots), nor is the HALO kernel with more than one K chunk; conv_kxn_kernel<true, 7, *> is never
 chosen (the kx-in-N halo variant is taken for 3x3 kernels only).  Tests for those paths belong with a change that makes
 them reachable."""
-import json
 import math
-import os
-import re
-import tempfile
-from collections import namedtuple
 
 import pytest
 import torch
 import torch.nn.functional as F
 
 from e2fgvi_b200 import ops
+from kernel_checks import (cdiv as _cdiv, check_close, conv_bn, conv_tile, expect_schedule, generic_tiles, halo_tiles, images_for, kxn_tiles, persistent_launch, print_tables, run_traced,
+                           same_launch as _same_launch, sms)
 
 pytestmark = pytest.mark.gpu
-
-C = 2.0 ** -14
-ROUND = {"f32": 0.0, "f16": 2.0 ** -11, "split": 2.0 ** -16}   # relative rounding of the stored output format
-
-Launch = namedtuple("Launch", "name grid smem")
-PERSISTENT = re.compile(r"^(linear_kernel|conv3x3_kernel|conv3x3_halo_kernel|conv_kxn_kernel)<")
-_TABLE = []
-_MARGINS = {}      # check -> worst err / (C * A + rounding) over its elements
-
-
-# ------------------------------------------------------------------------------------------------ which kernel ran
-_LITERALS = [(re.compile(r"\(bool\)0"), "false"), (re.compile(r"\(bool\)1"), "true"),
-             (re.compile(r"\((?:unsigned )?int\)(-?\d+)"), r"\1")]
-
-
-def _short(name):
-    """'void e2f::conv::conv3x3_kernel<(int)96, (bool)0>(e2f::conv::Maps, ...)' -> 'conv3x3_kernel<96, false>'."""
-    for pat, rep in _LITERALS:
-        name = pat.sub(rep, name)
-    m = re.search(r"(\w+)\s*(<[^()]*>)?\s*\(", name)
-    if m is None:
-        return name
-    return m.group(1) + re.sub(r"\s*,\s*", ", ", m.group(2) or "")
-
-
-def run_traced(fn):
-    """Run ``fn`` under torch.profiler (CUDA activity); return (its result, [Launch(name, grid, smem)] in launch
-    order) read from the Kineto trace, which records each kernel's grid and shared memory."""
-    torch.cuda.synchronize()
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        result = fn()
-        torch.cuda.synchronize()
-    with tempfile.TemporaryDirectory() as d:
-        path = os.path.join(d, "trace.json")
-        prof.export_chrome_trace(path)
-        with open(path) as f:
-            events = json.load(f)["traceEvents"]
-    kernels = sorted((e for e in events if e.get("cat") == "kernel"), key=lambda e: e.get("ts", 0))
-    return result, [Launch(_short(e["name"]), tuple(e.get("args", {}).get("grid", ())),
-                           e.get("args", {}).get("shared memory")) for e in kernels]
-
-
-def persistent_launch(launches):
-    """The one persistent GEMM launch among ``launches`` (split / pack kernels around it are ignored)."""
-    hits = [k for k in launches if PERSISTENT.match(k.name)]
-    assert len(hits) == 1, [k.name for k in launches]
-    return hits[0]
-
-
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def expect_schedule(case, launch, kernel, tiles):
-    """Assert the instantiation and grid == min(tiles, SMs); record the row of the schedule table."""
-    s = sms()
-    assert launch.name == kernel, (launch.name, kernel)
-    grid = min(tiles, s)
-    assert launch.grid == (grid, 1, 1), (launch.grid, tiles, s)
-    _TABLE.append((case, kernel, grid, tiles, -(-tiles // grid), launch.smem))
-    return -(-tiles // grid)
 
 
 @pytest.fixture(scope="module", autouse=True)
 def schedule_table():
     yield
-    if _TABLE:
-        print(f"\n{'case':44s} {'kernel':34s} {'grid':>5s} {'tiles':>6s} {'tiles/CTA':>9s} {'smem':>7s}")
-        for row in _TABLE:
-            print(f"{row[0]:44s} {row[1]:34s} {row[2]:5d} {row[3]:6d} {row[4]:9d} {str(row[5]):>7s}")
-    if _MARGINS:
-        print("\nworst |got - ref| / (C * A + rounding) per check")
-        for what, ratio in _MARGINS.items():
-            print(f"{what:44s} {ratio:.3f}")
-
-
-def check_close(got, ref, bound, tol, out_fmt="f32", what=""):
-    """rel-of-max < tol, and per element |got - ref| <= C * bound + ROUND[out_fmt] * |ref|."""
-    got = got.double()
-    assert got.shape == ref.shape, (what, got.shape, ref.shape)
-    err = (got - ref).abs()
-    lim = C * bound + ROUND[out_fmt] * ref.abs()
-    worst = (err / lim.clamp_min(1e-300)).max().item()
-    _MARGINS[what] = worst
-    assert worst <= 1.0, (what, int((err > lim).sum()), worst)
-    rel = (err.max() / ref.abs().max().clamp_min(1e-30)).item()
-    assert rel < tol, (what, rel)
-
-
-def _cdiv(a, b):
-    return -(-a // b)
+    print_tables()
 
 
 # ------------------------------------------------------------------------------------------------ linear
@@ -219,53 +131,7 @@ def test_linear_split_operand_with_pitch(cuda):
     check_close(got.reshape(m, n), ref, bound, 5e-5, "f32", "split pitch")
 
 
-# ------------------------------------------------------------------------------------------------ conv: tile arithmetic
-def conv_tile(h, w, stride=1):
-    """(tile_w, tile_h) that launch_conv3x3 / launch_conv3d pick for an h x w output grid (dense sources)."""
-    if w < 16 or h < 8:
-        return min(w, 16), min(h, 8)
-    best, tw, th = _cdiv(h, 8) * _cdiv(w, 16), 16, 8
-    for t in range(32, 7, -1):
-        u = 128 // t
-        if u < 4 or u > h or t > w or t * stride > 256 or u * stride > 256:
-            continue
-        cnt = _cdiv(h, u) * _cdiv(w, t)
-        if cnt < best:
-            best, tw, th = cnt, t, u
-    return tw, th
-
-
-def conv_bn(cog):
-    return 32 if cog <= 32 else 64 if cog <= 64 else 96 if cog == 96 else 128
-
-
-def generic_tiles(n, oh, ow, cout, groups=1, stride=1, tile=None):
-    """(BN, tiles) of conv3x3_kernel for an oh x ow output (incl. the N-tile halving for launches of few tiles)."""
-    tw, th = tile or conv_tile(oh, ow, stride)
-    cog = cout // groups
-    bn = conv_bn(cog)
-    per = n * _cdiv(oh, th) * _cdiv(ow, tw) * groups
-    if bn == 128 and cog % 64 == 0 and 2 * per * _cdiv(cog, 128) <= sms():
-        bn = 64
-    return bn, per * _cdiv(cog, bn)
-
-
-def halo_tiles(n, h, w):
-    return n * _cdiv(h, 16) * _cdiv(w, 8)
-
-
-def kxn_tiles(n, h, w, ks, groups=1):
-    return n * _cdiv(h, 4) * _cdiv(w, 32 - 2 * (ks // 2)) * groups
-
-
-def images_for(tiles_of, want):
-    """Smallest image count n with tiles_of(n) >= want."""
-    n = 1
-    while tiles_of(n) < want:
-        n += 1
-    return n
-
-
+# ------------------------------------------------------------------------------------------------ conv
 def conv_ref(x64, w64, b64, groups=1, stride=1, pad=1, slope=1.0, r64=None, tanh=False):
     """(reference, bound A) of leaky_relu(conv(x) + b) (+ r) (-> tanh) in float64.  LeakyReLU and tanh are
     1-Lipschitz, so the pre-activation's bound holds after them."""
@@ -512,12 +378,6 @@ def test_conv3d_multi_tile(cuda, cin, cout, k):
 
 
 # ------------------------------------------------------------------------------------------------ bitwise schedule invariance
-def _same_launch(la, lb):
-    a, b = persistent_launch(la), persistent_launch(lb)
-    assert (a.name, a.grid) == (b.name, b.grid), (a, b)
-    return a
-
-
 def test_linear_row_permutation_bitwise(cuda):
     """attn.qkv (fp16) and attn.proj (+ residual, fp32) of the 8-clip step, M = 46,080 token rows: permuting the rows
     permutes the result bit for bit; sampled rows equal a one-row call."""
