@@ -1,5 +1,5 @@
 // extern "C" boundary of libe2fgvi_b200.so (declared in include/e2fgvi_b200.h): argument validation, error
-// strings, launch accounting.  No torch types, no allocation; the only process-wide state is per-device-ordinal caches
+// strings, launch accounting, TMA tensor-map encoding.  No torch types, no allocation; the only process-wide state is per-device-ordinal caches
 // of immutable facts (SM count, "function attributes already set on device d", cluster occupancy; launch.h DeviceOnce).
 #include <atomic>
 #include <cstdarg>
@@ -33,6 +33,34 @@ void set_error(const char* fmt, ...) {
   va_start(ap, fmt);
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
+}
+
+int encode_tmap(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
+                const cuuint32_t* box, const cuuint32_t* estr, const char* what, CUtensorMapDataType type) {
+  using EncodeTiledFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+  static const EncodeTiledFn encode = [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess) p = nullptr;
+    return reinterpret_cast<EncodeTiledFn>(p);
+  }();
+  if (!encode) {
+    set_error("%s: cuTensorMapEncodeTiled is not available from the driver", what);
+    return -4;
+  }
+  const CUresult r = encode(map, type, static_cast<cuuint32_t>(rank), const_cast<void*>(base), dims, strides, box, estr,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    char shape[128] = "";
+    for (int i = 0, len = 0; i < rank; ++i)
+      len += snprintf(shape + len, sizeof(shape) - len, "%s%llu", i ? " x " : "", static_cast<unsigned long long>(dims[i]));
+    set_error("%s: cuTensorMapEncodeTiled failed with CUresult %d (dims %s)", what, static_cast<int>(r), shape);
+    return -4;
+  }
+  return 0;
 }
 
 static int finish(int status, const char* what) {

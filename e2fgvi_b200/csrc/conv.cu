@@ -113,22 +113,6 @@ struct Params {
 
 constexpr int EPI_TANH = 1, EPI_NCHW = 2;     // both only on the element-wise store path (Cout % 4 != 0: the 3-channel output conv)
 
-__device__ __forceinline__ void tma_load_4d(uint32_t smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2,
-                                            int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-
-__device__ __forceinline__ void tma_load_5d(uint32_t smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2,
-                                            int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-
 struct TileCoord {
   int n, y0, x0, g, co0;   // co0: first output channel of the tile (global index)
   int ph, oy, ox;          // phase and its output-pixel offset
@@ -777,20 +761,6 @@ __global__ void __launch_bounds__(HALO_THREADS, 1) conv3x3_halo_kernel(const __g
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess) p = nullptr;
-    return reinterpret_cast<EncodeTiledFn>(p);
-  }();
-  return fn;
-}
-
 // NCHW fp32 (C <= cin channels) -> row-gapped NHWC bf16 (hi, lo) [N][H][lead + W][cin] + tail, zeros in the gaps, the
 // tail and channels >= C: the operand layout of the window-packed conv.  One thread per (row pixel incl. gap, n*H+y).
 __global__ void __launch_bounds__(256) pack_rows_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ hi,
@@ -814,6 +784,94 @@ __global__ void __launch_bounds__(256) pack_rows_kernel(const float* __restrict_
     const __nv_bfloat162 l0 = __floats2bfloat162_rn(f[0] - g0.x, f[1] - g0.y), l1 = __floats2bfloat162_rn(f[2] - g1.x, f[3] - g1.y);
     *reinterpret_cast<uint2*>(hi + i * cin + c0) = make_uint2(*reinterpret_cast<const uint32_t*>(&h0), *reinterpret_cast<const uint32_t*>(&h1));
     *reinterpret_cast<uint2*>(lo + i * cin + c0) = make_uint2(*reinterpret_cast<const uint32_t*>(&l0), *reinterpret_cast<const uint32_t*>(&l1));
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Host side shared by the generic kernel's three launchers: launch_conv3x3 (2-D and gather convs), launch_conv3d (I3D)
+// and launch_dis_conv (the discriminator).
+
+// Tile shape of an h x w GEMM grid.  Images smaller than a 16 x 8 tile (SPyNet's coarse pyramid levels: 2x4, 4x8 pixels)
+// take a tile of their own size: the A boxes shrink from 16 KB to 1-4 KB per K block, and these few-CTA launches are
+// bound by the per-SM L2 port.  Otherwise, unless `search` is off (a row-gapped source keeps 16 x 8), the
+// tile_w x tile_h <= 128 box that covers the image with the FEWEST tiles: at 60 x 108 (every propagation / encoder conv
+// of a 432x240 clip) 12 x 10 tiles the image exactly with 54 tiles where 16 x 8 needs 56 — at 8 clips that is 432
+// instead of 448 tiles.  The candidates have tw <= 32 and th <= 16, and every launcher that searches runs at stride 1
+// or 2, so a source box (tile * stride elements per axis) stays within TMA's 256 without a check here.
+static void pick_tile(int h, int w, bool search, int& tile_w, int& tile_h) {
+  tile_w = w < TILE_W ? w : TILE_W;
+  tile_h = h < TILE_H ? h : TILE_H;
+  if (w < TILE_W || h < TILE_H || !search) return;
+  long long best = static_cast<long long>((h + TILE_H - 1) / TILE_H) * ((w + TILE_W - 1) / TILE_W);
+  for (int tw = 32; tw >= 8; --tw) {                        // ties go to the wider tile (longer contiguous TMA rows)
+    const int th = BM / tw;
+    if (th < 4 || th > h || tw > w) continue;
+    const long long cnt = static_cast<long long>((h + th - 1) / th) * ((w + tw - 1) / tw);
+    if (cnt < best) {
+      best = cnt;
+      tile_w = tw;
+      tile_h = th;
+    }
+  }
+}
+
+// N tile (see Cfg) for `cog` output channels per group, the same rule for every launcher.  The N tile only splits the
+// output channels: no element's K summation depends on it, so a layer computes the same bits at any BN.  (The
+// discriminator's layers have 8-128 channels but never 96.)
+static int pick_bn(int cog) { return cog <= 32 ? 32 : cog <= 64 ? 64 : cog == 96 ? 96 : 128; }
+
+// the hi and lo maps of one bf16 operand pair: the same geometry over two buffers
+static int encode_pair(CUtensorMap& map_hi, CUtensorMap& map_lo, const void* hi, const void* lo, int rank,
+                       const cuuint64_t* dims, const cuuint64_t* strides, const cuuint32_t* box, const cuuint32_t* estr,
+                       const char* what) {
+  const int e = encode_tmap(&map_hi, hi, rank, dims, strides, box, estr, what);
+  return e ? e : encode_tmap(&map_lo, lo, rank, dims, strides, box, estr, what);
+}
+
+// weights [Cout][kpad] bf16 (hi, lo), K blocks in the order the producer walks them: one {64, BN} box per K block
+static int encode_weights(Maps& maps, const void* w_hi, const void* w_lo, int kpad, int cout, int bn, const char* what) {
+  const cuuint64_t dims[2] = {static_cast<cuuint64_t>(kpad), static_cast<cuuint64_t>(cout)};
+  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(kpad) * 2};
+  const cuuint32_t box[2] = {BK, static_cast<cuuint32_t>(bn)};
+  const cuuint32_t estr[2] = {1, 1};
+  return encode_pair(maps.w_hi, maps.w_lo, w_hi, w_lo, 2, dims, strides, box, estr, what);
+}
+
+// one instantiation, its shared-memory size set once per device
+template <int BN, bool T3, bool DACT>
+static int launch_bn(const Maps& maps, const Params& p, int grid, cudaStream_t stream) {
+  const auto kern = [] {
+    if constexpr (DACT) return conv3x3_dact_kernel<BN>;
+    else return conv3x3_kernel<BN, T3>;
+  }();
+  static DeviceOnce configured;
+  if (const int e = configure_once(configured, Cfg<BN>::SMEM, kern)) return e;
+  kern<<<grid, THREADS, Cfg<BN>::SMEM, stream>>>(maps, p);
+  count_launch();
+  return static_cast<int>(cudaGetLastError());
+}
+
+// The launchers' common tail: count p's tiles over n images as the kernel does, size the persistent grid and launch the
+// instantiation for bn (the DACT kernel exists for BN 32 and 64: Cout <= 64).
+template <bool T3, bool DACT = false>
+static int launch_tiles(const Maps& maps, const Params& p, long long n, int bn, const char* who, cudaStream_t stream) {
+  const long long tiles = n * ((p.H + p.tile_h - 1) / p.tile_h) * ((p.W + p.tile_w - 1) / p.tile_w) * p.nphase * p.groups *
+                          ((p.Cout / p.groups + bn - 1) / bn);
+  if (tiles == 0) return 0;
+  if (tiles > 0x7FFFFFFFLL) {
+    set_error("%s: too many tiles", who);
+    return -2;
+  }
+  const int grid = tiles < num_sms() ? static_cast<int>(tiles) : num_sms();
+  if constexpr (DACT) {
+    return bn == 32 ? launch_bn<32, T3, true>(maps, p, grid, stream) : launch_bn<64, T3, true>(maps, p, grid, stream);
+  } else {
+    switch (bn) {
+      case 32: return launch_bn<32, T3, false>(maps, p, grid, stream);
+      case 64: return launch_bn<64, T3, false>(maps, p, grid, stream);
+      case 96: return launch_bn<96, T3, false>(maps, p, grid, stream);
+      default: return launch_bn<128, T3, false>(maps, p, grid, stream);
+    }
   }
 }
 
@@ -856,48 +914,20 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
   // GEMM grid = output size of the plain conv, or what the generalised geometry says
   const int h = geom ? geom->grid_h : (h_in + 2 * pad - ks) / stride + 1;
   const int w = geom ? geom->grid_w : (w_in + 2 * pad - ks) / stride + 1;
-  // Tile shape.  Images smaller than a 16 x 8 tile (SPyNet's coarse pyramid levels: 2x4, 4x8 pixels) take a tile of their
-  // own size: the A boxes shrink from 16 KB to 1-4 KB per K block, and these few-CTA launches are bound by the per-SM L2
-  // port.  Otherwise the tile_w x tile_h <= 128 box that covers the image with the FEWEST tiles: at 60 x 108 (every
-  // propagation / encoder conv of a 432x240 clip) 12 x 10 tiles the image exactly with 54 tiles where 16 x 8 needs 56 —
-  // at 8 clips that is 432 instead of 448 tiles.
-  int tile_w = TILE_W, tile_h = TILE_H;
-  if (geom) {
-    tile_w = geom->tile_w;
-    tile_h = geom->tile_h;
-  } else if (w < TILE_W || h < TILE_H) {
-    tile_w = w < TILE_W ? w : TILE_W;
-    tile_h = h < TILE_H ? h : TILE_H;
-  } else if (!in_rows) {
-    long long best = static_cast<long long>((h + TILE_H - 1) / TILE_H) * ((w + TILE_W - 1) / TILE_W);
-    for (int tw = 32; tw >= 8; --tw) {                        // ties go to the wider tile (longer contiguous TMA rows)
-      const int th = BM / tw;
-      if (th < 4 || th > h || tw > w || tw * stride > 256 || th * stride > 256) continue;
-      const long long cnt = static_cast<long long>((h + th - 1) / th) * ((w + tw - 1) / tw);
-      if (cnt < best) {
-        best = cnt;
-        tile_w = tw;
-        tile_h = th;
-      }
-    }
-  }
+  int tile_w = geom ? geom->tile_w : 0, tile_h = geom ? geom->tile_h : 0;
+  if (!geom) pick_tile(h, w, !in_rows, tile_w, tile_h);
   const int ntaps = geom ? geom->ntaps : ks * ks;
   if (ntaps < 1 || ntaps > 64 || tile_w < 1 || tile_h < 1 || tile_w * tile_h > BM || tile_w * stride > 256 ||
       tile_h * stride > 256 || (geom && (geom->nphase < 1 || geom->nphase > 9 || geom->ostep < 1))) {
     set_error("conv: unsupported geometry (taps=%d tile=%dx%d stride=%d)", ntaps, tile_w, tile_h, stride);
     return -2;
   }
-  EncodeTiledFn enc = get_encode();
-  if (!enc) {
-    set_error("cuTensorMapEncodeTiled is not available from the driver");
-    return -4;
-  }
   if (cout > MAX_COUT) {
     set_error("conv3x3: at most %d output channels (the bias is staged in shared memory), got %d", MAX_COUT, cout);
     return -2;
   }
   const int cog = cout / groups;
-  int bn = cog <= 32 ? 32 : (cog <= 64 ? 64 : (cog == 96 ? 96 : 128));
+  int bn = pick_bn(cog);
   // few tiles (single-clip propagation steps: 51 pixel tiles): halve the N tile so that twice as many SMs work
   if (bn == 128 && cog % 64 == 0 && !in_rows) {
     const long long t128 = static_cast<long long>(n) * ((h + tile_h - 1) / tile_h) * ((w + tile_w - 1) / tile_w) * groups *
@@ -906,17 +936,15 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
   }
   Maps maps;
   Params p;
+  memset(&p, 0, sizeof(p));
   p.N = n; p.H = h; p.W = w; p.Cout = cout; p.groups = groups; p.nsrc = nsrc;
   p.ks = ks; p.stride = stride; p.pad = pad;
   p.slope = slope; p.bias = bias; p.residual = residual; p.out = out; p.epi_flags = epi_flags;
   p.out_cs = cout;
   p.out_hi = static_cast<__nv_bfloat16*>(out_hi); p.out_lo = static_cast<__nv_bfloat16*>(out_lo);
-  p.chunks_total = 0;
-  p.rows_px = p.rows_g = 0;
   p.out_lead = out_lead;
   p.tile_w = tile_w; p.tile_h = tile_h;
-  p.bias_map = nullptr;
-  p.dact = static_cast<const __nv_bfloat16*>(dact); p.dact_slope = 0.f; p.dact_lead = dact_lead;
+  p.dact = static_cast<const __nv_bfloat16*>(dact); p.dact_lead = dact_lead;
   if (geom) {
     p.nphase = geom->nphase; p.ostep = geom->ostep; p.out_H = geom->out_h; p.out_W = geom->out_w;
     p.bias_map = geom->bias_map;
@@ -926,7 +954,7 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
   } else {
     p.nphase = 1; p.ostep = 1; p.out_H = h; p.out_W = w;
     for (int i = 0; i < ntaps; ++i) { p.tap_dy[i] = static_cast<int8_t>(i / ks - pad); p.tap_dx[i] = static_cast<int8_t>(i % ks - pad); }
-    p.ph_tap0[0] = 0; p.ph_tap0[1] = static_cast<uint8_t>(ntaps); p.ph_oy[0] = p.ph_ox[0] = 0;
+    p.ph_tap0[1] = static_cast<uint8_t>(ntaps);
   }
   p.out_pitch = conv_rows_pitch(p.out_W, out_lead, cout);   // == out_W + out_lead: split outputs have >= 8 channels
   p.out_nstride = static_cast<long long>(p.out_H) * p.out_W;
@@ -941,119 +969,72 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
   p.out_tail = out_lead ? conv_rows_tail(out_lead, cout) : 0;
   p.dact_pitch = dact_lead ? conv_rows_pitch(p.out_W, dact_lead, cout) : p.out_W;
   p.dact_nstride = static_cast<long long>(p.out_H) * p.dact_pitch;
-  for (int i = 0; i < MAX_SRC; ++i) p.cig[i] = p.chunks[i] = 0;
+  long long src_nstride[MAX_SRC];                            // pixels between consecutive images of each dense source
   if (in_rows) {
-    // ONE row-gapped source [N][H][w_in + pad][cin] (+ tail): dimension 1 steps by `stride` pixels, dimension 0 spans
-    // 64 elements = 64/cin pixels (overlapping windows; validated by tools/tma_window_probe.cu)
-    const int cin = src_channels[0];
-    p.rows_px = BK / cin;
+    p.rows_px = BK / src_channels[0];
     p.rows_g = (ks + p.rows_px - 1) / p.rows_px;
-    p.cig[0] = cin;
-    p.chunks[0] = 1;
-    p.chunks_total = 1;
-    const int pitch = conv_rows_pitch(w_in, pad, cin);
-    const cuuint64_t dims[4] = {BK, static_cast<cuuint64_t>((pitch + stride - 1) / stride), static_cast<cuuint64_t>(h_in),
-                                static_cast<cuuint64_t>(n)};
-    const cuuint64_t strides[3] = {static_cast<cuuint64_t>(stride) * cin * 2, static_cast<cuuint64_t>(pitch) * cin * 2,
-                                   static_cast<cuuint64_t>(h_in) * pitch * cin * 2};
-    const cuuint32_t box[4] = {BK, static_cast<cuuint32_t>(tile_w), static_cast<cuuint32_t>(tile_h * stride), 1};
-    const cuuint32_t estr[4] = {1, 1, static_cast<cuuint32_t>(stride), 1};
-    for (int part = 0; part < 2; ++part) {
-      CUresult r = enc(part ? &maps.a_lo[0] : &maps.a_hi[0], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4,
-                       const_cast<void*>(part ? src_lo[0] : src_hi[0]), dims, strides, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) {
-        set_error("conv2d: cuTensorMapEncodeTiled(row-gapped source) failed with CUresult %d (cin=%d w=%d h=%d n=%d)",
-                  static_cast<int>(r), cin, w_in, h_in, n);
-        return -4;
+    p.cig[0] = src_channels[0];
+    p.chunks[0] = p.chunks_total = 1;
+  } else {
+    for (int i = 0; i < nsrc; ++i) {
+      p.cig[i] = src_channels[i] / groups;
+      p.chunks[i] = (p.cig[i] + BK - 1) / BK;
+      p.chunks_total += p.chunks[i];
+      src_nstride[i] = static_cast<long long>(h_in) * w_in;
+      if (geom && geom->src_nstride && geom->src_nstride[i] > 0) {
+        if (geom->src_nstride[i] < src_nstride[i]) {
+          set_error("conv: source %d batch stride %lld is smaller than one image (%lld pixels)", i, geom->src_nstride[i],
+                    src_nstride[i]);
+          return -2;
+        }
+        src_nstride[i] = geom->src_nstride[i];
       }
     }
   }
   // HALO variant (see conv3x3_halo_kernel): dense 3x3 / s1 / p1 layers with <= 64 output channels whose weights fit
   // in shared memory next to >= 3 halo slots.  E2F_CONV_HALO=0 forces the generic kernel (A/B timing, debugging).
-  int chunks_all = 0;
-  for (int i = 0; i < nsrc; ++i) chunks_all += (src_channels[i] / groups + BK - 1) / BK;
   int halo_slots = 0;
   if (!geom && !in_rows && !dact && ks == 3 && stride == 1 && pad == 1 && groups == 1 && cout <= 64) {
     static const bool enabled = [] {
       const char* e = getenv("E2F_CONV_HALO");
       return !(e && e[0] == '0');
     }();
-    const int room = SMEM_LIMIT - 1024 - 256 - MAX_COUT * 4 - halo_w_bytes(bn, chunks_all) - EPI_WARPS * EPI_STAGE;
+    const int room = SMEM_LIMIT - 1024 - 256 - MAX_COUT * 4 - halo_w_bytes(bn, p.chunks_total) - EPI_WARPS * EPI_STAGE;
     if (enabled && room >= 3 * HALO_SLOT) halo_slots = room / HALO_SLOT < HALO_MAX_SLOTS ? room / HALO_SLOT : HALO_MAX_SLOTS;
+  }
+  if (in_rows) {
+    // ONE row-gapped source [N][H][w_in + pad][cin] (+ tail): dimension 1 steps by `stride` pixels, dimension 0 spans
+    // 64 elements = 64/cin pixels (overlapping windows; validated by tools/tma_window_probe.cu)
+    const int cin = src_channels[0], pitch = conv_rows_pitch(w_in, pad, cin);
+    const cuuint64_t dims[4] = {BK, static_cast<cuuint64_t>((pitch + stride - 1) / stride), static_cast<cuuint64_t>(h_in),
+                                static_cast<cuuint64_t>(n)};
+    const cuuint64_t strides[3] = {static_cast<cuuint64_t>(stride) * cin * 2, static_cast<cuuint64_t>(pitch) * cin * 2,
+                                   static_cast<cuuint64_t>(h_in) * pitch * cin * 2};
+    const cuuint32_t box[4] = {BK, static_cast<cuuint32_t>(tile_w), static_cast<cuuint32_t>(tile_h * stride), 1};
+    const cuuint32_t estr[4] = {1, 1, static_cast<cuuint32_t>(stride), 1};
+    if (const int e = encode_pair(maps.a_hi[0], maps.a_lo[0], src_hi[0], src_lo[0], 4, dims, strides, box, estr,
+                                  "conv2d row-gapped source"))
+      return e;
   }
   const cuuint32_t estr4[4] = {1, static_cast<cuuint32_t>(stride), static_cast<cuuint32_t>(stride), 1};
   for (int i = 0; i < (in_rows ? 0 : nsrc); ++i) {
     const int c = src_channels[i];
-    p.cig[i] = c / groups;
-    p.chunks[i] = (p.cig[i] + BK - 1) / BK;
-    p.chunks_total += p.chunks[i];
     const cuuint64_t dims[4] = {static_cast<cuuint64_t>(c), static_cast<cuuint64_t>(w_in),
                                 static_cast<cuuint64_t>(h_in), static_cast<cuuint64_t>(n)};
-    long long nstride = static_cast<long long>(h_in) * w_in;                       // pixels between consecutive images
-    if (geom && geom->src_nstride && geom->src_nstride[i] > 0) {
-      if (geom->src_nstride[i] < nstride) {
-        set_error("conv: source %d batch stride %lld is smaller than one image (%lld pixels)", i, geom->src_nstride[i], nstride);
-        return -2;
-      }
-      nstride = geom->src_nstride[i];
-    }
     const cuuint64_t strides[3] = {static_cast<cuuint64_t>(c) * 2, static_cast<cuuint64_t>(w_in) * c * 2,
-                                   static_cast<cuuint64_t>(nstride) * c * 2};
+                                   static_cast<cuuint64_t>(src_nstride[i]) * c * 2};
     // the box spans TILE*stride input elements and is traversed with elementStrides = stride: TILE elements land
     const cuuint32_t box[4] = {BK, static_cast<cuuint32_t>(halo_slots ? HALO_W : tile_w * stride),
                                static_cast<cuuint32_t>(halo_slots ? HALO_H : tile_h * stride), 1};
-    for (int part = 0; part < 2; ++part) {
-      CUresult r = enc(part ? &maps.a_lo[i] : &maps.a_hi[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4,
-                       const_cast<void*>(part ? src_lo[i] : src_hi[i]), dims, strides, box, estr4,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) {
-        set_error("conv2d: cuTensorMapEncodeTiled(source %d) failed with CUresult %d (c=%d w=%d h=%d n=%d)", i,
-                  static_cast<int>(r), c, w_in, h_in, n);
-        return -4;
-      }
-    }
+    if (const int e = encode_pair(maps.a_hi[i], maps.a_lo[i], src_hi[i], src_lo[i], 4, dims, strides, box, estr4,
+                                  "conv2d source"))
+      return e;
   }
-  {
-    const int kpad = (in_rows ? ks * p.rows_g : ntaps * p.chunks_total) * BK;
-    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(kpad), static_cast<cuuint64_t>(cout)};
-    const cuuint64_t strides[1] = {static_cast<cuuint64_t>(kpad) * 2};
-    const cuuint32_t box[2] = {BK, static_cast<cuuint32_t>(bn)};
-    const cuuint32_t estr[2] = {1, 1};
-    for (int part = 0; part < 2; ++part) {
-      CUresult r = enc(part ? &maps.w_lo : &maps.w_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
-                       const_cast<void*>(part ? w_lo : w_hi), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) {
-        set_error("conv3x3: cuTensorMapEncodeTiled(weight) failed with CUresult %d", static_cast<int>(r));
-        return -4;
-      }
-    }
-  }
-  static DeviceOnce configured, halo_configured;
-  const int dev = current_device();
-  if (!device_done(configured, dev)) {
-    cudaError_t e = cudaFuncSetAttribute(conv3x3_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<128>::SMEM);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(conv3x3_kernel<96, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<96>::SMEM);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(conv3x3_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64>::SMEM);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(conv3x3_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<32>::SMEM);
-    if (e != cudaSuccess) return static_cast<int>(e);
-    device_mark(configured, dev);
-  }
+  const int kpad = (in_rows ? ks * p.rows_g : ntaps * p.chunks_total) * BK;
+  if (const int e = encode_weights(maps, w_hi, w_lo, kpad, cout, bn, "conv3x3 weight")) return e;
   if (halo_slots) {
-    if (!device_done(halo_configured, dev)) {
-      cudaError_t e = cudaFuncSetAttribute(conv3x3_halo_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
-      if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(conv3x3_halo_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
-      if (e != cudaSuccess) return static_cast<int>(e);
-      device_mark(halo_configured, dev);
-    }
+    static DeviceOnce halo_configured;
+    if (const int e = configure_once(halo_configured, SMEM_LIMIT, conv3x3_halo_kernel<64>, conv3x3_halo_kernel<32>)) return e;
     const long long htiles = static_cast<long long>(n) * ((h + HTILE_H - 1) / HTILE_H) * ((w + HTILE_W - 1) / HTILE_W);
     if (htiles == 0) return 0;
     if (htiles > 0x7FFFFFFFLL) {
@@ -1061,7 +1042,7 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
       return -2;
     }
     const int hgrid = htiles < num_sms() ? static_cast<int>(htiles) : num_sms();
-    const int hsmem = 1024 + halo_w_bytes(bn, chunks_all) + halo_slots * HALO_SLOT + 256 + MAX_COUT * 4 + EPI_WARPS * EPI_STAGE;
+    const int hsmem = 1024 + halo_w_bytes(bn, p.chunks_total) + halo_slots * HALO_SLOT + 256 + MAX_COUT * 4 + EPI_WARPS * EPI_STAGE;
     if (bn == 32)
       conv3x3_halo_kernel<32><<<hgrid, HALO_THREADS, hsmem, stream>>>(maps, p, halo_slots);
     else
@@ -1069,41 +1050,8 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
     count_launch();
     return static_cast<int>(cudaGetLastError());
   }
-  const int tiles_y = (h + tile_h - 1) / tile_h, tiles_x = (w + tile_w - 1) / tile_w;
-  const int tiles_ng = (cout / groups + bn - 1) / bn;
-  const long long tiles = static_cast<long long>(n) * tiles_y * tiles_x * p.nphase * groups * tiles_ng;
-  if (tiles == 0) return 0;
-  if (tiles > 0x7FFFFFFFLL) {
-    set_error("conv3x3: too many tiles");
-    return -2;
-  }
-  const int grid = tiles < num_sms() ? static_cast<int>(tiles) : num_sms();
-  if (dact) {
-    static DeviceOnce dact_configured;
-    if (!device_done(dact_configured, dev)) {
-      cudaError_t e = cudaFuncSetAttribute(conv3x3_dact_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64>::SMEM);
-      if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(conv3x3_dact_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<32>::SMEM);
-      if (e != cudaSuccess) return static_cast<int>(e);
-      device_mark(dact_configured, dev);
-    }
-    if (bn == 32)
-      conv3x3_dact_kernel<32><<<grid, THREADS, Cfg<32>::SMEM, stream>>>(maps, p);
-    else
-      conv3x3_dact_kernel<64><<<grid, THREADS, Cfg<64>::SMEM, stream>>>(maps, p);
-    count_launch();
-    return static_cast<int>(cudaGetLastError());
-  }
-  if (bn == 32)
-    conv3x3_kernel<32, false><<<grid, THREADS, Cfg<32>::SMEM, stream>>>(maps, p);
-  else if (bn == 64)
-    conv3x3_kernel<64, false><<<grid, THREADS, Cfg<64>::SMEM, stream>>>(maps, p);
-  else if (bn == 96)
-    conv3x3_kernel<96, false><<<grid, THREADS, Cfg<96>::SMEM, stream>>>(maps, p);
-  else
-    conv3x3_kernel<128, false><<<grid, THREADS, Cfg<128>::SMEM, stream>>>(maps, p);
-  count_launch();
-  return static_cast<int>(cudaGetLastError());
+  return dact ? launch_tiles<false, true>(maps, p, n, bn, "conv3x3", stream)
+              : launch_tiles<false>(maps, p, n, bn, "conv3x3", stream);
 }
 
 
@@ -1118,30 +1066,11 @@ int launch_conv3d(const void* src_hi, const void* src_lo, int cin, int in_rows, 
   const int t_o = (t_in + pad[0] + pad[1] - ks) / stride + 1;
   const int h = (h_in + pad[2] + pad[3] - ks) / stride + 1;
   const int w = (w_in + pad[4] + pad[5] - ks) / stride + 1;
-  EncodeTiledFn enc = get_encode();
-  if (!enc) {
-    set_error("cuTensorMapEncodeTiled is not available from the driver");
-    return -4;
-  }
-  int tile_w = TILE_W, tile_h = TILE_H;
-  if (w < TILE_W || h < TILE_H) {
-    tile_w = w < TILE_W ? w : TILE_W;
-    tile_h = h < TILE_H ? h : TILE_H;
-  } else if (!in_rows) {                                     // fewest tiles, as launch_conv3x3
-    long long best = static_cast<long long>((h + TILE_H - 1) / TILE_H) * ((w + TILE_W - 1) / TILE_W);
-    for (int tw = 32; tw >= 8; --tw) {
-      const int th = BM / tw;
-      if (th < 4 || th > h || tw > w) continue;
-      const long long cnt = static_cast<long long>((h + th - 1) / th) * ((w + tw - 1) / tw);
-      if (cnt < best) {
-        best = cnt;
-        tile_w = tw;
-        tile_h = th;
-      }
-    }
-  }
-  // the N tile depends on cout alone, so a video's result does not depend on the batch it is computed in
-  const int bn = cout <= 32 ? 32 : (cout <= 64 ? 64 : (cout == 96 ? 96 : 128));
+  int tile_w, tile_h;
+  pick_tile(h, w, !in_rows, tile_w, tile_h);
+  // the N tile depends on cout alone (no halving for few tiles, unlike launch_conv3x3), so a video's result does not
+  // depend on the batch it is computed in
+  const int bn = pick_bn(cout);
   const long long n_img = static_cast<long long>(b) * t_o;
   Maps maps;
   Params p;
@@ -1162,7 +1091,6 @@ int launch_conv3d(const void* src_hi, const void* src_lo, int cin, int in_rows, 
     p.tap_dx[i] = static_cast<int8_t>(i % ks - pad[4]);
   }
   p.ph_tap0[0] = 0; p.ph_tap0[1] = static_cast<uint8_t>(ntaps);
-  const CUtensorMapDataType bf = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   int kpad;
   if (in_rows) {
     // 4-channel rows, dimension 1 steps by 2 pixels (16 B) and dimension 0 spans the 16-pixel window; the base is moved
@@ -1177,16 +1105,11 @@ int launch_conv3d(const void* src_hi, const void* src_lo, int cin, int in_rows, 
                                    static_cast<cuuint64_t>(t_in) * h_in * pitch * 8};
     const cuuint32_t box[5] = {BK, static_cast<cuuint32_t>(tile_w), static_cast<cuuint32_t>(tile_h * stride), 1, 1};
     const cuuint32_t estr[5] = {1, 1, static_cast<cuuint32_t>(stride), 1, 1};
-    for (int part = 0; part < 2; ++part) {
-      const __nv_bfloat16* base = static_cast<const __nv_bfloat16*>(part ? src_lo : src_hi) + (lead - pad[4]) * 4;
-      CUresult r = enc(part ? &maps.a_lo[0] : &maps.a_hi[0], bf, 5, const_cast<__nv_bfloat16*>(base), dims, strides, box,
-                       estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) {
-        set_error("conv3d: cuTensorMapEncodeTiled(row-gapped source) failed with CUresult %d", static_cast<int>(r));
-        return -4;
-      }
-    }
+    const int shift = (lead - pad[4]) * 4;
+    if (const int e = encode_pair(maps.a_hi[0], maps.a_lo[0], static_cast<const __nv_bfloat16*>(src_hi) + shift,
+                                  static_cast<const __nv_bfloat16*>(src_lo) + shift, 5, dims, strides, box, estr,
+                                  "conv3d row-gapped source"))
+      return e;
     kpad = ks * ks * p.rows_g * BK;
   } else {
     p.cig[0] = cin; p.chunks[0] = (cin + BK - 1) / BK; p.chunks_total = p.chunks[0];
@@ -1197,63 +1120,12 @@ int launch_conv3d(const void* src_hi, const void* src_lo, int cin, int in_rows, 
                                    static_cast<cuuint64_t>(t_in) * h_in * w_in * cin * 2};
     const cuuint32_t box[5] = {BK, static_cast<cuuint32_t>(tile_w), static_cast<cuuint32_t>(tile_h), 1, 1};
     const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-    for (int part = 0; part < 2; ++part) {
-      CUresult r = enc(part ? &maps.a_lo[0] : &maps.a_hi[0], bf, 5, const_cast<void*>(part ? src_lo : src_hi), dims, strides,
-                       box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) {
-        set_error("conv3d: cuTensorMapEncodeTiled(source) failed with CUresult %d (c=%d w=%d h=%d t=%d b=%d)",
-                  static_cast<int>(r), cin, w_in, h_in, t_in, b);
-        return -4;
-      }
-    }
+    if (const int e = encode_pair(maps.a_hi[0], maps.a_lo[0], src_hi, src_lo, 5, dims, strides, box, estr, "conv3d source"))
+      return e;
     kpad = ntaps * p.chunks_total * BK;
   }
-  {
-    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(kpad), static_cast<cuuint64_t>(cout)};
-    const cuuint64_t strides[1] = {static_cast<cuuint64_t>(kpad) * 2};
-    const cuuint32_t box[2] = {BK, static_cast<cuuint32_t>(bn)};
-    const cuuint32_t estr[2] = {1, 1};
-    for (int part = 0; part < 2; ++part) {
-      CUresult r = enc(part ? &maps.w_lo : &maps.w_hi, bf, 2, const_cast<void*>(part ? w_lo : w_hi), dims, strides, box,
-                       estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) {
-        set_error("conv3d: cuTensorMapEncodeTiled(weight) failed with CUresult %d", static_cast<int>(r));
-        return -4;
-      }
-    }
-  }
-  static DeviceOnce configured;
-  const int dev = current_device();
-  if (!device_done(configured, dev)) {
-    cudaError_t e = cudaFuncSetAttribute(conv3x3_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<128>::SMEM);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(conv3x3_kernel<96, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<96>::SMEM);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(conv3x3_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64>::SMEM);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(conv3x3_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<32>::SMEM);
-    if (e != cudaSuccess) return static_cast<int>(e);
-    device_mark(configured, dev);
-  }
-  const long long tiles = n_img * ((h + tile_h - 1) / tile_h) * ((w + tile_w - 1) / tile_w) * ((cout + bn - 1) / bn);
-  if (tiles == 0) return 0;
-  if (tiles > 0x7FFFFFFFLL) {
-    set_error("conv3d: too many tiles");
-    return -2;
-  }
-  const int grid = tiles < num_sms() ? static_cast<int>(tiles) : num_sms();
-  if (bn == 32)
-    conv3x3_kernel<32, true><<<grid, THREADS, Cfg<32>::SMEM, stream>>>(maps, p);
-  else if (bn == 64)
-    conv3x3_kernel<64, true><<<grid, THREADS, Cfg<64>::SMEM, stream>>>(maps, p);
-  else if (bn == 96)
-    conv3x3_kernel<96, true><<<grid, THREADS, Cfg<96>::SMEM, stream>>>(maps, p);
-  else
-    conv3x3_kernel<128, true><<<grid, THREADS, Cfg<128>::SMEM, stream>>>(maps, p);
-  count_launch();
-  return static_cast<int>(cudaGetLastError());
+  if (const int e = encode_weights(maps, w_hi, w_lo, kpad, cout, bn, "conv3d weight")) return e;
+  return launch_tiles<true>(maps, p, n_img, bn, "conv3d", stream);
 }
 
 // Temporal PatchGAN discriminator layers (Conv3d 3x5x5, stride (1, 2, 2), padding (1, pad, pad)): the T3 kernel with a
@@ -1272,31 +1144,11 @@ int launch_dis_conv(const void* src_hi, const void* src_lo, int cin, const void*
                     int cout, int pad, int transposed, float slope, const void* dact, float dact_slope, cudaStream_t stream) {
   using namespace conv;
   constexpr int KT = 3, KS = 5;
-  EncodeTiledFn enc = get_encode();
-  if (!enc) {
-    set_error("cuTensorMapEncodeTiled is not available from the driver");
-    return -4;
-  }
   const int stride = transposed ? 1 : 2;
   const int h = transposed ? (h_out + 1) / 2 : h_out, w = transposed ? (w_out + 1) / 2 : w_out;   // GEMM grid per phase
-  int tile_w = TILE_W, tile_h = TILE_H;
-  if (w < TILE_W || h < TILE_H) {
-    tile_w = w < TILE_W ? w : TILE_W;
-    tile_h = h < TILE_H ? h : TILE_H;
-  } else {                                                   // fewest tiles, as launch_conv3x3
-    long long best = static_cast<long long>((h + TILE_H - 1) / TILE_H) * ((w + TILE_W - 1) / TILE_W);
-    for (int tw = 32; tw >= 8; --tw) {
-      const int th = BM / tw;
-      if (th < 4 || th > h || tw > w) continue;
-      const long long cnt = static_cast<long long>((h + th - 1) / th) * ((w + tw - 1) / tw);
-      if (cnt < best) {
-        best = cnt;
-        tile_w = tw;
-        tile_h = th;
-      }
-    }
-  }
-  const int bn = cout <= 32 ? 32 : (cout <= 64 ? 64 : 128);
+  int tile_w, tile_h;
+  pick_tile(h, w, true, tile_w, tile_h);
+  const int bn = pick_bn(cout);
   const long long n_img = static_cast<long long>(b) * t;
   Maps maps;
   Params p;
@@ -1339,69 +1191,18 @@ int launch_dis_conv(const void* src_hi, const void* src_lo, int cin, const void*
     }
   }
   p.ph_tap0[p.nphase] = static_cast<uint8_t>(ntaps);
-  const CUtensorMapDataType bf = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   p.cig[0] = cin; p.chunks[0] = (cin + BK - 1) / BK; p.chunks_total = p.chunks[0];
-  {
-    const cuuint64_t dims[5] = {static_cast<cuuint64_t>(cin), static_cast<cuuint64_t>(w_src), static_cast<cuuint64_t>(h_src),
-                                static_cast<cuuint64_t>(t), static_cast<cuuint64_t>(b)};
-    const cuuint64_t strides[4] = {static_cast<cuuint64_t>(cin) * 2, static_cast<cuuint64_t>(w_src) * cin * 2,
-                                   static_cast<cuuint64_t>(h_src) * w_src * cin * 2,
-                                   static_cast<cuuint64_t>(t) * h_src * w_src * cin * 2};
-    const cuuint32_t box[5] = {BK, static_cast<cuuint32_t>(tile_w * stride), static_cast<cuuint32_t>(tile_h * stride), 1, 1};
-    const cuuint32_t estr[5] = {1, static_cast<cuuint32_t>(stride), static_cast<cuuint32_t>(stride), 1, 1};
-    for (int part = 0; part < 2; ++part) {
-      CUresult r = enc(part ? &maps.a_lo[0] : &maps.a_hi[0], bf, 5, const_cast<void*>(part ? src_lo : src_hi), dims, strides,
-                       box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) {
-        set_error("dis_conv: cuTensorMapEncodeTiled(source) failed with CUresult %d (c=%d w=%d h=%d t=%d b=%d)",
-                  static_cast<int>(r), cin, w_src, h_src, t, b);
-        return -4;
-      }
-    }
-  }
-  {
-    const int kpad = ntaps * p.chunks_total * BK;
-    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(kpad), static_cast<cuuint64_t>(cout)};
-    const cuuint64_t strides[1] = {static_cast<cuuint64_t>(kpad) * 2};
-    const cuuint32_t box[2] = {BK, static_cast<cuuint32_t>(bn)};
-    const cuuint32_t estr[2] = {1, 1};
-    for (int part = 0; part < 2; ++part) {
-      CUresult r = enc(part ? &maps.w_lo : &maps.w_hi, bf, 2, const_cast<void*>(part ? w_lo : w_hi), dims, strides, box,
-                       estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) {
-        set_error("dis_conv: cuTensorMapEncodeTiled(weight) failed with CUresult %d", static_cast<int>(r));
-        return -4;
-      }
-    }
-  }
-  static DeviceOnce configured;
-  const int dev = current_device();
-  if (!device_done(configured, dev)) {
-    cudaError_t e = cudaFuncSetAttribute(conv3x3_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<128>::SMEM);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(conv3x3_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64>::SMEM);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(conv3x3_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<32>::SMEM);
-    if (e != cudaSuccess) return static_cast<int>(e);
-    device_mark(configured, dev);
-  }
-  const long long tiles = n_img * ((h + tile_h - 1) / tile_h) * ((w + tile_w - 1) / tile_w) * p.nphase * ((cout + bn - 1) / bn);
-  if (tiles == 0) return 0;
-  if (tiles > 0x7FFFFFFFLL) {
-    set_error("dis_conv: too many tiles");
-    return -2;
-  }
-  const int grid = tiles < num_sms() ? static_cast<int>(tiles) : num_sms();
-  if (bn == 32)
-    conv3x3_kernel<32, true><<<grid, THREADS, Cfg<32>::SMEM, stream>>>(maps, p);
-  else if (bn == 64)
-    conv3x3_kernel<64, true><<<grid, THREADS, Cfg<64>::SMEM, stream>>>(maps, p);
-  else
-    conv3x3_kernel<128, true><<<grid, THREADS, Cfg<128>::SMEM, stream>>>(maps, p);
-  count_launch();
-  return static_cast<int>(cudaGetLastError());
+  const cuuint64_t dims[5] = {static_cast<cuuint64_t>(cin), static_cast<cuuint64_t>(w_src), static_cast<cuuint64_t>(h_src),
+                              static_cast<cuuint64_t>(t), static_cast<cuuint64_t>(b)};
+  const cuuint64_t strides[4] = {static_cast<cuuint64_t>(cin) * 2, static_cast<cuuint64_t>(w_src) * cin * 2,
+                                 static_cast<cuuint64_t>(h_src) * w_src * cin * 2,
+                                 static_cast<cuuint64_t>(t) * h_src * w_src * cin * 2};
+  const cuuint32_t box[5] = {BK, static_cast<cuuint32_t>(tile_w * stride), static_cast<cuuint32_t>(tile_h * stride), 1, 1};
+  const cuuint32_t estr[5] = {1, static_cast<cuuint32_t>(stride), static_cast<cuuint32_t>(stride), 1, 1};
+  if (const int e = encode_pair(maps.a_hi[0], maps.a_lo[0], src_hi, src_lo, 5, dims, strides, box, estr, "dis_conv source"))
+    return e;
+  if (const int e = encode_weights(maps, w_hi, w_lo, ntaps * p.chunks_total * BK, cout, bn, "dis_conv weight")) return e;
+  return launch_tiles<true>(maps, p, n_img, bn, "dis_conv", stream);
 }
 
 }  // namespace e2f

@@ -52,13 +52,6 @@ struct Params {
   __nv_bfloat16* out_lo;
 };
 
-__device__ __forceinline__ void tma_load_4d(uint32_t smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-
 // HALO = true (N <= 112 columns: the A operand dominates the L2 -> SM traffic): instead of one 4-row A box per (ky, chunk),
 // ONE box of TH + ks - 1 rows per chunk brings the tile's whole vertical halo; the A tile of tap row ky is rows
 // [32*ky, 32*ky + 128) of it — a descriptor start shifted by ky * 4096 B, a multiple of the 1024-byte swizzle atom — and only
@@ -302,20 +295,6 @@ __global__ void __launch_bounds__(THREADS, 1) conv_kxn_kernel(const __grid_const
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess) p = nullptr;
-    return reinterpret_cast<EncodeTiledFn>(p);
-  }();
-  return fn;
-}
-
 }  // namespace kxn
 
 // sources: nsrc <= 2 NHWC bf16 (hi, lo) tensors with src_c[i] stored channels (multiples of 8; for groups > 1 multiples of
@@ -326,11 +305,6 @@ int launch_conv_kxn(int nsrc, const void* const* src_hi, const void* const* src_
                     const void* w_lo, const float* bias, const float* residual, float* out, void* out_hi, void* out_lo, int n,
                     int h, int w, int cout, int groups, int co_pad, int ks, float slope, int flags, cudaStream_t stream) {
   using namespace kxn;
-  EncodeTiledFn enc = get_encode();
-  if (!enc) {
-    set_error("cuTensorMapEncodeTiled is not available from the driver");
-    return -4;
-  }
   const int NB = ks * co_pad, pad = ks / 2;
   if (nsrc < 1 || nsrc > MAX_SRC || groups < 1 || cout % groups || cout > 512) {
     set_error("conv_kxn: nsrc=%d groups=%d cout=%d", nsrc, groups, cout);
@@ -395,15 +369,10 @@ int launch_conv_kxn(int nsrc, const void* const* src_hi, const void* const* src_
     const cuuint64_t strides[3] = {static_cast<cuuint64_t>(c) * 2, static_cast<cuuint64_t>(w) * c * 2, static_cast<cuuint64_t>(h) * w * c * 2};
     const cuuint32_t box[4] = {BK, TW, static_cast<cuuint32_t>(halo ? HR : TH), 1};
     const cuuint32_t estr[4] = {1, 1, 1, 1};
-    for (int part = 0; part < 2; ++part) {
-      CUresult r = enc(part ? &maps.a_lo[i] : &maps.a_hi[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4,
-                       const_cast<void*>(part ? src_lo[i] : src_hi[i]), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) {
-        set_error("conv_kxn: cuTensorMapEncodeTiled(source %d) failed with CUresult %d", i, static_cast<int>(r));
-        return -4;
-      }
-    }
+    for (int part = 0; part < 2; ++part)
+      if (const int e = encode_tmap(part ? &maps.a_lo[i] : &maps.a_hi[i], part ? src_lo[i] : src_hi[i], 4, dims, strides, box,
+                                    estr, "conv_kxn source"))
+        return e;
   }
   {
     const int kcols = ks * p.chunks * BK;
@@ -411,27 +380,16 @@ int launch_conv_kxn(int nsrc, const void* const* src_hi, const void* const* src_
     const cuuint64_t strides[1] = {static_cast<cuuint64_t>(kcols) * 2};
     const cuuint32_t box[2] = {BK, static_cast<cuuint32_t>(NB)};
     const cuuint32_t estr[2] = {1, 1};
-    for (int part = 0; part < 2; ++part) {
-      CUresult r = enc(part ? &maps.w_lo : &maps.w_hi, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(part ? w_lo : w_hi), dims,
-                       strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) {
-        set_error("conv_kxn: cuTensorMapEncodeTiled(weight) failed with CUresult %d", static_cast<int>(r));
-        return -4;
-      }
-    }
+    for (int part = 0; part < 2; ++part)
+      if (const int e = encode_tmap(part ? &maps.w_lo : &maps.w_hi, part ? w_lo : w_hi, 2, dims, strides, box, estr,
+                                    "conv_kxn weight"))
+        return e;
   }
   static DeviceOnce cfg;
-  const int dev = current_device();
-  if (!device_done(cfg, dev)) {
-    cudaError_t e = cudaSuccess;
-    for (auto kern : {conv_kxn_kernel<false, 3, 16>, conv_kxn_kernel<false, 3, 32>, conv_kxn_kernel<false, 7, 16>,
-                      conv_kxn_kernel<false, 7, 32>, conv_kxn_kernel<true, 3, 16>, conv_kxn_kernel<true, 3, 32>,
-                      conv_kxn_kernel<true, 7, 16>, conv_kxn_kernel<true, 7, 32>})
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) return static_cast<int>(e);
-    device_mark(cfg, dev);
-  }
+  if (const int e = configure_once(cfg, 227 * 1024, conv_kxn_kernel<false, 3, 16>, conv_kxn_kernel<false, 3, 32>,
+                                   conv_kxn_kernel<false, 7, 16>, conv_kxn_kernel<false, 7, 32>, conv_kxn_kernel<true, 3, 16>,
+                                   conv_kxn_kernel<true, 3, 32>, conv_kxn_kernel<true, 7, 16>, conv_kxn_kernel<true, 7, 32>))
+    return e;
   const int step_x = TW - 2 * pad;
   const long long tiles = static_cast<long long>(n) * ((h + TH - 1) / TH) * ((w + step_x - 1) / step_x) * groups;
   if (tiles == 0) return 0;

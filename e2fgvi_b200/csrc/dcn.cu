@@ -257,20 +257,6 @@ __global__ void pack_weight_kernel(const float* __restrict__ w, __half* __restri
   wp[idx] = __float2half_rn(w[(static_cast<long long>(o) * cin + g * cpg + c) * 9 + tap]);
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess) p = nullptr;
-    return reinterpret_cast<EncodeTiledFn>(p);
-  }();
-  return fn;
-}
-
 // fp32 NHWC sources a [N][H][W][Ca], b [N][H][W][Cb] -> fp16 group-major [N][(Ca+Cb)/16][H][W][16]
 // (== torch.cat([a, b], 1).half() of feat_prop.py:126 in the layout the sampler wants); one thread per (group, pixel)
 __global__ void __launch_bounds__(256) pack_input_kernel(const float* __restrict__ a, const float* __restrict__ b,
@@ -302,12 +288,7 @@ static int launch_variant(const CUtensorMap& tmap, const void* x, const float* o
                           int M, int h, int w, float max_res, void* out_hi, void* out_lo, cudaStream_t stream) {
   auto kern = dcn_kernel<FUSED, GROUPED, OutT>;
   static DeviceOnce configured;                    // one per template instantiation, one bit per device
-  const int dev = current_device();
-  if (!device_done(configured, dev)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e != cudaSuccess) return static_cast<int>(e);
-    device_mark(configured, dev);
-  }
+  if (const int e = configure_once(configured, SMEM_BYTES, kern)) return e;
   const unsigned blocks = static_cast<unsigned>((M + BLOCK_M - 1) / BLOCK_M);
   kern<<<blocks, THREADS, SMEM_BYTES, stream>>>(tmap, static_cast<const __half*>(x), offset, mask, head,
                                                 reinterpret_cast<const float2*>(flow1),
@@ -349,23 +330,14 @@ int launch_dcn(const void* x, const float* offset, const float* mask, const floa
     set_error("N*H*W too large");
     return -2;
   }
-  EncodeTiledFn enc = get_encode();
-  if (!enc) {
-    set_error("cuTensorMapEncodeTiled is not available from the driver");
-    return -4;
-  }
   CUtensorMap tmap;
   const cuuint64_t dims[2] = {KTOT, COUT};
   const cuuint64_t strides[1] = {static_cast<cuuint64_t>(KTOT) * 2};
   const cuuint32_t box[2] = {BLOCK_K, COUT};
   const cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(&tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(w_packed), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed with CUresult %d", static_cast<int>(r));
-    return -4;
-  }
+  if (const int e = encode_tmap(&tmap, w_packed, 2, dims, strides, box, estr, "deformable conv weight",
+                                CU_TENSOR_MAP_DATA_TYPE_FLOAT16))
+    return e;
   const int Mi = static_cast<int>(M);
 #define E2F_DCN_LAUNCH(F, G, T) launch_variant<F, G, T>(tmap, x, offset, mask, head, flow1, flow2, bias, out, Mi, h, w, max_residue, out_hi, out_lo, stream)
   if (head) {

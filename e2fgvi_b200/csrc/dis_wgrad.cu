@@ -264,12 +264,7 @@ static int run_wgrad(const float* dy, const void* x_hi, const void* x_lo, float*
   using namespace wgrad;
   constexpr int TAPS = KT * KS * KS;
   static DeviceOnce configured;
-  const int dev = current_device();
-  if (!device_done(configured, dev)) {
-    const cudaError_t e = cudaFuncSetAttribute(wgrad_mma_kernel<KT, KS, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    if (e != cudaSuccess) return static_cast<int>(e);
-    device_mark(configured, dev);
-  }
+  if (const int e = configure_once(configured, SMEM, wgrad_mma_kernel<KT, KS, S>)) return e;
   const long long n_w = static_cast<long long>(cout) * TAPS * cin;
   float* wsb = work + slices * n_w;
   const long long pixels = static_cast<long long>(b) * t * h_o * w_o;

@@ -510,20 +510,11 @@ int launch_focal_attention(const void* qkv, const void* qkv_pooled, void* out, i
     return -2;
   }
   const dim3 grid((t * wh * ww + BM - 1) / BM, heads, static_cast<unsigned>(nwin));
-  cudaError_t e;
   prm.out_lo = nullptr;
   static DeviceOnce cfg;
-  const int dev = current_device();
-  if (!device_done(cfg, dev)) {
-    e = cudaFuncSetAttribute(focal_attn_kernel<SplitBf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(focal_attn_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(focal_attn_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e != cudaSuccess) return static_cast<int>(e);
-    cudaFuncSetAttribute(focal_attn_kernel<SplitBf16>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    cudaFuncSetAttribute(focal_attn_kernel<__half>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    cudaFuncSetAttribute(focal_attn_kernel<float>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    device_mark(cfg, dev);
-  }
+  if (const int e = configure_once_carveout(cfg, SMEM_BYTES, 100, focal_attn_kernel<SplitBf16>, focal_attn_kernel<__half>,
+                                            focal_attn_kernel<float>))
+    return e;
   if (out_dtype == 2) {
     prm.out_lo = static_cast<__nv_bfloat16*>(prm.out) + static_cast<size_t>(b) * t * h * w * prm.C;
     focal_attn_kernel<SplitBf16><<<grid, THREADS, SMEM_BYTES, stream>>>(prm);

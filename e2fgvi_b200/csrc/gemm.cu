@@ -288,38 +288,12 @@ __global__ void __launch_bounds__(256) split_bf16_kernel(const float* __restrict
   reinterpret_cast<uint4*>(lo)[i] = *reinterpret_cast<const uint4*>(l);
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess) p = nullptr;
-    return reinterpret_cast<EncodeTiledFn>(p);
-  }();
-  return fn;
-}
-
 static int make_map(CUtensorMap* tm, const void* base, int rows, int k, int box_rows) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) {
-    set_error("cuTensorMapEncodeTiled is not available from the driver");
-    return -4;
-  }
   const cuuint64_t dims[2] = {static_cast<cuuint64_t>(k), static_cast<cuuint64_t>(rows)};
   const cuuint64_t strides[1] = {static_cast<cuuint64_t>(k) * 2};
   const cuuint32_t box[2] = {BK, static_cast<cuuint32_t>(box_rows)};
   const cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed with CUresult %d (rows=%d k=%d)", static_cast<int>(r), rows, k);
-    return -4;
-  }
-  return 0;
+  return encode_tmap(tm, base, 2, dims, strides, box, estr, "linear operand");
 }
 
 template <typename OutT>
@@ -333,12 +307,7 @@ static int launch_variant(const void* ah, const void* al, const void* wh, const 
   if ((st = make_map(&twl, wl, n, k, BN))) return st;
   auto kern = linear_kernel<OutT>;
   static DeviceOnce cfg;
-  const int dev = current_device();
-  if (!device_done(cfg, dev)) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    if (e != cudaSuccess) return static_cast<int>(e);
-    device_mark(cfg, dev);
-  }
+  if ((st = configure_once(cfg, SMEM, kern))) return st;
   const int items = ((m + BM - 1) / BM) * ((n + BN - 1) / BN);
   const int grid = items < num_sms() ? items : num_sms();     // persistent: one CTA per SM
   kern<<<grid, THREADS, SMEM, stream>>>(tah, tal, twh, twl, bias, residual, static_cast<OutT*>(out), m, n, k);

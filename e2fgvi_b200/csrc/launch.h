@@ -1,5 +1,6 @@
 // Internal host-side launcher declarations shared by api.cu and the kernel translation units.
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <atomic>
 #include <cstdint>
@@ -28,6 +29,38 @@ int num_sms();                             // api.cu: SM count of the CURRENT de
 
 void count_launch();                       // api.cu: atomic launch counter behind e2f_launch_count()
 void set_error(const char* fmt, ...);      // api.cu: thread-local message behind e2f_last_error()
+
+// Opts `kernels` in to `smem` bytes of dynamic shared memory, once per device.  carveout >= 0 also sets the preferred
+// shared-memory carve-out (percent); that is a hint, so its result is ignored.  Returns the first cudaFuncSetAttribute
+// error, or 0; the device is marked configured only when every kernel took its size, so a failure is reported again on
+// the next call.
+template <typename... Kernels>
+int configure_once_carveout(DeviceOnce& once, int smem, int carveout, Kernels... kernels) {
+  const int dev = current_device();
+  if (device_done(once, dev)) return 0;
+  const void* const list[] = {reinterpret_cast<const void*>(kernels)...};
+  for (const void* k : list) {
+    const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return static_cast<int>(e);
+  }
+  if (carveout >= 0)
+    for (const void* k : list) cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, carveout);
+  device_mark(once, dev);
+  return 0;
+}
+template <typename... Kernels>
+int configure_once(DeviceOnce& once, int smem, Kernels... kernels) {
+  return configure_once_carveout(once, smem, -1, kernels...);
+}
+
+// api.cu: encodes a tiled TMA tensor map with the settings every kernel here uses: no interleave, 128-byte swizzle,
+// 256-byte L2 promotion, zero fill out of bounds.  dims / box / estr have `rank` entries, strides (bytes) rank - 1.  The
+// driver's entry point is looked up on the first call, so a launcher that validates its arguments before it encodes a
+// map makes no CUDA call for a rejected one.  Returns 0, or -4 with an error naming the map `what` when the driver lacks
+// the entry point or rejects the map.
+int encode_tmap(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
+                const cuuint32_t* box, const cuuint32_t* estr, const char* what,
+                CUtensorMapDataType type = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
 
 int launch_flow_warp_nhwc(const void* x, const float* flow, void* out, int n, int h, int w, int c, int dtype,
                           int pad_mode, cudaStream_t stream);

@@ -448,14 +448,9 @@ int launch_t2t_unfold(const float* img, float* tok, void* tok_hi_v, void* tok_lo
   const int smem2 = U2_CC * 7 * (w + 6) * 4;
   if (fast && c % U2_CC == 0 && smem2 <= 200 * 1024 && fh <= 65535 && bt <= 65535) {
     static DeviceOnce cfg;
-    const int dev = current_device();
-    if (!device_done(cfg, dev)) {
-      cudaFuncSetAttribute(t2t_unfold733_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-      cudaFuncSetAttribute(t2t_unfold733_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-      cudaFuncSetAttribute(t2t_unfold733_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-      cudaFuncSetAttribute(t2t_unfold733_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-      device_mark(cfg, dev);
-    }
+    if (const int e = configure_once(cfg, 200 * 1024, t2t_unfold733_kernel<true, false>, t2t_unfold733_kernel<false, false>,
+                                     t2t_unfold733_kernel<true, true>, t2t_unfold733_kernel<false, true>))
+      return e;
     const dim3 grid(c / U2_CC, fh, bt);
     if (gelu && nhwc)
       t2t_unfold733_kernel<true, true><<<grid, threads, smem2, stream>>>(img, tok, tok_hi, tok_lo, c, h, w, fh, fw);
@@ -683,18 +678,14 @@ static int fold733_band(int w, int fh, int extra_rows, size_t* smem, int CC = 4,
   return tr;
 }
 
-static void fold733_configure() {
-  static DeviceOnce cfg;
-  const int dev = current_device();
-  if (device_done(cfg, dev)) return;
-  cudaFuncSetAttribute(t2t_fold733_kernel<true, true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  cudaFuncSetAttribute(t2t_fold733_kernel<true, false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  cudaFuncSetAttribute(t2t_fold733_kernel<false, false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  cudaFuncSetAttribute(t2t_fold733_kernel<false, false, 8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+static int fold733_configure() {
+  static DeviceOnce folds, fullwidth;
+  if (const int e = configure_once(folds, 200 * 1024, t2t_fold733_kernel<false, false, 4>,
+                                   t2t_fold733_kernel<false, false, 8, true>))
+    return e;
   // three ~63 KB bands per SM need the large shared-memory carve-out (ncu: the default left room for two)
-  cudaFuncSetAttribute(t2t_fold733_kernel<true, true, 4>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  cudaFuncSetAttribute(t2t_fold733_kernel<true, false, 4>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  device_mark(cfg, dev);
+  return configure_once_carveout(fullwidth, 200 * 1024, cudaSharedmemCarveoutMaxShared, t2t_fold733_kernel<true, true, 4>,
+                                 t2t_fold733_kernel<true, false, 4>);
 }
 
 // Fused fold/normalise/unfold(/GELU).  Returns -2 (unsupported) when the geometry is not 7/3/3 or no band fits in
@@ -710,7 +701,7 @@ static int launch_fold733_fullwidth(const float* tin, float* tok, void* tok_hi, 
   auto* hi = static_cast<__nv_bfloat16*>(tok_hi);
   auto* lo = static_cast<__nv_bfloat16*>(tok_lo);
   const dim3 grid(c / CC, (fh + tr - 1) / tr, bt);
-  fold733_configure();
+  if (const int e = fold733_configure()) return e;
   if (gelu)
     t2t_fold733_kernel<true, true, CC><<<grid, 256, smem, stream>>>(tin, tok, hi, lo, nullptr, nullptr, 1, c, h, w, fh, fw, tr,
                                                                     out_pitch);
@@ -739,12 +730,7 @@ int launch_t2t_fold_unfold(const float* tin, float* tok, void* tok_hi, void* tok
   const size_t smem = smem_of(tr);
   if (smem > 200 * 1024 || bands > 65535) return -2;
   static DeviceOnce cfg;
-  const int dev = current_device();
-  if (!device_done(cfg, dev)) {
-    cudaFuncSetAttribute(t2t_ffn_mid_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    cudaFuncSetAttribute(t2t_ffn_mid_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    device_mark(cfg, dev);
-  }
+  if (const int e = configure_once(cfg, 200 * 1024, t2t_ffn_mid_kernel<true>, t2t_ffn_mid_kernel<false>)) return e;
   auto* hi = static_cast<__nv_bfloat16*>(tok_hi);
   auto* lo = static_cast<__nv_bfloat16*>(tok_lo);
   const dim3 grid((c / MID_CC) * xt, bands, bt);
@@ -765,7 +751,7 @@ int launch_t2t_fold_nhwc(const float* tok, const float* bias, const float* resid
   size_t smem = 0;
   const int tr = fold733_band(w, (h + 2) / 3, 0, &smem, 8);
   if (tr < 1) return -2;
-  fold733_configure();
+  if (const int e = fold733_configure()) return e;
   const dim3 grid(c / 8, (h + 3 * tr - 1) / (3 * tr), bt);
   t2t_fold733_kernel<false, false, 8, true><<<grid, 256, smem, stream>>>(tok, nullptr, nullptr, nullptr, img, bias, normalize, c,
                                                                          h, w, fh, fw, tr, c * 49, residual);
@@ -785,7 +771,7 @@ int launch_t2t_fold(const float* tok, const float* bias, float* img, int bt, int
     size_t smem = 0;
     const int tr = fold733_band(w, (h + 2) / 3, 0, &smem);
     if (tr >= 1) {
-      fold733_configure();
+      if (const int e = fold733_configure()) return e;
       const dim3 grid(c / 4, (h + 3 * tr - 1) / (3 * tr), bt);
       t2t_fold733_kernel<false, false, 4><<<grid, 256, smem, stream>>>(tok, nullptr, nullptr, nullptr, img, bias, normalize, c, h,
                                                                        w, fh, fw, tr, c * 49);

@@ -1,4 +1,5 @@
 """CPU: the C-ABI library builds, loads and exports every symbol include/e2fgvi_b200.h declares."""
+import ctypes
 import os
 import re
 
@@ -51,6 +52,20 @@ def test_argument_errors_new_entry_points(lib):
     assert lib.e2f_prop_prologue(16, None, 16, 0, 16, 0, *[16] * 9, 1, 4, 4, 32, None) == -1   # feat_n2 without flow_prev
     assert b"both" in lib.e2f_last_error()
     assert lib.e2f_prop_prologue(8, 16, 16, 0, 16, 0, *[16] * 9, 1, 4, 4, 32, None) == -3      # misaligned prop
+
+
+def test_conv_launcher_rejections_without_gpu(lib):
+    """The conv launchers' own shape checks come before the driver is asked to encode a tensor map."""
+    src = (ctypes.c_void_p * 1)(16)
+    channels = (ctypes.c_int * 1)(64)
+    # kx-in-N conv: only 3x3 and 7x7 kernels
+    assert lib.e2f_conv_kxn_bf16x3(1, src, src, channels, 16, 16, None, None, 16, None, None,
+                                   1, 8, 32, 32, 1, 32, 5, 1.0, 0, None) == -2
+    assert b"conv_kxn: unsupported shape" in lib.e2f_last_error()
+    # generic conv: the bias is staged in shared memory for at most 512 output channels
+    assert lib.e2f_conv2d_rows_bf16x3(1, src, src, channels, 0, 16, 16, None, None, None, 16, 16, 0,
+                                      1, 8, 16, 520, 1, 1.0, 3, 1, 1, None) == -2
+    assert b"at most 512 output channels" in lib.e2f_last_error()
 
 
 def test_no_cpu_fallback():
