@@ -37,22 +37,44 @@ def flow_warp(x, flow):
     return F.grid_sample(x, torch.stack((gfx, gfy), dim=3), mode="bilinear", padding_mode="border", align_corners=True)
 
 
+def quarter(frames):
+    """The 1/4 bilinear downsample of e2fgvi.py:214-218: (n, c, h, w) -> (n, c, h // 4, w // 4)."""
+    return F.interpolate(frames, scale_factor=1 / 4, mode="bilinear", align_corners=True, recompute_scale_factor=True)
+
+
+def pyramid(x, mean, std):
+    """flow_comp.py:101-115,152-158: resize (n, 3, h, w) to multiples of 32, normalise, five 2x2 average pools.
+    Returns the six levels, finest first."""
+    h, w = x.shape[2:4]
+    w_up = w if w % 32 == 0 else 32 * (w // 32 + 1)
+    h_up = h if h % 32 == 0 else 32 * (h // 32 + 1)
+    levels = [(F.interpolate(x, size=(h_up, w_up), mode="bilinear", align_corners=False) - mean) / std]
+    for _ in range(5):
+        levels.append(F.avg_pool2d(levels[-1], 2, 2, count_include_pad=False))
+    return levels
+
+
+def upsample_flow(flow):
+    """flow_comp.py:121-126: the coarser level's flow (n, 2, h, w) at twice the size, times 2."""
+    return F.interpolate(flow, scale_factor=2, mode="bilinear", align_corners=True) * 2.0
+
+
+def resize_flow(flow, h, w):
+    """flow_comp.py:160-167: the level-0 flow (n, 2, h_up, w_up) resized to (h, w), u scaled by w / w_up, v by
+    h / h_up."""
+    h_up, w_up = flow.shape[2:4]
+    flow = F.interpolate(flow, size=(h, w), mode="bilinear", align_corners=False)
+    return torch.stack((flow[:, 0] * (float(w) / float(w_up)), flow[:, 1] * (float(h) / float(h_up))), dim=1)
+
+
 def spynet(params, mean, std, ref, supp, slopes=None, record=None):
     """SPyNet.forward (flow_comp.py:136-169).  params[level][k] = (weight, bias); slopes[level][k] (k < 4): 0/1 mask
     of the ReLU after conv k or None; ``record`` (a list) receives the (pre-activation > 0) masks."""
     h, w = ref.shape[2:4]
-    w_up = w if w % 32 == 0 else 32 * (w // 32 + 1)
-    h_up = h if h % 32 == 0 else 32 * (h // 32 + 1)
-    ref = F.interpolate(ref, size=(h_up, w_up), mode="bilinear", align_corners=False)
-    supp = F.interpolate(supp, size=(h_up, w_up), mode="bilinear", align_corners=False)
-    refs, supps = [(ref - mean) / std], [(supp - mean) / std]
-    for _ in range(5):
-        refs.append(F.avg_pool2d(refs[-1], 2, 2, count_include_pad=False))
-        supps.append(F.avg_pool2d(supps[-1], 2, 2, count_include_pad=False))
-    refs, supps = refs[::-1], supps[::-1]
-    flow = ref.new_zeros(ref.size(0), 2, h_up // 32, w_up // 32)
+    refs, supps = pyramid(ref, mean, std)[::-1], pyramid(supp, mean, std)[::-1]
+    flow = ref.new_zeros(ref.size(0), 2, refs[0].shape[2], refs[0].shape[3])
     for level in range(6):
-        up = flow if level == 0 else F.interpolate(flow, scale_factor=2, mode="bilinear", align_corners=True) * 2.0
+        up = flow if level == 0 else upsample_flow(flow)
         y = torch.cat([refs[level], flow_warp(supps[level], up.permute(0, 2, 3, 1)), up], 1)
         rec = []
         for k in range(5):
@@ -65,16 +87,14 @@ def spynet(params, mean, std, ref, supp, slopes=None, record=None):
         if record is not None:
             record.append(rec)
         flow = up + y
-    flow = F.interpolate(flow, size=(h, w), mode="bilinear", align_corners=False)
-    return torch.stack((flow[:, 0] * (float(w) / float(w_up)), flow[:, 1] * (float(h) / float(h_up))), dim=1)
+    return resize_flow(flow, h, w)
 
 
 def forward_bidirect_flow(params, mean, std, frames, slopes=None, record=None):
     """e2fgvi.py:210-234 on frames (b, l_t, 3, h, w) in [0, 1].  Both directions run as one batch (forward pairs, then
     backward pairs), which is the order of ``slopes`` / ``record``."""
     b, l_t, c, h, w = frames.shape
-    small = F.interpolate(frames.reshape(-1, c, h, w), scale_factor=1 / 4, mode="bilinear", align_corners=True,
-                          recompute_scale_factor=True).view(b, l_t, c, h // 4, w // 4)
+    small = quarter(frames.reshape(-1, c, h, w)).view(b, l_t, c, h // 4, w // 4)
     a = small[:, :-1].reshape(-1, c, h // 4, w // 4)
     z = small[:, 1:].reshape(-1, c, h // 4, w // 4)
     n = a.size(0)
