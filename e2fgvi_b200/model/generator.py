@@ -57,18 +57,11 @@ class BaseNetwork(nn.Module):
                 nn.init.normal_(m.weight.data, 0.0, gain)
                 if getattr(m, "bias", None) is not None:
                     nn.init.constant_(m.bias.data, 0.0)
-        self._invalidate_derived()          # `.data` updates do not bump Parameter versions
-
-    def _invalidate_derived(self):
-        """Forget every kernel operand derived from the parameters (see ``ops.invalidate_weight_caches``)."""
-        ops.invalidate_weight_caches()
-        for m in self.modules():
-            if isinstance(m, SecondOrderDeformableAlignment):
-                m._packed = None
+        ops.invalidate_weight_caches()      # `.data` updates do not bump Parameter versions
 
     def load_state_dict(self, *args, **kwargs):
         out = super().load_state_dict(*args, **kwargs)
-        self._invalidate_derived()
+        ops.invalidate_weight_caches()
         if self._graphs is not None:
             self._graphs = {}                               # captured graphs hold the old derived operands
         return out

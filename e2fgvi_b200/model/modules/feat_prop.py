@@ -44,30 +44,25 @@ class SecondOrderDeformableAlignment(nn.Module):
             nn.Conv2d(co, co, 3, 1, 1), nn.LeakyReLU(0.1, inplace=True),
             nn.Conv2d(co, 27 * deform_groups, 3, 1, 1))
         self.fused = True  # False: torch epilogue + ops.modulated_deform_conv2d (the reference's operator split)
-        self._packed = None  # (weight version, data_ptr, fp16 GEMM operand)
         self.init_offset()
 
     def packed_weight(self):
         """fp16 [Cout, 9*Cin] operand of the DCN GEMM, re-packed whenever the parameter changes or moves."""
-        w = self.weight
-        tag = (w._version, w.data_ptr(), w.device)
-        if self._packed is None or self._packed[0] != tag:
-            self._packed = (tag, ops.pack_dcn_weight(w, self.deform_groups))
-        return self._packed[1]
+        # ops.pack_dcn_weight is looked up when the operand is built, so a replacement of it takes effect
+        return ops._derived_one(self.weight, ("dcn", self.deform_groups), lambda w, g: ops.pack_dcn_weight(w, g),
+                                self.deform_groups)
 
     def init_offset(self):
         """Zero the last offset conv (feat_prop.py:32-33)."""
         nn.init.zeros_(self.conv_offset[-1].weight)
         nn.init.zeros_(self.conv_offset[-1].bias)
 
-    def offset_head(self, cond_sources, flow_1, flow_2, flows=None):
+    def offset_head(self, cond_sources, flow_1, flow_2):
         """conv_offset on cat[cond..., flow_1, flow_2] (feat_prop.py:36-37) without building the cat: each tensor is
         one TMA source of the first conv; LeakyReLU(0.1) is fused into the conv epilogues.  Returns the raw
-        27*dg-channel head, fp32, channels_last.  ``flows``: cat(flow_1, flow_2) already in conv-operand form (from
-        ``ops.prop_prologue``)."""
+        27*dg-channel head, fp32, channels_last."""
         co = self.conv_offset
-        if flows is None:
-            flows = torch.cat([flow_1, flow_2], dim=1)
+        flows = torch.cat([flow_1, flow_2], dim=1)
         y = ops.conv3x3(list(cond_sources) + [flows], co[0].weight, co[0].bias, negative_slope=0.1, out="split")
         y = ops.conv3x3([y], co[2].weight, co[2].bias, negative_slope=0.1, out="split")
         y = ops.conv3x3([y], co[4].weight, co[4].bias, negative_slope=0.1, out="split")
@@ -88,8 +83,8 @@ class SecondOrderDeformableAlignment(nn.Module):
         return ops.deform_align_fused(x, head, flow_1, flow_2, self.packed_weight(), self.bias, self.deform_groups,
                                       self.max_residue_magnitude, out_split=True)
 
-    def align(self, x, cond_sources, flow_1, flow_2, flows=None):
-        head = self.offset_head(cond_sources, flow_1, flow_2, flows)
+    def align(self, x, cond_sources, flow_1, flow_2):
+        head = self.offset_head(cond_sources, flow_1, flow_2)
         if self.fused:
             return ops.deform_align_fused(x, head, flow_1, flow_2, self.packed_weight(), self.bias, self.deform_groups,
                                           self.max_residue_magnitude)
@@ -193,7 +188,6 @@ class BidirectionalPropagation(nn.Module):
         frames = [x[:, i].contiguous(memory_format=torch.channels_last) for i in range(t)]
         # every frame is a source of two convs per direction: split it into the bf16 operand pair once
         frame_ops = [ops.split_nhwc(f) for f in frames]
-        fused = self.fused_prologue and c % 16 == 0
         swept = {}
         for name in self.DIRECTIONS:
             backward = name == "backward_"
@@ -204,12 +198,7 @@ class BidirectionalPropagation(nn.Module):
             hist = []
             for i, idx in enumerate(order):
                 cur = frame_ops[idx]
-                if i > 0 and fused:
-                    # one launch: both warps, the second-order flow, the operand splits and the DCN input (rank 3)
-                    xg, cond_n1, cond_n2, flows_op, flow_n1, flow_n2 = ops.prop_prologue(
-                        prop, hist[-2] if i > 1 else None, flows[:, i - 1], flows[:, i - 2] if i > 1 else None)
-                    prop = align.align(xg, [cond_n1, cur, cond_n2], flow_n1, flow_n2, flows=flows_op)
-                elif i > 0:
+                if i > 0:
                     flow_n1 = flows[:, i - 1]
                     grid_n1 = flow_n1.permute(0, 2, 3, 1)
                     cond_n1 = flow_warp(prop, grid_n1)

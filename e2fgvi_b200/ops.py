@@ -102,8 +102,7 @@ def flow_warp(x, flow, interpolation="bilinear", padding_mode="zeros", align_cor
 def pack_dcn_weight(weight, deform_groups):
     """fp32 [Cout,Cin,3,3] -> fp16 [Cout, 9*Cin] GEMM operand in sampler K-order (k = (g*9+tap)*cpg + c).
 
-    Not cached here (a data_ptr-keyed cache is unsound once the allocator reuses addresses); modules that own a
-    long-lived weight cache the result themselves (see SecondOrderDeformableAlignment.packed_weight)."""
+    Not cached here; ``SecondOrderDeformableAlignment.packed_weight`` caches it per parameter (``_derived_one``)."""
     _need_cuda(weight)
     cout, cin, kh, kw = weight.shape
     if (kh, kw) != (3, 3):
@@ -117,6 +116,36 @@ def pack_dcn_weight(weight, deform_groups):
 
 def _pair(v):
     return tuple(v) if isinstance(v, (tuple, list)) else (v, v)
+
+
+def _square(kernel_size, stride, padding):
+    """(k, s, p) of a square kernel / stride / padding given as ints or pairs."""
+    (k, k2), (s, s2), (p, p2) = _pair(kernel_size), _pair(stride), _pair(padding)
+    if k != k2 or s != s2 or p != p2:
+        raise NotImplementedError("square kernel / stride / padding only (E2FGVI uses 7 / 3 / 3)")
+    return k, s, p
+
+
+def _outputs(out, modes, shape, device, into=None):
+    """Check ``out`` against the ``modes`` a wrapper accepts, then return its (fp32, bf16 hi, bf16 lo) output buffers
+    of ``shape``: fp32 for "f32" / "both", the split pair for "split" / "both", None for what is not asked for (a
+    "rows" pair comes from ``_rows_pair``).  ``into`` = (o32, hi, lo): existing buffers to return instead of new ones."""
+    if out not in modes:
+        raise ValueError(f"out must be one of {', '.join(map(repr, modes))}, got {out!r}")
+    f32, split = out in ("f32", "both"), out in ("split", "both")
+    if into is not None:
+        o32, hi, lo = into
+        if (f32 and o32 is None) or (split and (hi is None or lo is None)):
+            raise ValueError("`into` lacks a buffer for the requested output")
+        return (o32 if f32 else None), (hi if split else None), (lo if split else None)
+    return (torch.empty(shape, dtype=torch.float32, device=device) if f32 else None,
+            torch.empty(shape, dtype=torch.bfloat16, device=device) if split else None,
+            torch.empty(shape, dtype=torch.bfloat16, device=device) if split else None)
+
+
+def _result(out, t32, sp):
+    """What a wrapper with "f32" / "split" / "both" modes returns: the fp32 tensor, the split operand, or both."""
+    return t32 if out == "f32" else sp if out == "split" else (t32, sp)
 
 
 def modulated_deform_conv2d(x, offset, mask, weight, bias=None, stride=1, padding=0, dilation=1, groups=1,
@@ -320,26 +349,17 @@ def t2t_unfold(img, kernel_size, stride, padding, gelu=False, out="f32"):
     gather kernel, optionally followed by the exact GELU.  img (BT,C,H,W) fp32 -> tokens (BT, L, C*k*k): fp32
     tensor (out="f32") or a ``SplitMat`` (out="split")."""
     _need_cuda(img)
-    (k, k2), (s, s2), (p, p2) = _pair(kernel_size), _pair(stride), _pair(padding)
-    if k != k2 or s != s2 or p != p2:
-        raise NotImplementedError("square kernel / stride / padding only (E2FGVI uses 7 / 3 / 3)")
+    k, s, p = _square(kernel_size, stride, padding)
     bt, c, h, w = img.shape
+    fh, fw = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
+    shape = (bt, fh * fw, c * k * k)
+    tok, hi, lo = _outputs(out, ("f32", "split"), shape, img.device)
     # channels_last storage (conv / linear epilogues write it) is read in place by the staged 7/3/3 kernel
     nhwc = ((k, s, p) == (7, 3, 3) and c % 8 == 0 and img.dtype == torch.float32 and not img.is_contiguous()
             and img.permute(0, 2, 3, 1).is_contiguous() and bt <= 65535
             and 8 * 7 * (w + 6) * 4 <= 200 * 1024)      # the staged kernel's shared-memory row buffer (t2t.cu: U2_CC rows)
     if not nhwc:
         img = img.contiguous().float()
-    fh, fw = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
-    shape = (bt, fh * fw, c * k * k)
-    tok = hi = lo = None
-    if out == "f32":
-        tok = torch.empty(shape, dtype=torch.float32, device=img.device)
-    elif out == "split":
-        hi = torch.empty(shape, dtype=torch.bfloat16, device=img.device)
-        lo = torch.empty(shape, dtype=torch.bfloat16, device=img.device)
-    else:
-        raise ValueError("out must be 'f32' or 'split'")
     numel = shape[0] * shape[1] * shape[2]
     with _timed("t2t_unfold", float(numel * 4 + img.numel() * 4)):
         fn = _lib.load().e2f_t2t_unfold_nhwc if nhwc else _lib.load().e2f_t2t_unfold
@@ -357,9 +377,7 @@ def t2t_fold_unfold(tokens, output_size, kernel_size, stride, padding, gelu=Fals
     shape, fp32 (out="f32") or ``SplitMat`` (out="split").  ``pitch`` (multiple of 4 >= C*k*k) pads every output row
     with zero columns — ``linear`` zero-pads its weight to match — so that GEMM rows start on 128-byte lines."""
     _need_cuda(tokens)
-    (k, k2), (s, s2), (p, p2) = _pair(kernel_size), _pair(stride), _pair(padding)
-    if k != k2 or s != s2 or p != p2:
-        raise NotImplementedError("square kernel / stride / padding only (E2FGVI uses 7 / 3 / 3)")
+    k, s, p = _square(kernel_size, stride, padding)
     h, w = output_size
     tokens = tokens.contiguous().float()
     bt, n_tok, ck = tokens.shape
@@ -374,15 +392,7 @@ def t2t_fold_unfold(tokens, output_size, kernel_size, stride, padding, gelu=Fals
     pitch = ck if pitch is None else int(pitch)
     if pitch < ck or pitch % 4:
         raise ValueError(f"t2t_fold_unfold: pitch {pitch} must be a multiple of 4 >= {ck}")
-    oshape = (bt, n_tok, pitch)
-    tok = hi = lo = None
-    if out == "f32":
-        tok = torch.empty(oshape, dtype=torch.float32, device=tokens.device)
-    elif out == "split":
-        hi = torch.empty(oshape, dtype=torch.bfloat16, device=tokens.device)
-        lo = torch.empty(oshape, dtype=torch.bfloat16, device=tokens.device)
-    else:
-        raise ValueError("out must be 'f32' or 'split'")
+    tok, hi, lo = _outputs(out, ("f32", "split"), (bt, n_tok, pitch), tokens.device)
     with _timed("t2t_fold_unfold", float(tokens.numel() * 8)):
         st = _lib.load().e2f_t2t_fold_unfold(tokens.data_ptr(), None if tok is None else tok.data_ptr(),
                                              None if hi is None else hi.data_ptr(),
@@ -404,15 +414,9 @@ def window_pool(x, weight, bias, window_size, out="split"):
     wh, ww = window_size
     if H % wh or W % ww:
         raise ValueError(f"token grid {H}x{W} must be a multiple of the window {wh}x{ww}")
-    shape = (B, T, H // wh, W // ww, C)
-    dev = x.hi.device
+    o32, ohi, olo = _outputs(out, ("f32", "split"), (B, T, H // wh, W // ww, C), x.hi.device)
     w32 = weight.detach().float().contiguous()
     b32 = None if bias is None else bias.detach().float().contiguous()
-    o32 = torch.empty(shape, dtype=torch.float32, device=dev) if out == "f32" else None
-    ohi = torch.empty(shape, dtype=torch.bfloat16, device=dev) if out == "split" else None
-    olo = torch.empty(shape, dtype=torch.bfloat16, device=dev) if out == "split" else None
-    if out not in ("f32", "split"):
-        raise ValueError("out must be 'f32' or 'split'")
     with _timed("window_pool", float(x.hi.numel() * 4)):
         st = _lib.load().e2f_window_pool(x.hi.data_ptr(), x.lo.data_ptr(), w32.data_ptr(),
                                          None if b32 is None else b32.data_ptr(),
@@ -444,23 +448,17 @@ def layer_norm(x, weight, bias, eps=1e-5, out="f32"):
     ``SplitMat`` (operand of the following ``linear``); "both": (tensor, SplitMat)."""
     _need_cuda(x, weight, bias)
     c = x.shape[-1]
+    o32, hi, lo = _outputs(out, ("f32", "split", "both"), x.shape, x.device)
     xc = x.contiguous().float()
     rows = xc.numel() // c
-    want_f32, want_split = out in ("f32", "both"), out in ("split", "both")
-    if not (want_f32 or want_split):
-        raise ValueError("out must be 'f32', 'split' or 'both'")
-    o32 = torch.empty_like(xc) if want_f32 else None
-    hi = torch.empty(xc.shape, dtype=torch.bfloat16, device=x.device) if want_split else None
-    lo = torch.empty(xc.shape, dtype=torch.bfloat16, device=x.device) if want_split else None
     g32, b32 = weight.detach().float().contiguous(), bias.detach().float().contiguous()
-    with _timed("layernorm_split", float(xc.numel() * 4 * (1 + want_f32 + want_split))):
+    with _timed("layernorm_split", float(xc.numel() * 4 * (1 + (o32 is not None) + (hi is not None)))):
         st = _lib.load().e2f_layernorm_split(xc.data_ptr(), g32.data_ptr(), b32.data_ptr(),
                                              None if o32 is None else o32.data_ptr(),
                                              None if hi is None else hi.data_ptr(),
                                              None if lo is None else lo.data_ptr(), rows, c, float(eps), _stream())
     _lib.check(st, "e2f_layernorm_split")
-    sp = SplitMat(hi, lo) if want_split else None
-    return o32 if out == "f32" else sp if out == "split" else (o32, sp)
+    return _result(out, o32, None if hi is None else SplitMat(hi, lo))
 
 
 def layer_norm_pool(x, weight, bias, eps, pool_weight, pool_bias, window_size):
@@ -498,9 +496,7 @@ def t2t_fold(tokens, output_size, kernel_size, stride, padding, normalize=False,
     tokens (BT, L, C*k*k) fp32 -> img (BT, C, H, W) fp32.  ``channels_last=True`` returns the image in channels_last
     storage (what the decoder's convs read) and lets ``residual`` (BT,C,H,W) be added by the same kernel."""
     _need_cuda(tokens, bias, residual)
-    (k, k2), (s, s2), (p, p2) = _pair(kernel_size), _pair(stride), _pair(padding)
-    if k != k2 or s != s2 or p != p2:
-        raise NotImplementedError("square kernel / stride / padding only (E2FGVI uses 7 / 3 / 3)")
+    k, s, p = _square(kernel_size, stride, padding)
     tokens = tokens.contiguous().float()
     bt, L, ck = tokens.shape
     h, w = output_size
@@ -546,25 +542,48 @@ def split_bf16(x):
     return hi, lo
 
 
-_WEIGHT_SPLITS = {}  # id(Parameter) -> (weakref to it, (version, data_ptr), hi, lo); dropped when the parameter dies
+# The one cache of operands derived from parameters (bf16 splits, packed weights, folded bias maps):
+#   (id(param), tag)         -> (weakref, version, data_ptr, operand)                            (_derived_one)
+#   (tuple of ids, tag)      -> (weakrefs, ((version, data_ptr) per parameter), operand)          (_derived)
+_DERIVED = {}
 
 
-def _split_weight(weight, k_pad=0):
-    """bf16 (hi, lo) split of a (N, K) weight, cached per parameter; k_pad > K appends zero columns (for an A operand
-    whose rows are padded to k_pad)."""
-    key = (id(weight), k_pad)
-    tag = (weight._version, weight.data_ptr())
-    hit = _WEIGHT_SPLITS.get(key)
-    if hit is None or hit[0]() is not weight or hit[1] != tag:
-        w2 = weight.detach().reshape(weight.shape[0], -1)
-        if k_pad > w2.shape[1]:
-            w2 = torch.nn.functional.pad(w2.float(), (0, k_pad - w2.shape[1]))
-        hi, lo = split_bf16(w2)
-        if hit is None or hit[0]() is not weight:
-            weakref.finalize(weight, _WEIGHT_SPLITS.pop, key, None)
-        hit = (weakref.ref(weight), tag, hi, lo)
-        _WEIGHT_SPLITS[key] = hit
-    return hit[2], hit[3]
+def _derived_one(param, tag, build, *args):
+    """The operand ``build(param, *args)`` makes from the parameter ``param``, cached under ``tag``: rebuilt when the
+    parameter changes version or address, dropped when it dies.  ``linear`` and the convs look their weights up on
+    every call and a one-clip step is bound by host launch time, so a hit builds no closure, list or generator."""
+    key = (id(param), tag)
+    hit = _DERIVED.get(key)
+    if hit is not None and hit[1] == param._version and hit[2] == param.data_ptr() and hit[0]() is param:
+        return hit[3]
+    val = build(param, *args)
+    if hit is None or hit[0]() is not param:
+        weakref.finalize(param, _DERIVED.pop, key, None)
+    _DERIVED[key] = (weakref.ref(param), param._version, param.data_ptr(), val)
+    return val
+
+
+def _derived(params, tag, build):
+    """The operand ``build()`` makes from a list of parameters, cached under ``tag``: rebuilt when any of them
+    changes version or address, dropped when the first one dies."""
+    key = (tuple(id(p) for p in params), tag)
+    stamp = tuple((p._version, p.data_ptr()) for p in params)
+    hit = _DERIVED.get(key)
+    if hit is None or hit[1] != stamp or any(r() is not p for r, p in zip(hit[0], params)):
+        val = build()
+        if hit is None or hit[0][0]() is not params[0]:
+            weakref.finalize(params[0], _DERIVED.pop, key, None)
+        hit = _DERIVED[key] = (tuple(weakref.ref(p) for p in params), stamp, val)
+    return hit[2]
+
+
+def _padded_split(weight, k):
+    """bf16 (hi, lo) split of an (N, K) or (N, K, 1, 1) weight as (N, k), k >= K: zero columns appended to match an
+    operand whose rows are padded to k."""
+    w2 = weight.detach().reshape(weight.shape[0], -1)
+    if k > w2.shape[1]:
+        w2 = torch.nn.functional.pad(w2.float(), (0, k - w2.shape[1]))
+    return split_bf16(w2)
 
 
 def linear(x, weight, bias=None, residual=None, out_dtype=torch.float32, tile_hint=0):
@@ -588,7 +607,7 @@ def linear(x, weight, bias=None, residual=None, out_dtype=torch.float32, tile_hi
         x2 = x.reshape(-1, k)
         m = x2.shape[0]
         a_hi, a_lo = split_bf16(x2)
-    w_hi, w_lo = _split_weight(weight, k_pad)
+    w_hi, w_lo = _derived_one(weight, ("split", k_pad), _padded_split, k)
     b32 = None if bias is None else bias.detach().float().contiguous()
     res = None
     if residual is not None:
@@ -651,9 +670,12 @@ def rows_channels(c):
     return None
 
 
-def _rows_numel(n, h, w, lead, cin):
+def _rows_pair(n, h, w, lead, cin, device):
+    """Flat bf16 (hi, lo) buffers of a ``RowsNHWC`` operand: n x h rows of ``lead`` + w pixels x ``cin`` channels."""
     lib = _lib.load()
-    return (n * h * int(lib.e2f_conv_rows_pitch(w, lead, cin)) + int(lib.e2f_conv_rows_tail(lead, cin))) * cin
+    numel = (n * h * int(lib.e2f_conv_rows_pitch(w, lead, cin)) + int(lib.e2f_conv_rows_tail(lead, cin))) * cin
+    return (torch.empty(numel, dtype=torch.bfloat16, device=device),
+            torch.empty(numel, dtype=torch.bfloat16, device=device))
 
 
 def pack_rows(x, lead, cin=None):
@@ -667,10 +689,8 @@ def pack_rows(x, lead, cin=None):
     if cin is None or c > cin:
         raise ValueError(f"pack_rows: {c} channels do not fit a row-gapped layout (<= 32)")
     x = x.contiguous().float()
-    numel = _rows_numel(n, h, w, lead, cin)
-    hi = torch.empty(numel, dtype=torch.bfloat16, device=x.device)
-    lo = torch.empty(numel, dtype=torch.bfloat16, device=x.device)
-    with _timed("pack_rows", float(x.numel() * 4 + numel * 4)):
+    hi, lo = _rows_pair(n, h, w, lead, cin, x.device)
+    with _timed("pack_rows", float(x.numel() * 4 + hi.numel() * 4)):
         st = _lib.load().e2f_pack_rows_bf16(x.data_ptr(), hi.data_ptr(), lo.data_ptr(), n, c, h, w, cin, lead, _stream())
     _lib.check(st, "e2f_pack_rows_bf16")
     return RowsNHWC(hi, lo, (n, c, h, w), lead, cin)
@@ -738,24 +758,21 @@ def merge_conv_groups(weight, src_channels, groups):
     return merged, groups // m
 
 
-_CONV_PACKS = {}  # (id(Parameter), src channels, groups) -> (weakref, tag, hi, lo, effective groups)
+def _conv3x3_operand(weight, src_channels, groups, rows_cin):
+    """(hi, lo, effective groups) of a conv3x3-path weight: the value of its ("conv3x3", src_channels, groups,
+    rows_cin) ``_derived`` entry.  rows_cin > 0: window-packed K for a ``RowsNHWC`` source of that many channels."""
+    if rows_cin:
+        return (*pack_conv_rows_weight(weight, rows_cin), 1)
+    w_eff, g_eff = merge_conv_groups(weight, src_channels, groups)
+    return (*pack_conv3x3_weight(w_eff, src_channels, g_eff), g_eff)
 
 
-def _packed_conv_weight(weight, src_channels, groups, rows_cin=0):
-    key = (id(weight), tuple(src_channels), groups, rows_cin)
-    tag = (weight._version, weight.data_ptr())
-    hit = _CONV_PACKS.get(key)
-    if hit is None or hit[0]() is not weight or hit[1] != tag:
-        if rows_cin:
-            (hi, lo), g_eff = pack_conv_rows_weight(weight, rows_cin), 1
-        else:
-            w_eff, g_eff = merge_conv_groups(weight, src_channels, groups)
-            hi, lo = pack_conv3x3_weight(w_eff, src_channels, g_eff)
-        if hit is None or hit[0]() is not weight:
-            weakref.finalize(weight, _CONV_PACKS.pop, key, None)
-        hit = (weakref.ref(weight), tag, hi, lo, g_eff)
-        _CONV_PACKS[key] = hit
-    return hit[2], hit[3], hit[4]
+def _source_arrays(sources):
+    """ctypes arrays (hi pointers, lo pointers, stored channel counts) of a conv's ``SplitNHWC`` / ``RowsNHWC``
+    operands."""
+    k = len(sources)
+    return ((_lib._vp * k)(*[s.hi.data_ptr() for s in sources]), (_lib._vp * k)(*[s.lo.data_ptr() for s in sources]),
+            (_lib._i * k)(*[s.cin if isinstance(s, RowsNHWC) else s.hi.shape[-1] for s in sources]))
 
 
 def conv3x3(sources, weight, bias=None, groups=1, negative_slope=1.0, residual=None, out="f32", stride=1,
@@ -782,80 +799,48 @@ def conv3x3(sources, weight, bias=None, groups=1, negative_slope=1.0, residual=N
         if rows_in.shape[1] != weight.shape[1]:
             raise ValueError("conv3x3: weight does not match the source's channel count")
         splits = [rows_in]
-        true_channels = padded_channels = [rows_in.cin]
+        true_channels = [rows_in.cin]
     else:
         splits = [split_nhwc(s) for s in (sources if isinstance(sources, (list, tuple)) else [sources])]
         true_channels = [s.shape[1] for s in splits]
-        padded_channels = [s.hi.shape[-1] for s in splits]
-    n, _, h, w = splits[0].shape
+        if groups != 1 and any(s.hi.shape[-1] != c for s, c in zip(splits, true_channels)):
+            raise NotImplementedError("grouped conv3x3 needs channel counts that are multiples of 8")
+    n, _, h_in, w_in = splits[0].shape
     for s in splits:
-        if (s.shape[0], s.shape[2], s.shape[3]) != (n, h, w):
+        if (s.shape[0], s.shape[2], s.shape[3]) != (n, h_in, w_in):
             raise ValueError("conv3x3 sources must share N, H, W")
-    if groups != 1 and true_channels != padded_channels:
-        raise NotImplementedError("grouped conv3x3 needs channel counts that are multiples of 8")
-    h_in, w_in = h, w
+    if out == "rows" and (out_lead <= 0 or cout not in (8, 16, 32)):
+        raise ValueError("conv3x3: out='rows' needs out_lead > 0 and 8, 16 or 32 output channels")
     h, w = (h_in + 2 * pad - ks) // stride + 1, (w_in + 2 * pad - ks) // stride + 1
-    w_hi, w_lo, g_eff = _packed_conv_weight(weight, true_channels, groups, rows_in.cin if rows_in is not None else 0)
+    o32, ohi, olo = _outputs(out, ("f32", "split", "both", "rows"), (n, h, w, cout), weight.device)
+    if out == "rows":
+        ohi, olo = _rows_pair(n, h, w, out_lead, cout, weight.device)
+    rows_cin = 0 if rows_in is None else rows_in.cin
+    w_hi, w_lo, g_eff = _derived_one(weight, ("conv3x3", tuple(true_channels), groups, rows_cin), _conv3x3_operand,
+                                     true_channels, groups, rows_cin)
     b32 = None if bias is None else bias.detach().float().contiguous()
     res = None
     if residual is not None:
         res = residual.permute(0, 2, 3, 1).contiguous().float()
-    want_f32, want_split, want_rows = out in ("f32", "both"), out in ("split", "both"), out == "rows"
-    if not (want_f32 or want_split or want_rows):
-        raise ValueError("out must be 'f32', 'split', 'both' or 'rows'")
-    if want_rows and (out_lead <= 0 or cout not in (8, 16, 32)):
-        raise ValueError("conv3x3: out='rows' needs out_lead > 0 and 8, 16 or 32 output channels")
-    dev = weight.device
-    o32 = torch.empty((n, h, w, cout), dtype=torch.float32, device=dev) if want_f32 else None
-    ohi = olo = None
-    if want_split:
-        ohi = torch.empty((n, h, w, cout), dtype=torch.bfloat16, device=dev)
-        olo = torch.empty((n, h, w, cout), dtype=torch.bfloat16, device=dev)
-    elif want_rows:
-        numel = _rows_numel(n, h, w, out_lead, cout)
-        ohi = torch.empty(numel, dtype=torch.bfloat16, device=dev)
-        olo = torch.empty(numel, dtype=torch.bfloat16, device=dev)
-    k = len(splits)
-    hi_arr = (_lib._vp * k)(*[s.hi.data_ptr() for s in splits])
-    lo_arr = (_lib._vp * k)(*[s.lo.data_ptr() for s in splits])
-    ch_arr = (_lib._i * k)(*padded_channels)
     with _timed("conv3x3_bf16x3", 2.0 * n * h * w * cout * weight.shape[1] * ks * ks):
-        st = _lib.load().e2f_conv2d_rows_bf16x3(k, hi_arr, lo_arr, ch_arr, 1 if rows_in is not None else 0,
+        st = _lib.load().e2f_conv2d_rows_bf16x3(len(splits), *_source_arrays(splits), 1 if rows_in is not None else 0,
                                                 w_hi.data_ptr(), w_lo.data_ptr(),
                                                 None if b32 is None else b32.data_ptr(),
                                                 None if res is None else res.data_ptr(),
                                                 None if o32 is None else o32.data_ptr(),
                                                 None if ohi is None else ohi.data_ptr(),
                                                 None if olo is None else olo.data_ptr(),
-                                                out_lead if want_rows else 0, n, h_in, w_in, cout,
+                                                out_lead if out == "rows" else 0, n, h_in, w_in, cout,
                                                 g_eff, float(negative_slope), ks, stride, pad, _stream())
     _lib.check(st, "e2f_conv2d_rows_bf16x3")
-    if want_rows:
+    if out == "rows":
         return RowsNHWC(ohi, olo, (n, cout, h, w), out_lead, cout)
-    t32 = o32.permute(0, 3, 1, 2) if want_f32 else None
-    sp = SplitNHWC(ohi, olo, (n, cout, h, w)) if want_split else None
-    return t32 if out == "f32" else sp if out == "split" else (t32, sp)
+    return _result(out, None if o32 is None else o32.permute(0, 3, 1, 2),
+                   None if ohi is None else SplitNHWC(ohi, olo, (n, cout, h, w)))
 
 
 # ------------------------------------------------------------------------------------------------- SoftSplit / SoftComp
 KXN_CONVS = os.environ.get("E2F_KXN", "1") != "0"     # small-Cout layers on the kx-in-N kernel (E2F_KXN=0: A/B, debugging)
-
-_DERIVED = {}   # (id(param), tag...) -> (weakref, (version, data_ptr) tuple, value): weight-derived operands, per parameter
-
-
-def _derived(params, tag, build):
-    """Cache of operands derived from one or more nn.Parameters (packed weights, folded bias maps); rebuilt when any
-    of them changes version or address, dropped when the first one dies."""
-    key = (tuple(id(p) for p in params),) + tuple(tag)
-    stamp = tuple((p._version, p.data_ptr()) for p in params)
-    hit = _DERIVED.get(key)
-    if hit is None or any(r() is not p for r, p in zip(hit[0], params)) or hit[1] != stamp:
-        val = build()
-        if hit is None or hit[0][0]() is not params[0]:
-            weakref.finalize(params[0], _DERIVED.pop, key, None)
-        hit = (tuple(weakref.ref(p) for p in params), stamp, val)
-        _DERIVED[key] = hit
-    return hit[2]
 
 
 def _best_tile(gh, gw, stride):
@@ -869,12 +854,6 @@ def _best_tile(gh, gw, stride):
         if best_cost is None or key < best_cost:
             best, best_cost = (tw, th), key
     return best
-
-
-def _as_split_nhwc(x):
-    if isinstance(x, SplitNHWC):
-        return x
-    return split_nhwc(x)
 
 
 def _nhwc_stride(t, what):
@@ -898,23 +877,7 @@ def _conv_gather(sources, w_hi, w_lo, bias, bias_map, residual, out, cout, strid
     gh, gw = grid
     oh, ow = out_size
     tw, th = _best_tile(gh, gw, stride)
-    dev = sources[0].hi.device
-    want_f32, want_split = out in ("f32", "both"), out in ("split", "both")
-    if not (want_f32 or want_split):
-        raise ValueError("out must be 'f32', 'split' or 'both'")
-    o32 = ohi = olo = None
-    if into is not None:
-        o32, ohi, olo = into
-        if (want_f32 and o32 is None) or (want_split and (ohi is None or olo is None)):
-            raise ValueError("conv: `into` lacks a buffer for the requested output")
-        o32 = o32 if want_f32 else None
-        ohi, olo = (ohi, olo) if want_split else (None, None)
-    else:
-        if want_f32:
-            o32 = torch.empty((n, oh, ow, cout), dtype=torch.float32, device=dev)
-        if want_split:
-            ohi = torch.empty((n, oh, ow, cout), dtype=torch.bfloat16, device=dev)
-            olo = torch.empty((n, oh, ow, cout), dtype=torch.bfloat16, device=dev)
+    o32, ohi, olo = _outputs(out, ("f32", "split", "both"), (n, oh, ow, cout), sources[0].hi.device, into)
     outs = [t for t in (o32, ohi, olo) if t is not None]
     for t in outs:
         if tuple(t.shape) != (n, oh, ow, cout):
@@ -939,9 +902,6 @@ def _conv_gather(sources, w_hi, w_lo, bias, bias_map, residual, out, cout, strid
     tap0 = (ctypes.c_uint8 * (nph + 1))(*([p[0] for p in phases] + [nt]))
     oy = (ctypes.c_uint8 * nph)(*[p[1] for p in phases])
     ox = (ctypes.c_uint8 * nph)(*[p[2] for p in phases])
-    hi_arr = (_lib._vp * k)(*[s_.hi.data_ptr() for s_ in sources])
-    lo_arr = (_lib._vp * k)(*[s_.lo.data_ptr() for s_ in sources])
-    ch_arr = (_lib._i * k)(*[s_.hi.shape[-1] for s_ in sources])
     sn = [_nhwc_stride(s_.hi, "conv source") for s_ in sources]
     for s_, v in zip(sources, sn):
         if _nhwc_stride(s_.lo, "conv source") != v:
@@ -950,15 +910,14 @@ def _conv_gather(sources, w_hi, w_lo, bias, bias_map, residual, out, cout, strid
     b32 = None if bias is None else bias.detach().float().contiguous()
     with _timed("conv3x3_bf16x3", flops):
         st = _lib.load().e2f_conv_gather_bf16x3(
-            k, hi_arr, lo_arr, ch_arr, w_hi.data_ptr(), w_lo.data_ptr(), None if b32 is None else b32.data_ptr(),
+            k, *_source_arrays(sources), w_hi.data_ptr(), w_lo.data_ptr(), None if b32 is None else b32.data_ptr(),
             None if bias_map is None else bias_map.data_ptr(), None if res is None else res.data_ptr(),
             None if o32 is None else o32.data_ptr(), None if ohi is None else ohi.data_ptr(),
             None if olo is None else olo.data_ptr(), n, h_in, w_in, cout, float(slope), stride, gh, gw, tw, th, nt, dy, dx,
             nph, tap0, oy, ox, ostep, oh, ow, sn_arr, out_nstride, _stream())
     _lib.check(st, "e2f_conv_gather_bf16x3")
-    t32 = o32.permute(0, 3, 1, 2) if want_f32 else None
-    sp = SplitNHWC(ohi, olo, (n, cout, oh, ow)) if want_split else None
-    return t32 if out == "f32" else sp if out == "split" else (t32, sp)
+    return _result(out, None if o32 is None else o32.permute(0, 3, 1, 2),
+                   None if ohi is None else SplitNHWC(ohi, olo, (n, cout, oh, ow)))
 
 
 def conv_frames(sources, weight, bias=None, negative_slope=1.0, residual=None, out="f32", into=None):
@@ -969,12 +928,12 @@ def conv_frames(sources, weight, bias=None, negative_slope=1.0, residual=None, o
     cout, ks = weight.shape[0], weight.shape[2]
     pad = ks // 2
     _need_cuda(weight, bias, residual)
-    splits = [_as_split_nhwc(s_) for s_ in (sources if isinstance(sources, (list, tuple)) else [sources])]
+    splits = [split_nhwc(s_) for s_ in (sources if isinstance(sources, (list, tuple)) else [sources])]
     chans = [s_.shape[1] for s_ in splits]         # true channel counts (storage may be zero-padded to a multiple of 8)
     if sum(chans) != weight.shape[1]:
         raise ValueError(f"conv_frames: source channels {chans} do not add up to the weight's {weight.shape[1]} input channels")
     n, _, h, w = splits[0].shape
-    w_hi, w_lo, _ = _packed_conv_weight(weight, chans, 1)
+    w_hi, w_lo, _ = _derived_one(weight, ("conv3x3", tuple(chans), 1, 0), _conv3x3_operand, chans, 1, 0)
     taps = [(ky - pad, kx - pad) for ky in range(ks) for kx in range(ks)]
     return _conv_gather(splits, w_hi, w_lo, bias, None, residual, out, cout, 1, (h, w), taps, [(0, 0, 0)], 1, (h, w),
                         2.0 * n * h * w * cout * weight.shape[1] * ks * ks, slope=negative_slope, into=into)
@@ -987,18 +946,16 @@ def soft_split(x, weight, bias, kernel_size, stride, padding):
 
     x (BT,C,H,W) fp32 (any memory format) or ``SplitNHWC``; weight (hidden, C*k*k) = ``ss.embedding.weight``;
     bias (hidden,).  Returns tokens (BT, fh*fw, hidden) fp32 — exactly ``embedding(unfold(x).permute(0, 2, 1))``."""
-    (k, k2), (s, s2), (p, p2) = _pair(kernel_size), _pair(stride), _pair(padding)
-    if k != k2 or s != s2 or p != p2:
-        raise NotImplementedError("square kernel / stride / padding only (E2FGVI uses 7 / 3 / 3)")
-    src = _as_split_nhwc(x)
+    k, s, p = _square(kernel_size, stride, padding)
+    src = split_nhwc(x)
     n, c, h, w = src.shape
     hidden = weight.shape[0]
     if weight.shape[1] != c * k * k or k * k > 64 or c % 8:
         raise ValueError(f"soft_split: weight {tuple(weight.shape)} does not match C={c}, k={k}")
     _need_cuda(weight, bias)
     fh, fw = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
-    w_hi, w_lo = _derived([weight], ("soft_split", c, k),
-                          lambda: pack_conv3x3_weight(weight.detach().view(hidden, c, k, k), [c], 1))
+    w_hi, w_lo = _derived_one(weight, ("soft_split", c, k),
+                              lambda wt: pack_conv3x3_weight(wt.detach().view(hidden, c, k, k), [c], 1))
     taps = [(ky - p, kx - p) for ky in range(k) for kx in range(k)]
     tok = _conv_gather([src], w_hi, w_lo, bias, None, None, "f32", hidden, s, (fh, fw), taps, [(0, 0, 0)], 1,
                        (fh, fw), 2.0 * n * fh * fw * hidden * c * k * k)
@@ -1033,9 +990,7 @@ def soft_comp(tokens, weight, bias, output_size, kernel_size, stride, padding, b
     ``bias_map_extra``: the base model's ``sc.bias`` (C, H, W) parameter or None; ``residual`` (BT, C, H, W) fp32 added
     in the epilogue (enc_feat + trans_feat, e2fgvi.py:263).  Returns (BT, C, H, W) fp32 channels_last (out="f32"),
     a ``SplitNHWC`` (out="split", operand of the HQ model's bias_conv) or both."""
-    (k, k2), (s, s2), (p, p2) = _pair(kernel_size), _pair(stride), _pair(padding)
-    if k != k2 or s != s2 or p != p2:
-        raise NotImplementedError("square kernel / stride / padding only (E2FGVI uses 7 / 3 / 3)")
+    k, s, p = _square(kernel_size, stride, padding)
     h, w = output_size
     fh, fw = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
     hidden = weight.shape[1]
@@ -1055,12 +1010,12 @@ def soft_comp(tokens, weight, bias, output_size, kernel_size, stride, padding, b
     taps, phases, kpos = _soft_comp_tables(k, s, p)
     src = SplitNHWC(hi.view(n, fh, fw, hidden), lo.view(n, fh, fw, hidden), (n, hidden, fh, fw))
 
-    def pack():
+    def pack(weight):
         order = torch.tensor([ky * k + kx for ky, kx in kpos], device=weight.device)
         wp = weight.detach().float().view(c, k * k, hidden)[:, order, :].reshape(c, k * k * hidden)
         return split_bf16(wp)
 
-    w_hi, w_lo = _derived([weight], ("soft_comp", k, s), pack)
+    w_hi, w_lo = _derived_one(weight, ("soft_comp", k, s), pack)
 
     def fold_bias():
         # fold of the Linear bias: every pixel receives b[c, ky, kx] from each token patch that covers it (border
@@ -1119,7 +1074,7 @@ def conv_kxn(x, weight, bias=None, negative_slope=1.0, residual=None, out="f32",
     the encoder's groups-of-32 conv (e2fgvi.py:97; two sources, group-wise concatenation never built).
     x: (N,C,H,W) fp32 / ``SplitNHWC`` or a list of up to two of them; residual (N,Cout,H,W) logical with NHWC storage;
     out = "f32" | "split" | "both"; ``tanh_nchw``: tanh + contiguous NCHW fp32 result (the prediction, e2fgvi.py:262)."""
-    srcs = [_as_split_nhwc(s_) for s_ in (x if isinstance(x, (list, tuple)) else [x])]
+    srcs = [split_nhwc(s_) for s_ in (x if isinstance(x, (list, tuple)) else [x])]
     n, _, h, w = srcs[0].shape
     chans = [s_.shape[1] for s_ in srcs]
     cout, cin_g, ks, ks2 = weight.shape
@@ -1131,30 +1086,19 @@ def conv_kxn(x, weight, bias=None, negative_slope=1.0, residual=None, out="f32",
         if (s_.shape[0], s_.shape[2], s_.shape[3]) != (n, h, w) or not s_.hi.is_contiguous() or not s_.lo.is_contiguous():
             raise ValueError("conv_kxn: sources must be dense and share N, H, W")
     _need_cuda(weight, bias, residual)
-    w_hi, w_lo = _derived([weight], ("kxn", co_pad, tuple(chans), groups),
-                          lambda: pack_conv_kxn_weight(weight, co_pad, chans, groups))
-    b32 = None if bias is None else bias.detach().float().contiguous()
-    dev = weight.device
-    want_f32, want_split = out in ("f32", "both"), out in ("split", "both")
     if tanh_nchw and out != "f32":
         raise ValueError("conv_kxn: tanh_nchw returns the fp32 NCHW tensor only")
-    if want_split and (cout // groups) % 8:
+    if out in ("split", "both") and (cout // groups) % 8:
         raise ValueError("conv_kxn: split output needs Cout / groups % 8 == 0")
+    o32, ohi, olo = _outputs(out, ("f32", "split", "both"), (n, cout, h, w) if tanh_nchw else (n, h, w, cout),
+                             weight.device)
+    w_hi, w_lo = _derived_one(weight, ("kxn", co_pad, tuple(chans), groups), pack_conv_kxn_weight, co_pad, chans, groups)
+    b32 = None if bias is None else bias.detach().float().contiguous()
     res = None
     if residual is not None:
         res = residual.permute(0, 2, 3, 1).contiguous().float()          # no-op for NHWC storage
-    o32 = ohi = olo = None
-    if want_f32:
-        o32 = torch.empty((n, cout, h, w) if tanh_nchw else (n, h, w, cout), dtype=torch.float32, device=dev)
-    if want_split:
-        ohi = torch.empty((n, h, w, cout), dtype=torch.bfloat16, device=dev)
-        olo = torch.empty((n, h, w, cout), dtype=torch.bfloat16, device=dev)
-    k = len(srcs)
-    hi_arr = (_lib._vp * k)(*[s_.hi.data_ptr() for s_ in srcs])
-    lo_arr = (_lib._vp * k)(*[s_.lo.data_ptr() for s_ in srcs])
-    ch_arr = (_lib._i * k)(*[s_.hi.shape[-1] for s_ in srcs])
     with _timed("conv3x3_bf16x3", 2.0 * n * h * w * cout * cin_g * ks * ks):
-        st = _lib.load().e2f_conv_kxn_bf16x3(k, hi_arr, lo_arr, ch_arr, w_hi.data_ptr(), w_lo.data_ptr(),
+        st = _lib.load().e2f_conv_kxn_bf16x3(len(srcs), *_source_arrays(srcs), w_hi.data_ptr(), w_lo.data_ptr(),
                                              None if b32 is None else b32.data_ptr(),
                                              None if res is None else res.data_ptr(),
                                              None if o32 is None else o32.data_ptr(), None if ohi is None else ohi.data_ptr(),
@@ -1163,9 +1107,8 @@ def conv_kxn(x, weight, bias=None, negative_slope=1.0, residual=None, out="f32",
     _lib.check(st, "e2f_conv_kxn_bf16x3")
     if tanh_nchw:
         return o32
-    t32 = o32.permute(0, 3, 1, 2) if want_f32 else None
-    sp = SplitNHWC(ohi, olo, (n, cout, h, w)) if want_split else None
-    return t32 if out == "f32" else sp if out == "split" else (t32, sp)
+    return _result(out, None if o32 is None else o32.permute(0, 3, 1, 2),
+                   None if ohi is None else SplitNHWC(ohi, olo, (n, cout, h, w)))
 
 
 def conv3x3_tanh_nchw(x, weight, bias):
@@ -1174,13 +1117,13 @@ def conv3x3_tanh_nchw(x, weight, bias):
     prediction fused into the conv epilogue.  x: (N,C,H,W) fp32 or ``SplitNHWC``."""
     if KXN_CONVS and weight.shape[0] <= 32 and tuple(weight.shape[2:]) == (3, 3):
         return conv_kxn(x, weight, bias, tanh_nchw=True)
-    src = _as_split_nhwc(x)
+    src = split_nhwc(x)
     n, c, h, w = src.shape
     cout = weight.shape[0]
     _need_cuda(weight, bias)
     if tuple(weight.shape[1:]) != (c, 3, 3) or cout > 32 or cout % 4 == 0:
         raise ValueError(f"conv3x3_tanh_nchw: weight {tuple(weight.shape)} (needs (Cout, {c}, 3, 3), Cout <= 32, Cout % 4 != 0)")
-    w_hi, w_lo, _ = _packed_conv_weight(weight, [c], 1)
+    w_hi, w_lo, _ = _derived_one(weight, ("conv3x3", (c,), 1, 0), _conv3x3_operand, [c], 1, 0)
     b32 = None if bias is None else bias.detach().float().contiguous()
     out = torch.empty((n, cout, h, w), dtype=torch.float32, device=weight.device)
     with _timed("conv3x3_bf16x3", 2.0 * n * h * w * cout * c * 9):
@@ -1239,15 +1182,12 @@ def spynet_level_input(pyr, k, prev_flow, lead=3):
     img = pyr.levels[k]
     _, _, hk, wk = img.shape
     P = 2 * pyr.b * (pyr.l_t - 1)
-    numel = _rows_numel(P, hk, wk, lead, 8)
-    dev = img.device
-    hi = torch.empty(numel, dtype=torch.bfloat16, device=dev)
-    lo = torch.empty(numel, dtype=torch.bfloat16, device=dev)
-    flow_up = torch.empty((P, hk, wk, 2), dtype=torch.float32, device=dev)
     if prev_flow is not None:
         if tuple(prev_flow.shape) != (P, hk // 2, wk // 2, 2) or not prev_flow.is_contiguous() or prev_flow.dtype != torch.float32:
             raise ValueError(f"spynet_level_input: prev_flow {tuple(prev_flow.shape)} != {(P, hk // 2, wk // 2, 2)} fp32 contiguous")
-    st = _lib.load().e2f_spynet_level_input(img.data_ptr(), None if prev_flow is None else prev_flow.data_ptr(),
+    hi, lo = _rows_pair(P, hk, wk, lead, 8, img.device)
+    flow_up = torch.empty((P, hk, wk, 2), dtype=torch.float32, device=img.device)
+    st =_lib.load().e2f_spynet_level_input(img.data_ptr(), None if prev_flow is None else prev_flow.data_ptr(),
                                             hi.data_ptr(), lo.data_ptr(), flow_up.data_ptr(), pyr.b, pyr.l_t, hk, wk, lead,
                                             _stream())
     _lib.check(st, "e2f_spynet_level_input")
@@ -1338,26 +1278,19 @@ def conv2d_dgrad(dy, weight, act=None, out="f32", out_lead=3):
         raise ValueError(f"conv2d_dgrad: dy has {dy.shape[1]} channels, the weight {cout} outputs")
     n, _, h, w = dy.shape
     _need_cuda(weight, dy.hi)
-    w_hi, w_lo = _derived([weight], ("dgrad", dy_c if rows else 0), lambda: pack_conv_dgrad_weight(weight, dy_c if rows else 0))
     act_ptr, act_lead = None, 0
     if act is not None:
         if act.shape != (n, cin, h, w) or (isinstance(act, RowsNHWC) and act.cin != cin) or (
                 isinstance(act, SplitNHWC) and act.hi.shape[-1] != cin):
             raise ValueError(f"conv2d_dgrad: act {act.shape} does not match ({n}, {cin}, {h}, {w})")
         act_ptr, act_lead = act.hi.data_ptr(), (act.lead if isinstance(act, RowsNHWC) else 0)
-    dev = weight.device
-    dx = torch.empty((n, h, w, cin), dtype=torch.float32, device=dev)
-    ohi = olo = None
-    lead = out_lead if out == "rows" else 0
+    dx, ohi, olo = _outputs(out, ("f32", "rows", "split"), (n, h, w, cin), weight.device)
+    if dx is None:                    # every mode returns dx; "rows" / "split" add an operand
+        dx = torch.empty((n, h, w, cin), dtype=torch.float32, device=weight.device)
     if out == "rows":
-        numel = _rows_numel(n, h, w, out_lead, cin)
-        ohi = torch.empty(numel, dtype=torch.bfloat16, device=dev)
-        olo = torch.empty(numel, dtype=torch.bfloat16, device=dev)
-    elif out == "split":
-        ohi = torch.empty((n, h, w, cin), dtype=torch.bfloat16, device=dev)
-        olo = torch.empty((n, h, w, cin), dtype=torch.bfloat16, device=dev)
-    elif out != "f32":
-        raise ValueError("conv2d_dgrad: out must be 'f32', 'rows' or 'split'")
+        ohi, olo = _rows_pair(n, h, w, out_lead, cin, weight.device)
+    lead = out_lead if out == "rows" else 0
+    w_hi, w_lo = _derived_one(weight, ("dgrad", dy_c if rows else 0), pack_conv_dgrad_weight, dy_c if rows else 0)
     with _timed(f"conv2d_dgrad_c{cin}", 2.0 * n * h * w * cout * cin * 49):
         st = _lib.load().e2f_conv2d_dgrad_bf16x3(dy.hi.data_ptr(), dy.lo.data_ptr(), dy_c, 3 if rows else 0,
                                                  w_hi.data_ptr(), w_lo.data_ptr(), act_ptr, act_lead, dx.data_ptr(),
@@ -1415,12 +1348,10 @@ def attention_flops(B, T, H, W, C, window_size, expand_size, focal_window, use_p
 
 
 def invalidate_weight_caches():
-    """Drop every operand derived from model parameters (bf16 splits, packed conv / gather-conv weights, folded bias
-    maps).  The caches key on ``(param._version, data_ptr)``; in-place updates through ``param.data`` (``nn.init`` on
-    ``.data``, EMA ``p.data.copy_()``, manual surgery) do NOT bump the version, so call this after such updates.
+    """Drop every operand derived from model parameters (bf16 splits, packed conv / gather-conv / DCN weights, folded
+    bias maps).  The cache keys on ``(param._version, data_ptr)``; in-place updates through ``param.data`` (``nn.init``
+    on ``.data``, EMA ``p.data.copy_()``, manual surgery) do NOT bump the version, so call this after such updates.
     ``InpaintGenerator.init_weights`` and ``load_state_dict`` do it for you."""
-    _WEIGHT_SPLITS.clear()
-    _CONV_PACKS.clear()
     _DERIVED.clear()
 
 
