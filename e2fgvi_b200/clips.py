@@ -285,9 +285,8 @@ class PeerStitcher(ClipStitcher):
 
 
 def peer_stitch_available(world, device=None):
-    """True when the stitch can use peer memory: CUDA, several ranks, all on this node with peer access to this device.
-    ``E2F_STITCH=nccl`` forces the NCCL all-gather (A/B measurements)."""
-    if os.environ.get("E2F_STITCH", "peer") == "nccl" or world <= 1 or not torch.cuda.is_available():
+    """True when the stitch can use peer memory: CUDA, several ranks, all on this node with peer access to this device."""
+    if world <= 1 or not torch.cuda.is_available():
         return False
     if int(os.environ.get("LOCAL_WORLD_SIZE", str(world))) != world or torch.cuda.device_count() < world:
         return False
@@ -297,7 +296,7 @@ def peer_stitch_available(world, device=None):
 
 def make_stitcher(num_clips, frames_per_clip, rank, world, payload="fp32", device=None):
     """``PeerStitcher`` on one NVLink box, ``ClipStitcher`` (NCCL / gloo all-gather) otherwise.  The choice is made from
-    the same inputs on every rank (world size, visible devices, environment), so all ranks pick the same class."""
+    the same inputs on every rank (world size, ranks on this node, visible devices), so all ranks pick the same class."""
     use_peer = peer_stitch_available(world, device)
     if world > 1 and dist.is_initialized():
         votes = [None] * world

@@ -25,7 +25,6 @@
 // fragments (no CTA-wide staging tile, so the pipeline gets that room).
 #include <cuda.h>
 #include <cuda_bf16.h>
-#include <cstdlib>
 #include <cstring>
 #include "common.cuh"
 #include "launch.h"
@@ -992,15 +991,11 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
     }
   }
   // HALO variant (see conv3x3_halo_kernel): dense 3x3 / s1 / p1 layers with <= 64 output channels whose weights fit
-  // in shared memory next to >= 3 halo slots.  E2F_CONV_HALO=0 forces the generic kernel (A/B timing, debugging).
+  // in shared memory next to >= 3 halo slots.  Every other shape runs on the generic kernel.
   int halo_slots = 0;
   if (!geom && !in_rows && !dact && ks == 3 && stride == 1 && pad == 1 && groups == 1 && cout <= 64) {
-    static const bool enabled = [] {
-      const char* e = getenv("E2F_CONV_HALO");
-      return !(e && e[0] == '0');
-    }();
     const int room = SMEM_LIMIT - 1024 - 256 - MAX_COUT * 4 - halo_w_bytes(bn, p.chunks_total) - EPI_WARPS * EPI_STAGE;
-    if (enabled && room >= 3 * HALO_SLOT) halo_slots = room / HALO_SLOT < HALO_MAX_SLOTS ? room / HALO_SLOT : HALO_MAX_SLOTS;
+    if (room >= 3 * HALO_SLOT) halo_slots = room / HALO_SLOT < HALO_MAX_SLOTS ? room / HALO_SLOT : HALO_MAX_SLOTS;
   }
   if (in_rows) {
     // ONE row-gapped source [N][H][w_in + pad][cin] (+ tail): dimension 1 steps by `stride` pixels, dimension 0 spans

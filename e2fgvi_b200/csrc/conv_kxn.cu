@@ -15,7 +15,6 @@
 // Pipeline = conv.cu: persistent CTAs, TMA warp + two consumer warpgroups (64 accumulator rows each, in registers).
 #include <cuda.h>
 #include <cuda_bf16.h>
-#include <cstdlib>
 #include "common.cuh"
 #include "launch.h"
 
@@ -352,13 +351,6 @@ int launch_conv_kxn(int nsrc, const void* const* src_hi, const void* const* src_
   bool halo = NB <= 112 && ks == 3 && p.chunks >= 2;
   if (halo && p.a_slots * p.a_slot_bytes + p.w_slots * p.w_slot_bytes + extra > 227 * 1024) p.w_slots = 2;
   if (halo && p.a_slots * p.a_slot_bytes + p.w_slots * p.w_slot_bytes + extra > 227 * 1024) halo = false;
-  {
-    static const bool off = [] {
-      const char* e = getenv("E2F_KXN_HALO");
-      return e && e[0] == '0';
-    }();
-    if (off) halo = false;
-  }
   if (!halo && p.stages * p.stage_bytes + extra > 227 * 1024) {
     set_error("conv_kxn: stage does not fit in shared memory");
     return -2;

@@ -21,7 +21,6 @@
 //   warps 8-11 loaders: per-key source addresses (wrap / pooled / padding) then coalesced 16-byte cp.async gathers of
 //              K and V rows (256 B each) into swizzled smem, 2-stage ring of 64-key tiles
 // Roofline (SURVEY §8d): 4*B*nW*heads*(T*wh*ww)*(T*(wh*ww+ring+fh*fw))*128 FLOP on the tensor pipe.
-#include <cstdlib>
 #include <type_traits>
 #include <cuda_bf16.h>
 #include "common.cuh"
@@ -70,10 +69,6 @@ struct Params {
   int nWh, nWw;
   int use_pooled;
   float scale_log2;               // scale * log2(e)
-#ifdef E2F_ATTN_DEVTOOLS          // developer builds only (-DE2F_ATTN_DEVTOOLS): never compiled into the shipped library
-  int debug;                      // perf-experiment bits (E2F_ATTN_DEBUG): 2 skip gathers
-  long long* trace;               // optional [3 roles][64 events] clock64 stamps of CTA (0,0,0) (E2F_ATTN_TRACE)
-#endif
   int n1, n2;                     // expanded-window positions listed once / more than once by the reference
   uint8_t ring_pos[MAX_RING];     // positions (er*EW + ec): the n1 single ones first, then the n2 multiple ones
   uint8_t ring_mult[MAX_RING];    // multiplicity of each entry
@@ -142,19 +137,6 @@ __global__ void __launch_bounds__(THREADS, 1) focal_attn_kernel(const __grid_con
   uint64_t* v_empty = k_empty + KV_STAGES;      // V stage read by PV(kt)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  // The ablation bits and the clock64 trace of round 1 exist only in developer builds: in the shipped library `dbg` is
-  // the compile-time constant 0 and stamp() is empty, so no environment variable can alter the result.
-#ifdef E2F_ATTN_DEVTOOLS
-  const int dbg = prm.debug;
-  const bool tracing = prm.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
-  int tr_n = 0;
-  auto stamp = [&](int role) {     // role 1: loader (warp 8 lane 0)
-    if (tracing && tr_n < 64) prm.trace[role * 64 + tr_n++] = clock64();
-  };
-#else
-  constexpr int dbg = 0;
-  auto stamp = [](int) {};
-#endif
 
   // ---- problem geometry (uniform per CTA)
   const int area = prm.wh * prm.ww;
@@ -414,20 +396,17 @@ __global__ void __launch_bounds__(THREADS, 1) focal_attn_kernel(const __grid_con
           bias = fbias[e];
         }
       }
-      if (lt == 0 && kt < 12) stamp(1);                  // [5kt+0] index math done
       // The K stage is recycled as soon as S(kt-2) has read it (k_empty), the V stage only after PV(kt-2) (v_empty): the
       // gather of K(kt) — the operand the next S waits for — overlaps the softmax and the PV of the tiles in flight
       // instead of starting after them.
       mbar_wait(&k_empty[stage], ((kt / KV_STAGES) & 1) ^ 1);
-      if (lt == 0 && kt < 12) stamp(1);                  // [5kt+1] K stage free
       if (lt < BN) {
         key_ptr[stage * BN + lt] = p;
         key_bias[(kt & (BIAS_SLOTS - 1)) * BN + lt] = bias;
       }
       loader_barrier();
-      if (!(dbg & 2) || kt < KV_STAGES) gather_rows<BN>(smem_u32(smem + Smem::K + stage * KTILE), key_ptr + stage * BN, lwarp, lane, 0);
+      gather_rows<BN>(smem_u32(smem + Smem::K + stage * KTILE), key_ptr + stage * BN, lwarp, lane, 0);
       cp_async_commit();
-      if (lt == 0 && kt < 12) stamp(1);                  // [5kt+2] K gather issued
       if (kt > 0) {                                      // V(kt-1), committed one group earlier, has landed
         cp_async_wait<1>();
         fence_proxy_async_smem();
@@ -438,11 +417,9 @@ __global__ void __launch_bounds__(THREADS, 1) focal_attn_kernel(const __grid_con
       fence_proxy_async_smem();
       __syncwarp();
       if (lane == 0) mbar_arrive(&k_full[stage]);
-      if (lt == 0 && kt < 12) stamp(1);                  // [5kt+3] K landed + arrived
       mbar_wait(&v_empty[stage], ((kt / KV_STAGES) & 1) ^ 1);
-      if (!(dbg & 2) || kt < KV_STAGES) gather_rows<BN>(smem_u32(smem + Smem::V + stage * KTILE), key_ptr + stage * BN, lwarp, lane, prm.C);
+      gather_rows<BN>(smem_u32(smem + Smem::V + stage * KTILE), key_ptr + stage * BN, lwarp, lane, prm.C);
       cp_async_commit();
-      if (lt == 0 && kt < 12) stamp(1);                  // [5kt+4] V gather issued
     }
     cp_async_wait<0>();                                 // V of the last tile
     fence_proxy_async_smem();
@@ -484,14 +461,6 @@ int launch_focal_attention(const void* qkv, const void* qkv_pooled, void* out, i
   prm.nWh = h / wh; prm.nWw = w / ww;
   prm.use_pooled = use_pooled;
   prm.scale_log2 = scale * LOG2E;
-#ifdef E2F_ATTN_DEVTOOLS
-  {
-    const char* dbg = getenv("E2F_ATTN_DEBUG");
-    prm.debug = dbg ? atoi(dbg) : 0;
-    const char* tr = getenv("E2F_ATTN_TRACE");      // hex device address of a [3][64] int64 buffer (perf experiments)
-    prm.trace = tr ? reinterpret_cast<long long*>(strtoull(tr, nullptr, 16)) : nullptr;
-  }
-#endif
   // order the expanded-window positions: single-listed first, multiply-listed last (positions never listed are dropped)
   prm.n1 = prm.n2 = 0;
   for (int pass = 0; pass < 2; ++pass)

@@ -9,7 +9,6 @@ sweep directions (feat_prop.py:94-103) and the caller passes (forward, backward)
 (flows_backward, flows_forward) (e2fgvi.py:249-250).
 """
 import math
-import os
 
 import torch
 import torch.nn as nn
@@ -120,8 +119,9 @@ class BidirectionalPropagation(nn.Module):
                 nn.Conv2d((2 + i) * channel, channel, 3, 1, 1), nn.LeakyReLU(0.1, inplace=True),
                 nn.Conv2d(channel, channel, 3, 1, 1))
         self.fusion = nn.Conv2d(2 * channel, channel, 1, 1, 0)
-        # False (or E2F_PROP_FUSED=0): the operator-by-operator sequence of feat_prop.py:106-126
-        self.fused_prologue = os.environ.get("E2F_PROP_FUSED", "1") != "0"
+        # False: forward() runs the operator-by-operator sequence of feat_prop.py:106-126, as it does for channel counts
+        # that are not a multiple of 16
+        self.fused_prologue = True
 
     def propagate_frames(self, x32, x_hi, x_lo, flows_backward, flows_forward, into=None):
         """The fast path: every per-frame tensor is a FRAME SLICE of a (b,t,h,w,c) buffer, read and written in place.

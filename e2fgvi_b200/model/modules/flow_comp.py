@@ -68,37 +68,24 @@ def _basic_module_rows(module, rows, residual, keep=None):
     list or None) receives the five convs' input operands, the ReLU outputs the backward pass needs."""
     convs = [holder.conv for holder in module.basic_module]
     y = rows
-    last = len(convs) - 1
     if keep is not None:
         keep.append(y)
-    if ops.KXN_CONVS:
-        # 8 -> 32 and 32 -> 64 on the window-packed kernel (wide enough outputs), then 64 -> 32, 32 -> 16 and 16 -> 2 on
-        # the kx-in-N kernel: with <= 32 output channels the plain implicit GEMM re-reads its A tile for every tap
-        y = ops.conv3x3(y, convs[0].weight, convs[0].bias, negative_slope=0.0, out="rows", out_lead=convs[1].padding[0])
-        if keep is not None:
-            keep.append(y)
-        y = ops.conv3x3(y, convs[1].weight, convs[1].bias, negative_slope=0.0, out="split")
-        if keep is not None:
-            keep.append(y)
-        y = ops.conv_kxn(y, convs[2].weight, convs[2].bias, negative_slope=0.0, out="split")
-        if keep is not None:
-            keep.append(y)
-        y = ops.conv_kxn(y, convs[3].weight, convs[3].bias, negative_slope=0.0, out="split")
-        if keep is not None:
-            keep.append(y)
-        out = ops.conv_kxn(y, convs[4].weight, convs[4].bias, residual=residual.permute(0, 3, 1, 2))
-        return out.permute(0, 2, 3, 1)                         # NHWC storage: a view, (P, hk, wk, 2) contiguous
-    for i, conv in enumerate(convs):
-        if i == last:
-            out = ops.conv3x3(y, conv.weight, conv.bias, negative_slope=1.0, out="f32", residual=residual.permute(0, 3, 1, 2))
-            return out.permute(0, 2, 3, 1)                     # NHWC storage: a view, (P, hk, wk, 2) contiguous
-        nxt = convs[i + 1]
-        if ops.rows_channels(nxt.in_channels) == nxt.in_channels:
-            y = ops.conv3x3(y, conv.weight, conv.bias, negative_slope=0.0, out="rows", out_lead=nxt.padding[0])
-        else:
-            y = ops.conv3x3(y, conv.weight, conv.bias, negative_slope=0.0, out="split")
-        if keep is not None:
-            keep.append(y)
+    # 8 -> 32 and 32 -> 64 on the window-packed kernel (wide enough outputs), then 64 -> 32, 32 -> 16 and 16 -> 2 on
+    # the kx-in-N kernel: with <= 32 output channels the plain implicit GEMM re-reads its A tile for every tap
+    y = ops.conv3x3(y, convs[0].weight, convs[0].bias, negative_slope=0.0, out="rows", out_lead=convs[1].padding[0])
+    if keep is not None:
+        keep.append(y)
+    y = ops.conv3x3(y, convs[1].weight, convs[1].bias, negative_slope=0.0, out="split")
+    if keep is not None:
+        keep.append(y)
+    y = ops.conv_kxn(y, convs[2].weight, convs[2].bias, negative_slope=0.0, out="split")
+    if keep is not None:
+        keep.append(y)
+    y = ops.conv_kxn(y, convs[3].weight, convs[3].bias, negative_slope=0.0, out="split")
+    if keep is not None:
+        keep.append(y)
+    out = ops.conv_kxn(y, convs[4].weight, convs[4].bias, residual=residual.permute(0, 3, 1, 2))
+    return out.permute(0, 2, 3, 1)                             # NHWC storage: a view, (P, hk, wk, 2) contiguous
 
 
 # Layout of each input gradient that the next (shallower) input gradient reads as its dy: row-gapped (window-packed K)

@@ -8,7 +8,6 @@
 Same names / argument meaning / error behaviour as the reference operators; every call goes through the C ABI of
 ``libe2fgvi_b200.so`` on the current CUDA stream.  There is no CPU path: CPU tensors raise.
 """
-import os
 import weakref
 
 import torch
@@ -840,9 +839,6 @@ def conv3x3(sources, weight, bias=None, groups=1, negative_slope=1.0, residual=N
 
 
 # ------------------------------------------------------------------------------------------------- SoftSplit / SoftComp
-KXN_CONVS = os.environ.get("E2F_KXN", "1") != "0"     # small-Cout layers on the kx-in-N kernel (E2F_KXN=0: A/B, debugging)
-
-
 def _best_tile(gh, gw, stride):
     """(tile_w, tile_h) with tile_w * tile_h <= 128 that wastes the fewest accumulator rows on a gh x gw GEMM grid
     (12 x 10 tiles the 20x36 and 60x108 token grids exactly; 18 x 7 the 90x162 one)."""
@@ -1114,24 +1110,11 @@ def conv_kxn(x, weight, bias=None, negative_slope=1.0, residual=None, out="f32",
 def conv3x3_tanh_nchw(x, weight, bias):
     """``torch.tanh(F.conv2d(x, weight, bias, 1, 1))`` returned as a CONTIGUOUS (N, Cout, H, W) fp32 tensor: the
     decoder's 64 -> 3 output conv (e2fgvi.py:149-150) with the tanh of :262 and the NHWC -> NCHW layout change of the
-    prediction fused into the conv epilogue.  x: (N,C,H,W) fp32 or ``SplitNHWC``."""
-    if KXN_CONVS and weight.shape[0] <= 32 and tuple(weight.shape[2:]) == (3, 3):
-        return conv_kxn(x, weight, bias, tanh_nchw=True)
-    src = split_nhwc(x)
-    n, c, h, w = src.shape
-    cout = weight.shape[0]
-    _need_cuda(weight, bias)
-    if tuple(weight.shape[1:]) != (c, 3, 3) or cout > 32 or cout % 4 == 0:
-        raise ValueError(f"conv3x3_tanh_nchw: weight {tuple(weight.shape)} (needs (Cout, {c}, 3, 3), Cout <= 32, Cout % 4 != 0)")
-    w_hi, w_lo, _ = _derived_one(weight, ("conv3x3", (c,), 1, 0), _conv3x3_operand, [c], 1, 0)
-    b32 = None if bias is None else bias.detach().float().contiguous()
-    out = torch.empty((n, cout, h, w), dtype=torch.float32, device=weight.device)
-    with _timed("conv3x3_bf16x3", 2.0 * n * h * w * cout * c * 9):
-        st = _lib.load().e2f_conv3x3_tanh_nchw(src.hi.data_ptr(), src.lo.data_ptr(), src.hi.shape[-1], w_hi.data_ptr(),
-                                               w_lo.data_ptr(), None if b32 is None else b32.data_ptr(), out.data_ptr(),
-                                               n, h, w, cout, _stream())
-    _lib.check(st, "e2f_conv3x3_tanh_nchw")
-    return out
+    prediction fused into the conv epilogue, on the kx-in-N kernel.  x: (N,C,H,W) fp32 or ``SplitNHWC``."""
+    c = x.shape[1]
+    if tuple(weight.shape[1:]) != (c, 3, 3) or weight.shape[0] > 32:
+        raise ValueError(f"conv3x3_tanh_nchw: weight {tuple(weight.shape)} (needs (Cout, {c}, 3, 3), Cout <= 32)")
+    return conv_kxn(x, weight, bias, tanh_nchw=True)
 
 
 # ------------------------------------------------------------------------------------------------- SPyNet glue

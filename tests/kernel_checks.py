@@ -89,6 +89,24 @@ def _traced(fn):
                            e.get("args", {}).get("shared memory")) for e in kernels], recorded
 
 
+def conv3x3_tanh_nchw_entry(x, weight, bias):
+    """tanh(conv2d(x, weight, bias, 1, 1)) as contiguous (N, Cout, H, W) fp32 through the C entry e2f_conv3x3_tanh_nchw
+    (the implicit-GEMM conv with the tanh / NCHW epilogue), which the Python wrappers do not call: they run the decoder's
+    output conv on the kx-in-N kernel."""
+    from e2fgvi_b200 import _lib, ops
+    src = ops.split_nhwc(x)
+    n, c, h, w = src.shape
+    cout = weight.shape[0]
+    w_hi, w_lo, _ = ops._conv3x3_operand(weight, [c], 1, 0)
+    b32 = bias.detach().float().contiguous()
+    out = torch.empty((n, cout, h, w), dtype=torch.float32, device=weight.device)
+    st = _lib.load().e2f_conv3x3_tanh_nchw(src.hi.data_ptr(), src.lo.data_ptr(), src.hi.shape[-1], w_hi.data_ptr(),
+                                           w_lo.data_ptr(), b32.data_ptr(), out.data_ptr(), n, h, w, cout,
+                                           torch.cuda.current_stream().cuda_stream)
+    _lib.check(st, "e2f_conv3x3_tanh_nchw")
+    return out
+
+
 def persistent_launch(launches):
     """The one persistent GEMM launch among ``launches`` (split / pack kernels around it are ignored)."""
     hits = [k for k in launches if PERSISTENT.match(k.name)]

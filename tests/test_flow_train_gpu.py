@@ -163,12 +163,9 @@ def _restate_grads(sd, frames, dfwd, dbwd, slopes=None, record=None):
 
 # (b, l_t, H, W, model, whole): the training size; flows that are not a multiple of 32 (30x50 -> 32x64); the HQ model.
 # ``whole``: also run the whole generator (the base model's fold size is fixed to 240x432 frames).
-# ``kxn``: the default conv kernels, or E2F_KXN=0's (the convs 3 and 4 then keep row-gapped operands, not dense ones).
-@pytest.mark.parametrize("kxn", [True, False])
 @pytest.mark.parametrize("b,l_t,H,W,hq,whole", [(1, 3, 240, 432, False, True), (2, 2, 120, 200, False, False),
                                                 (1, 3, 120, 216, True, True)])
-def test_module_gradients_against_float64(cuda, monkeypatch, b, l_t, H, W, hq, whole, kxn):
-    monkeypatch.setattr(ops, "KXN_CONVS", kxn)
+def test_module_gradients_against_float64(cuda, b, l_t, H, W, hq, whole):
     # Flows of about 3 pixels (they still clamp at the border).  The warp's coordinate gradient jumps where a sample
     # crosses an integer coordinate or the border; with flows of tens of pixels a few samples of the finest levels lie
     # within fp32 rounding of such a kink, take the other side than in float64, and that O(1) difference reaches every
@@ -202,8 +199,6 @@ def test_module_gradients_against_float64(cuda, monkeypatch, b, l_t, H, W, hq, w
     matched = [_l2rel(a, t.grad) for a, t in zip(got, [t for row in params_m for pair in row for t in pair])]
     names = [f"{lv}.{k}.{kind}" for lv in range(6) for k in range(5) for kind in ("w", "b")]
     print(f"max L2-relative error: matched {max(matched):.2e}, plain {max(plain):.2e}")
-    if not kxn:
-        assert any(isinstance(o, ops.RowsNHWC) for o in keep[-1][1][3:])      # the E2F_KXN=0 operands were exercised
     # The finest level's gradients reach no warp adjoint: with the ReLU decisions matched they are held to 1e-4.  The
     # coarser levels' gradients pass through the finest levels' warps.  Even at these flows a few of the ~65k sample
     # coordinates of the finest level lie within the fp32 / fp64 flow difference (~3e-5 px) of an integer, where the

@@ -33,7 +33,7 @@ import torch
 import torch.nn.functional as F
 
 from e2fgvi_b200 import ops
-from kernel_checks import (cdiv as _cdiv, check_close, conv_bn, conv_tile, expect_schedule, generic_tiles, halo_tiles, images_for, kxn_tiles, persistent_launch, print_tables, run_traced,
+from kernel_checks import (cdiv as _cdiv, check_close, conv3x3_tanh_nchw_entry, conv_bn, conv_tile, expect_schedule, generic_tiles, halo_tiles, images_for, kxn_tiles, persistent_launch, print_tables, run_traced,
                            same_launch as _same_launch, sms)
 
 pytestmark = pytest.mark.gpu
@@ -239,17 +239,16 @@ def test_conv_halo_multi_tile(cuda, case):
         check_close(got, ref, bound, 5e-5, "f32", "HALO " + case)
 
 
-def test_conv_halo_tanh_nchw_multi_tile(cuda, monkeypatch):
-    """The decoder output conv (64 -> 3, tanh, NCHW store) on the HALO kernel: with the kx-in-N convs switched off,
-    conv3x3_tanh_nchw goes through launch_conv3x3."""
-    monkeypatch.setattr(ops, "KXN_CONVS", False)
+def test_conv_halo_tanh_nchw_multi_tile(cuda):
+    """The decoder output conv (64 -> 3, tanh, NCHW store) on the HALO kernel: the C entry e2f_conv3x3_tanh_nchw goes
+    through launch_conv3x3 (ops.conv3x3_tanh_nchw runs this layer on the kx-in-N kernel)."""
     s = sms()
     h, w = 48, 80
     n = images_for(lambda k: halo_tiles(k, h, w), 3 * s)
     (x,), weight, b, _ = _conv_operands(cuda, 105, n, [64], h, w, 3, 64, 3)
     with torch.no_grad():
         weight.mul_(3.0)                       # pre-activations over tanh's curved range
-    got, launches = run_traced(lambda: ops.conv3x3_tanh_nchw(x, weight, b))
+    got, launches = run_traced(lambda: conv3x3_tanh_nchw_entry(x, weight, b))
     expect_schedule("conv HALO tanh/NCHW", persistent_launch(launches), "conv3x3_halo_kernel<32>",
                     halo_tiles(n, h, w))
     assert got.is_contiguous() and got.shape == (n, 3, h, w)
@@ -422,7 +421,7 @@ def _perm_check(cuda, case, fn, x_list, res, kernel, tiles, seed):
             assert torch.equal(oa[perm], ob), case
 
 
-def test_conv_image_permutation_bitwise(cuda, monkeypatch):
+def test_conv_image_permutation_bitwise(cuda):
     """Generic, HALO, kx-in-N convs at 64 images (8 clips x 8 frames) of the 432 x 240 model: permuting the images
     permutes the result bit for bit."""
     n = 64
@@ -465,10 +464,9 @@ def test_conv_image_permutation_bitwise(cuda, monkeypatch):
         _perm_check(cuda, "perm kxn encoder7 grouped n=64",
                     lambda xs, r: ops.conv_kxn(xs, w7, b7, negative_slope=0.2, out="both", groups=8),
                     [x0, x1], None, "conv_kxn_kernel<true, 3, 32>", kxn_tiles(n, 60, 108, 3, 8), 5)
-        # the same decoder output conv on the HALO kernel
-        monkeypatch.setattr(ops, "KXN_CONVS", False)
+        # the same decoder output conv on the HALO kernel (the C entry e2f_conv3x3_tanh_nchw)
         x = rnd(n, 64, 120, 216)
-        _perm_check(cuda, "perm HALO tanh/NCHW 120x216 n=64", lambda xs, r: ops.conv3x3_tanh_nchw(xs[0], wd, bd),
+        _perm_check(cuda, "perm HALO tanh/NCHW 120x216 n=64", lambda xs, r: conv3x3_tanh_nchw_entry(xs[0], wd, bd),
                     [x], None, "conv3x3_halo_kernel<32>", halo_tiles(n, 120, 216), 6)
 
 

@@ -1,5 +1,4 @@
-"""Micro-benchmark of the focal attention kernel alone (B clips, T=8, 20x36 tokens, 4 heads x 128).
-E2F_ATTN_DEBUG bits (perf experiments only): 1 skip softmax math, 2 skip gathers, 4 skip MMAs."""
+"""Micro-benchmark of the focal attention kernel alone (B clips, T=8, 20x36 tokens, 4 heads x 128)."""
 import os
 import sys
 
@@ -26,4 +25,4 @@ for _ in range(n):
 e1.record()
 torch.cuda.synchronize()
 ms = e0.elapsed_time(e1) / n
-print(f"ATTN debug={os.environ.get('E2F_ATTN_DEBUG', '0')} B={B}: {ms * 1e3:.1f} us/launch  {flops / ms / 1e9:.1f} TFLOP/s")
+print(f"ATTN B={B}: {ms * 1e3:.1f} us/launch  {flops / ms / 1e9:.1f} TFLOP/s")
