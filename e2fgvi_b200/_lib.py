@@ -87,6 +87,13 @@ SIGNATURES = {
     "e2f_conv2d_dgrad_bf16x3": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _i, _fp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "e2f_conv2d_wgrad_work_elems": (_c.c_int64, [_i, _i, _i, _i, _i]),
     "e2f_conv2d_wgrad_bf16x3": (_i, [_fp, _vp, _vp, _i, _fp, _fp, _fp, _i, _i, _i, _i, _i, _vp]),
+    "e2f_conv_dgrad_bf16x3": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "e2f_conv3x3_wgrad_work_elems": (_c.c_int64, [_i, _i, _i, _i, _i, _i, _i]),
+    "e2f_conv3x3_wgrad_bf16x3": (_i, [_fp, _i, _c.POINTER(_vp), _c.POINTER(_vp), _c.POINTER(_i), _i, _fp, _fp, _fp, _i, _i,
+                                      _i, _i, _i, _i, _vp]),
+    "e2f_upsample2x_backward": (_i, [_fp, _fp, _fp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "e2f_tanh_backward_rows": (_i, [_fp, _fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "e2f_leaky_relu_backward": (_i, [_fp, _fp, _fp, _vp, _vp, _c.c_int64, _f, _vp]),
     "e2f_launch_count": (_c.c_int64, []),
 }
 

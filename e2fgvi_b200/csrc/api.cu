@@ -775,4 +775,84 @@ int e2f_conv2d_wgrad_bf16x3(const float* dy, const void* x_hi, const void* x_lo,
   return finish(launch_conv2d_wgrad(dy, x_hi, x_lo, x_lead, dw, db, work, n, h, w, cin, cout, static_cast<cudaStream_t>(stream)), who);
 }
 
+static bool groups_ok(int g) { return g == 1 || g == 2 || g == 4 || g == 8; }
+
+int e2f_conv_dgrad_bf16x3(const void* dy_hi, const void* dy_lo, int dy_c, int dy_lead, const void* wt_hi, const void* wt_lo,
+                          const void* act, const float* residual, float* dx, void* dx_hi, void* dx_lo, int n, int h_in,
+                          int w_in, int cin, int groups, int ks, int stride, void* stream) {
+  const char* who = "e2f_conv_dgrad_bf16x3";
+  if (!dy_hi || !dy_lo || !wt_hi || !wt_lo) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if ((!dx && !dx_hi) || (!dx_hi) != (!dx_lo)) { set_error("%s: need dx and/or both of dx_hi/dx_lo", who); return E2F_ERR_BAD_ARG; }
+  if (n < 0 || h_in <= 0 || w_in <= 0) { set_error("%s: bad shape n=%d h_in=%d w_in=%d", who, n, h_in, w_in); return E2F_ERR_BAD_ARG; }
+  if (!((ks == 3 || ks == 7) && stride == 1) && !(ks == 3 && stride == 2)) { set_error("%s: ks=%d stride=%d (3 or 7 at stride 1, 3 at stride 2)", who, ks, stride); return E2F_ERR_UNSUPPORTED; }
+  if (!groups_ok(groups) || (stride == 2 && groups != 1)) { set_error("%s: groups=%d (1, 2, 4 or 8; 1 at stride 2)", who, groups); return E2F_ERR_UNSUPPORTED; }
+  if (cin < 8 || cin > 512 || cin % (8 * groups)) { set_error("%s: cin=%d (<= 512, a multiple of 8 per group)", who, cin); return E2F_ERR_UNSUPPORTED; }
+  if (dy_lead != 0 && (dy_lead != ks / 2 || stride != 1 || groups != 1)) { set_error("%s: dy_lead=%d (0: dense; %d: row-gapped, stride 1, groups 1)", who, dy_lead, ks / 2); return E2F_ERR_BAD_ARG; }
+  if (dy_lead ? !rows_c(dy_c) || dy_c < 8 : (dy_c < 8 || dy_c % (8 * groups))) { set_error("%s: dy_c=%d (row-gapped: 8, 16 or 32; dense: a multiple of 8 per group)", who, dy_c); return E2F_ERR_UNSUPPORTED; }
+  if (!aligned(dy_hi, 16) || !aligned(dy_lo, 16) || !aligned(wt_hi, 16) || !aligned(wt_lo, 16) || (dx && !aligned(dx, 16)) ||
+      (dx_hi && (!aligned(dx_hi, 16) || !aligned(dx_lo, 16))) || (act && !aligned(act, 16)) || (residual && !aligned(residual, 16))) { set_error("%s: alignment (16 bytes)", who); return E2F_ERR_ALIGNMENT; }
+  if (n == 0) return 0;
+  return finish(launch_conv_dgrad(dy_hi, dy_lo, dy_c, dy_lead, wt_hi, wt_lo, act, residual, dx, dx_hi, dx_lo, n, h_in, w_in,
+                                  cin, groups, ks, stride, static_cast<cudaStream_t>(stream)), who);
+}
+
+static bool conv3x3_wgrad_ok(const char* who, int n, int h_in, int w_in, int cin, int cout, int groups, int stride) {
+  if (n < 0 || h_in <= 0 || w_in <= 0 || (stride != 1 && stride != 2) || !groups_ok(groups)) { set_error("%s: bad shape n=%d %dx%d stride=%d groups=%d", who, n, h_in, w_in, stride, groups); return false; }
+  if (cin % (8 * groups) || cin / groups > 512 || cout < 8 || cout > 512 || cout % (8 * groups)) { set_error("%s: cin=%d cout=%d (multiples of 8 per group, <= 512 per group)", who, cin, cout); return false; }
+  return true;
+}
+
+int64_t e2f_conv3x3_wgrad_work_elems(int n, int h_in, int w_in, int cin, int cout, int groups, int stride) {
+  if (!conv3x3_wgrad_ok("e2f_conv3x3_wgrad_work_elems", n, h_in, w_in, cin, cout, groups, stride)) return E2F_ERR_BAD_ARG;
+  return static_cast<int64_t>(conv3x3_wgrad_work_elems(n, h_in, w_in, cin / groups, cout, groups, stride));
+}
+
+int e2f_conv3x3_wgrad_bf16x3(const float* dy, int nsrc, const void* const* x_hi, const void* const* x_lo, const int* x_c,
+                             int x_lead, float* dw, float* db, float* work, int n, int h_in, int w_in, int cout, int groups,
+                             int stride, void* stream) {
+  const char* who = "e2f_conv3x3_wgrad_bf16x3";
+  if (!dy || !x_hi || !x_lo || !x_c || !dw) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if (nsrc < 1 || nsrc > 2) { set_error("%s: nsrc=%d (1 or 2)", who, nsrc); return E2F_ERR_BAD_ARG; }
+  int cin = 0;
+  for (int i = 0; i < nsrc; ++i) {
+    if (!x_hi[i] || !x_lo[i]) { set_error("%s: null source %d", who, i); return E2F_ERR_BAD_ARG; }
+    if (x_c[i] < 8 || x_c[i] % (8 * groups)) { set_error("%s: source %d has %d channels (a multiple of 8 per group)", who, i, x_c[i]); return E2F_ERR_BAD_ARG; }
+    if (!aligned(x_hi[i], 16) || !aligned(x_lo[i], 16)) { set_error("%s: alignment (sources 16 bytes)", who); return E2F_ERR_ALIGNMENT; }
+    cin += x_c[i];
+  }
+  if (!conv3x3_wgrad_ok(who, n, h_in, w_in, cin, cout, groups, stride)) return E2F_ERR_BAD_ARG;
+  if (x_lead != 0 && (x_lead != 1 || nsrc != 1 || groups != 1 || !rows_c(x_c[0]))) { set_error("%s: x_lead=%d (0: dense; 1: one row-gapped source of 8, 16 or 32 channels, groups 1)", who, x_lead); return E2F_ERR_BAD_ARG; }
+  if (!work) { set_error("%s: null workspace (e2f_conv3x3_wgrad_work_elems floats needed)", who); return E2F_ERR_BAD_ARG; }
+  if (!aligned(dy, 16) || !aligned(dw, 4) || (db && !aligned(db, 4)) || !aligned(work, 4)) { set_error("%s: alignment (dy 16 bytes)", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_conv3x3_wgrad(dy, nsrc, x_hi, x_lo, x_c, x_lead, dw, db, work, n, h_in, w_in, cout, groups, stride,
+                                     static_cast<cudaStream_t>(stream)), who);
+}
+
+int e2f_upsample2x_backward(const float* dy, const float* act, float* dx, void* dx_hi, void* dx_lo, int n, int h, int w, int c,
+                            void* stream) {
+  const char* who = "e2f_upsample2x_backward";
+  if (!dy || (!dx && !dx_hi) || (!dx_hi) != (!dx_lo)) { set_error("%s: need dy, and dx and/or both of dx_hi/dx_lo", who); return E2F_ERR_BAD_ARG; }
+  if (n < 0 || h <= 0 || w <= 0 || c < 8 || c % 8) { set_error("%s: bad shape n=%d %dx%d c=%d (c a multiple of 8)", who, n, h, w, c); return E2F_ERR_BAD_ARG; }
+  if (!aligned(dy, 32) || (act && !aligned(act, 32)) || (dx && !aligned(dx, 32)) || (dx_hi && (!aligned(dx_hi, 16) || !aligned(dx_lo, 16)))) { set_error("%s: alignment (fp32 32 bytes, bf16 16 bytes)", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_upsample2x_backward(dy, act, dx, dx_hi, dx_lo, n, h, w, c, 0.2f, static_cast<cudaStream_t>(stream)), who);
+}
+
+int e2f_tanh_backward_rows(const float* dout, const float* out, float* dy, void* dy_hi, void* dy_lo, int n, int c, int h, int w,
+                           int lead, void* stream) {
+  const char* who = "e2f_tanh_backward_rows";
+  if (!dout || !out || !dy || !dy_hi || !dy_lo) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if (n < 0 || h <= 0 || w <= 0 || c < 1 || c > 8 || lead < 1 || lead > 8) { set_error("%s: bad shape n=%d c=%d %dx%d lead=%d (c 1..8, lead 1..8)", who, n, c, h, w, lead); return E2F_ERR_BAD_ARG; }
+  if (!aligned(dout, 4) || !aligned(out, 4) || !aligned(dy, 16) || !aligned(dy_hi, 16) || !aligned(dy_lo, 16)) { set_error("%s: alignment (dy, dy_hi, dy_lo 16 bytes)", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_tanh_backward_rows(dout, out, dy, dy_hi, dy_lo, n, c, h, w, lead, static_cast<cudaStream_t>(stream)), who);
+}
+
+int e2f_leaky_relu_backward(const float* dy, const float* act, float* dx, void* dx_hi, void* dx_lo, int64_t count, float slope,
+                            void* stream) {
+  const char* who = "e2f_leaky_relu_backward";
+  if (!dy || !act || (!dx && !dx_hi) || (!dx_hi) != (!dx_lo)) { set_error("%s: need dy, act, and dx and/or both of dx_hi/dx_lo", who); return E2F_ERR_BAD_ARG; }
+  if (count < 0 || count % 8) { set_error("%s: count=%lld (a multiple of 8)", who, static_cast<long long>(count)); return E2F_ERR_BAD_ARG; }
+  if (!aligned(dy, 16) || !aligned(act, 16) || (dx && !aligned(dx, 16)) || (dx_hi && (!aligned(dx_hi, 16) || !aligned(dx_lo, 16)))) { set_error("%s: alignment (16 bytes)", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_leaky_backward(dy, act, dx, dx_hi, dx_lo, count, slope, static_cast<cudaStream_t>(stream)), who);
+}
+
 }  // extern "C"

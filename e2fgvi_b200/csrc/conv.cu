@@ -103,7 +103,9 @@ struct Params {
   // T3 and the DACT instantiations only: derivative of the LeakyReLU(dact_slope) that produced `dact` (bf16, the hi part
   // of the saved activation, Cout channels per pixel; pixel (n, y, x) at n * dact_nstride + y * dact_pitch + dact_lead
   // + x: dense or row-gapped).  The result is multiplied by 1 where dact > 0, else by dact_slope (LeakyReLU keeps the
-  // sign of its input, so its output decides).  Null: no multiply.
+  // sign of its input, so its output decides).  Null: no multiply.  With a residual the epilogue computes
+  // (acc + residual) * derivative: the input gradient of a tensor that several convs read (the encoder's x0) adds the
+  // other convs' contributions before the derivative of the activation that produced it.
   const __nv_bfloat16* dact;
   float dact_slope;
   int dact_pitch, dact_lead;
@@ -214,6 +216,14 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
           f[g4 * 4 + i] = a > 0.f ? a : a * p.slope;
         }
       }
+      if (p.residual && pix_ok) {
+        const float4* r4 = reinterpret_cast<const float4*>(p.residual + pix() * p.Cout + co);
+#pragma unroll
+        for (int g4 = 0; g4 < 4; ++g4) {
+          const float4 ra = __ldg(r4 + g4);
+          f[g4 * 4] += ra.x; f[g4 * 4 + 1] += ra.y; f[g4 * 4 + 2] += ra.z; f[g4 * 4 + 3] += ra.w;
+        }
+      }
       if constexpr (T3 || DACT) {
         if (p.dact && pix_ok) {
           const uint4* d4 = reinterpret_cast<const uint4*>(p.dact + dpix() * p.Cout + co);
@@ -225,14 +235,6 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
             for (int i = 0; i < 8; ++i)
               if (!(__bfloat162float(m[i]) > 0.f)) f[h8 * 8 + i] *= p.dact_slope;
           }
-        }
-      }
-      if (p.residual && pix_ok) {
-        const float4* r4 = reinterpret_cast<const float4*>(p.residual + pix() * p.Cout + co);
-#pragma unroll
-        for (int g4 = 0; g4 < 4; ++g4) {
-          const float4 ra = __ldg(r4 + g4);
-          f[g4 * 4] += ra.x; f[g4 * 4 + 1] += ra.y; f[g4 * 4 + 2] += ra.z; f[g4 * 4 + 3] += ra.w;
         }
       }
       if (p.bias_map && pix_ok) {
@@ -320,6 +322,12 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
             const float a = __uint_as_float(v[g8 * 8 + i]) + bb[i];
             f[i] = a > 0.f ? a : a * p.slope;
           }
+          if (p.residual) {
+            const float4* r4 = reinterpret_cast<const float4*>(p.residual + pix() * p.Cout + cb);
+            const float4 ra = __ldg(r4), rb = __ldg(r4 + 1);
+            f[0] += ra.x; f[1] += ra.y; f[2] += ra.z; f[3] += ra.w;
+            f[4] += rb.x; f[5] += rb.y; f[6] += rb.z; f[7] += rb.w;
+          }
           if constexpr (T3 || DACT) {
             if (p.dact) {
               const uint4 u = __ldg(reinterpret_cast<const uint4*>(p.dact + dpix() * p.Cout + cb));
@@ -328,12 +336,6 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
               for (int i = 0; i < 8; ++i)
                 if (!(__bfloat162float(m[i]) > 0.f)) f[i] *= p.dact_slope;
             }
-          }
-          if (p.residual) {
-            const float4* r4 = reinterpret_cast<const float4*>(p.residual + pix() * p.Cout + cb);
-            const float4 ra = __ldg(r4), rb = __ldg(r4 + 1);
-            f[0] += ra.x; f[1] += ra.y; f[2] += ra.z; f[3] += ra.w;
-            f[4] += rb.x; f[5] += rb.y; f[6] += rb.z; f[7] += rb.w;
           }
           if (p.bias_map) {
             const float4* r4 = reinterpret_cast<const float4*>(p.bias_map + mpix() * p.Cout + cb);
@@ -365,10 +367,10 @@ __device__ __forceinline__ void epilogue_tile(const Params& p, const TileCoord& 
             if (cb + i < co_end) {
               float a = __uint_as_float(v[g8 * 8 + i]) + bias_s[cb + i];
               a = a > 0.f ? a : a * p.slope;
+              if (p.residual) a += __ldg(p.residual + pix() * p.Cout + cb + i);
               if constexpr (T3 || DACT) {
                 if (p.dact && !(__bfloat162float(p.dact[dpix() * p.Cout + cb + i]) > 0.f)) a *= p.dact_slope;
               }
-              if (p.residual) a += __ldg(p.residual + pix() * p.Cout + cb + i);
               if (p.bias_map) a += __ldg(p.bias_map + mpix() * p.Cout + cb + i);
               if (p.epi_flags & EPI_TANH) a = tanhf(a);
               if (p.out) {
@@ -851,7 +853,7 @@ static int launch_bn(const Maps& maps, const Params& p, int grid, cudaStream_t s
 }
 
 // The launchers' common tail: count p's tiles over n images as the kernel does, size the persistent grid and launch the
-// instantiation for bn (the DACT kernel exists for BN 32 and 64: Cout <= 64).
+// instantiation for bn.
 template <bool T3, bool DACT = false>
 static int launch_tiles(const Maps& maps, const Params& p, long long n, int bn, const char* who, cudaStream_t stream) {
   const long long tiles = n * ((p.H + p.tile_h - 1) / p.tile_h) * ((p.W + p.tile_w - 1) / p.tile_w) * p.nphase * p.groups *
@@ -862,15 +864,11 @@ static int launch_tiles(const Maps& maps, const Params& p, long long n, int bn, 
     return -2;
   }
   const int grid = tiles < num_sms() ? static_cast<int>(tiles) : num_sms();
-  if constexpr (DACT) {
-    return bn == 32 ? launch_bn<32, T3, true>(maps, p, grid, stream) : launch_bn<64, T3, true>(maps, p, grid, stream);
-  } else {
-    switch (bn) {
-      case 32: return launch_bn<32, T3, false>(maps, p, grid, stream);
-      case 64: return launch_bn<64, T3, false>(maps, p, grid, stream);
-      case 96: return launch_bn<96, T3, false>(maps, p, grid, stream);
-      default: return launch_bn<128, T3, false>(maps, p, grid, stream);
-    }
+  switch (bn) {
+    case 32: return launch_bn<32, T3, DACT>(maps, p, grid, stream);
+    case 64: return launch_bn<64, T3, DACT>(maps, p, grid, stream);
+    case 96: return launch_bn<96, T3, DACT>(maps, p, grid, stream);
+    default: return launch_bn<128, T3, DACT>(maps, p, grid, stream);
   }
 }
 
@@ -900,14 +898,14 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
                    const void* w_hi, const void* w_lo, const float* bias, const float* residual, float* out,
                    void* out_hi, void* out_lo, int n, int h_in, int w_in, int cout, int groups, float slope, int ks,
                    int stride, int pad, int in_rows, int out_lead, cudaStream_t stream, const ConvGeom* geom, int epi_flags,
-                   const void* dact, int dact_lead) {
+                   const void* dact, int dact_lead, float dact_slope) {
   using namespace conv;
   if (epi_flags && ((cout & 3) == 0 || out_hi || residual || geom)) {
     set_error("conv: tanh / NCHW epilogues are implemented for the element-wise store path (Cout %% 4 != 0, fp32 output only)");
     return -2;
   }
-  if (dact && (geom || groups != 1 || cout > 64 || cout % 8)) {
-    set_error("conv: the ReLU-derivative epilogue needs a plain conv, groups 1 and Cout <= 64, Cout %% 8 == 0");
+  if (dact && (cout % 8 || (geom && geom->out_nstride > 0))) {
+    set_error("conv: the ReLU-derivative epilogue needs Cout %% 8 == 0 and a dense output");
     return -2;
   }
   // GEMM grid = output size of the plain conv, or what the generalised geometry says
@@ -943,7 +941,7 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
   p.out_hi = static_cast<__nv_bfloat16*>(out_hi); p.out_lo = static_cast<__nv_bfloat16*>(out_lo);
   p.out_lead = out_lead;
   p.tile_w = tile_w; p.tile_h = tile_h;
-  p.dact = static_cast<const __nv_bfloat16*>(dact); p.dact_lead = dact_lead;
+  p.dact = static_cast<const __nv_bfloat16*>(dact); p.dact_lead = dact_lead; p.dact_slope = dact_slope;
   if (geom) {
     p.nphase = geom->nphase; p.ostep = geom->ostep; p.out_H = geom->out_h; p.out_W = geom->out_w;
     p.bias_map = geom->bias_map;
@@ -1198,6 +1196,53 @@ int launch_dis_conv(const void* src_hi, const void* src_lo, int cin, const void*
     return e;
   if (const int e = encode_weights(maps, w_hi, w_lo, ntaps * p.chunks_total * BK, cout, bn, "dis_conv weight")) return e;
   return launch_tiles<true>(maps, p, n_img, bn, "dis_conv", stream);
+}
+
+// Input gradient of a k x k conv (2-D, see include/e2fgvi_b200.h e2f_conv_dgrad_bf16x3) on launch_conv3x3's kernel: dY
+// is the source, dX [n][h_in][w_in][cin] the output.
+//  * stride 1, pad k / 2: a plain conv of dY with the rotated, in / out-swapped weight (groups as the forward's);
+//  * k = 3, stride 2, pad 1: four output phases (y % 2, x % 2).  Phase ph = 2 oy + ox lists the taps with ky = oy + 1 and
+//    kx = ox + 1 (mod 2) in increasing (ky, kx) order — 1, 2, 2 and 4 taps — and tap (ky, kx) reads dY at (gy + (oy + 1 -
+//    ky) / 2, gx + (ox + 1 - kx) / 2) for output pixel (2 gy + oy, 2 gx + ox); the weight lists phase 0's taps, then
+//    phase 1's, ... with the forward's (unrotated) values.
+int launch_conv_dgrad(const void* dy_hi, const void* dy_lo, int dy_c, int dy_lead, const void* w_hi, const void* w_lo,
+                      const void* act, const float* residual, float* dx, void* dx_hi, void* dx_lo, int n, int h_in,
+                      int w_in, int cin, int groups, int ks, int stride, cudaStream_t stream) {
+  using namespace conv;
+  const void* srch[1] = {dy_hi};
+  const void* srcl[1] = {dy_lo};
+  const int ch[1] = {dy_c};
+  if (stride == 1)
+    return launch_conv3x3(1, srch, srcl, ch, w_hi, w_lo, nullptr, residual, dx, dx_hi, dx_lo, n, h_in, w_in, cin, groups,
+                          1.f, ks, 1, ks / 2, dy_lead ? 1 : 0, 0, stream, nullptr, 0, act, 0, 0.2f);
+  int8_t dy[9], dxo[9];
+  uint8_t tap0[5], oy[4], ox[4];
+  int nt = 0;
+  for (int ph = 0; ph < 4; ++ph) {
+    oy[ph] = static_cast<uint8_t>(ph >> 1);
+    ox[ph] = static_cast<uint8_t>(ph & 1);
+    tap0[ph] = static_cast<uint8_t>(nt);
+    for (int ky = 0; ky < 3; ++ky)
+      for (int kx = 0; kx < 3; ++kx) {
+        if (((oy[ph] + 1 - ky) & 1) || ((ox[ph] + 1 - kx) & 1)) continue;
+        dy[nt] = static_cast<int8_t>((oy[ph] + 1 - ky) / 2);
+        dxo[nt] = static_cast<int8_t>((ox[ph] + 1 - kx) / 2);
+        ++nt;
+      }
+  }
+  tap0[4] = static_cast<uint8_t>(nt);
+  ConvGeom g;
+  memset(&g, 0, sizeof(g));
+  g.grid_h = (h_in + 1) / 2;
+  g.grid_w = (w_in + 1) / 2;
+  g.out_h = h_in;
+  g.out_w = w_in;
+  pick_tile(g.grid_h, g.grid_w, true, g.tile_w, g.tile_h);
+  g.ntaps = nt; g.nphase = 4; g.ostep = 2;
+  g.tap_dy = dy; g.tap_dx = dxo; g.ph_tap0 = tap0; g.ph_oy = oy; g.ph_ox = ox;
+  const int h_o = (h_in - 1) / 2 + 1, w_o = (w_in - 1) / 2 + 1;
+  return launch_conv3x3(1, srch, srcl, ch, w_hi, w_lo, nullptr, residual, dx, dx_hi, dx_lo, n, h_o, w_o, cin, groups, 1.f,
+                        3, 1, 0, 0, 0, stream, &g, 0, act, 0, 0.2f);
 }
 
 }  // namespace e2f

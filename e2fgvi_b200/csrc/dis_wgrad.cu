@@ -2,10 +2,13 @@
 // (1, pad, pad)), see launch_dis_conv for the forward:
 //     dW[co][ci][kt][ky][kx] = sum over (b, t, y, x) of dY[b][t][y][x][co] * X[b][t + kt - 1][2y + ky - pad][2x + kx - pad][ci]
 //     db[co]                 = sum over (b, t, y, x) of dY[b][t][y][x][co]
-// and of SPyNet's 2-D 7x7 / stride 1 / pad 3 convs (KT = 1, KS = 7, S = 1), whose X is dense or row-gapped (each image
-// row `x_lead` zero pixels in front, `x_pitch` pixels apart: the operand the forward conv read).
-// dW is a GEMM with M = cout, N = TAPS * cin (column j = tap * cin + ci, taps in (kt, ky, kx) order) and K = the output
-// pixels, on wgmma with the bf16 three-term split and fp32 accumulation (the accuracy class of the forward convs).
+// of SPyNet's 2-D 7x7 / stride 1 / pad 3 convs (KT = 1, KS = 7, S = 1), whose X is dense or row-gapped (each image
+// row `x_lead` zero pixels in front, `x_pitch` pixels apart: the operand the forward conv read), and of the encoder's and
+// decoder's 3x3 / pad 1 convs (KT = 1, KS = 3, S = 1 or 2), grouped, with one or two sources read group-wise
+// concatenated (the torch.cat in front of encoder convs 5-8).
+// dW of group g is a GEMM with M = the group's cog outputs, N = TAPS * cig (column j = tap * cig + ci, taps in (kt, ky,
+// kx) order, ci over the group's slice of source 0, then of source 1) and K = the output pixels, on wgmma with the bf16
+// three-term split and fp32 accumulation (the accuracy class of the forward convs).
 //  * One warpgroup per CTA computes a 64 (co) x 128 (j) tile over one K slice, 64 pixels per K block.  Both operands
 //    are pixel-major in memory and the B operand is a gather (each column group reads its own tap's shifted, strided,
 //    zero-padded pixels), so the warpgroup stages them itself into the K-major 128-byte-swizzled layout the wgmma
@@ -41,31 +44,44 @@ __device__ __forceinline__ void st_pair(uint32_t base, int row, int k, uint32_t 
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(base + sw128_offset(row, k >> 3) + (k & 7) * 2), "r"(v) : "memory");
 }
 
+// The X operand: up to two sources, each [..][pixel][cs] bf16 (hi, lo); group g reads channels [g cig, (g + 1) cig) of
+// each, source 0's first.  One source: cig[1] = 0.
+struct Src {
+  const __nv_bfloat16* h[2];
+  const __nv_bfloat16* l[2];
+  int cs[2], cig[2];
+};
+
 // Tap (kt, ky, kx) of output pixel (t, y, x) reads X at (t + kt - KT / 2, S y + ky - pad, S x + kx - pad).
+// blockIdx.y = group * M tiles per group + M tile.
 template <int KT, int KS, int S>
-__global__ void __launch_bounds__(THREADS) wgrad_mma_kernel(const float* __restrict__ dy, const __nv_bfloat16* __restrict__ xh,
-                                                            const __nv_bfloat16* __restrict__ xl, float* __restrict__ ws,
+__global__ void __launch_bounds__(THREADS) wgrad_mma_kernel(const float* __restrict__ dy, const Src xs, float* __restrict__ ws,
                                                             int b, int t, int h_in, int w_in, int x_pitch, int x_lead,
-                                                            int cin, int h_o, int w_o, int cout, int pad, int slices) {
+                                                            int h_o, int w_o, int cout, int groups, int pad, int slices) {
   constexpr int TAPS = KT * KS * KS;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int m0 = blockIdx.y * MT, n0 = blockIdx.x * NT;
+  const int cog = cout / groups, mtiles = (cog + MT - 1) / MT;
+  const int grp = blockIdx.y / mtiles;
+  const int m0 = (blockIdx.y - grp * mtiles) * MT, n0 = blockIdx.x * NT;
+  const int cin = xs.cig[0] + xs.cig[1];
   const int N = TAPS * cin;
   const long long pixels = static_cast<long long>(b) * t * h_o * w_o;
   const long long len = slice_len(pixels, slices);
   const long long k0 = len * blockIdx.z;
   const long long k1 = k0 + len < pixels ? k0 + len : pixels;
   // B staging tasks of this thread: (pixel pair kp, column group jg of 8 channels of one tap), q = tid + 128 r
-  int bdt[4], bdy[4], bdx[4], bci[4];
+  int bdt[4], bdy[4], bdx[4], bci[4], bsrc[4];
   bool bok[4];
 #pragma unroll
   for (int r = 0; r < 4; ++r) {
     const int j0 = n0 + 8 * ((tid + THREADS * r) >> 5);
     bok[r] = j0 < N;
     const int tap = bok[r] ? j0 / cin : 0;
-    bci[r] = bok[r] ? j0 - tap * cin : 0;
+    const int ci = bok[r] ? j0 - tap * cin : 0;
+    bsrc[r] = ci < xs.cig[0] ? 0 : 1;                     // cig[0] % 8 == 0: a column group never straddles the sources
+    bci[r] = bsrc[r] ? grp * xs.cig[1] + ci - xs.cig[0] : grp * xs.cig[0] + ci;
     bdt[r] = tap / (KS * KS) - KT / 2;
     bdy[r] = (tap / KS) % KS - pad;
     bdx[r] = tap % KS - pad;
@@ -85,8 +101,8 @@ __global__ void __launch_bounds__(THREADS) wgrad_mma_kernel(const float* __restr
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const long long k = base + 2 * kp + e;
-        if (k < k1 && co < cout) {
-          const float4* src = reinterpret_cast<const float4*>(dy + k * cout + co);
+        if (k < k1 && co < cog) {
+          const float4* src = reinterpret_cast<const float4*>(dy + k * cout + grp * cog + co);
           const float4 p0 = __ldg(src), p1 = __ldg(src + 1);
           v[e][0] = p0.x; v[e][1] = p0.y; v[e][2] = p0.z; v[e][3] = p0.w;
           v[e][4] = p1.x; v[e][5] = p1.y; v[e][6] = p1.z; v[e][7] = p1.w;
@@ -121,9 +137,12 @@ __global__ void __launch_bounds__(THREADS) wgrad_mma_kernel(const float* __restr
           const int fr = static_cast<int>(n % t);
           const int ti = fr + bdt[r], yi = S * y + bdy[r], xi = S * x + bdx[r];
           if (ti >= 0 && ti < t && yi >= 0 && yi < h_in && xi >= 0 && xi < w_in) {
-            const long long off = (((n + bdt[r]) * h_in + yi) * static_cast<long long>(x_pitch) + x_lead + xi) * cin + bci[r];
-            vh[e] = __ldg(reinterpret_cast<const uint4*>(xh + off));
-            vl[e] = __ldg(reinterpret_cast<const uint4*>(xl + off));
+            // selects, not xs.h[bsrc[r]]: a dynamic index would copy the parameter struct to local memory
+            const bool s1 = bsrc[r] != 0;
+            const long long off = (((n + bdt[r]) * h_in + yi) * static_cast<long long>(x_pitch) + x_lead + xi) *
+                                  (s1 ? xs.cs[1] : xs.cs[0]) + bci[r];
+            vh[e] = __ldg(reinterpret_cast<const uint4*>((s1 ? xs.h[1] : xs.h[0]) + off));
+            vl[e] = __ldg(reinterpret_cast<const uint4*>((s1 ? xs.l[1] : xs.l[0]) + off));
           }
         }
       }
@@ -158,7 +177,7 @@ __global__ void __launch_bounds__(THREADS) wgrad_mma_kernel(const float* __restr
   for (int i = 0; i < NT / 2; ++i) {
     const int m = m0 + 16 * warp + (lane >> 2) + ((i >> 1) & 1) * 8;
     const int n = n0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
-    if (m < cout && n < N) dst[static_cast<size_t>(m) * N + n] = it ? acc[i] : 0.f;   // it == 0: an empty slice
+    if (m < cog && n < N) dst[static_cast<size_t>(grp * cog + m) * N + n] = it ? acc[i] : 0.f;   // it == 0: an empty slice
   }
 }
 
@@ -230,9 +249,9 @@ __global__ void __launch_bounds__(256) reduce_kernel(const float* __restrict__ w
 
 // Split-K slice count: enough CTAs to fill the GPU about twice at the tile count, at least 4 K blocks per slice, at
 // most 64 slices.  A function of the shape alone, so results do not depend on the device.
-static int wgrad_slices(long long pixels, int cout, int n_cols) {
+static int wgrad_slices(long long pixels, int cout, int n_cols, int groups = 1) {
   using namespace wgrad;
-  const long long tiles = static_cast<long long>((cout + MT - 1) / MT) * ((n_cols + NT - 1) / NT);
+  const long long tiles = static_cast<long long>(groups) * ((cout / groups + MT - 1) / MT) * ((n_cols + NT - 1) / NT);
   long long s = (264 + tiles - 1) / tiles;
   const long long cap = pixels / (4 * KB);
   if (s > cap) s = cap;
@@ -258,20 +277,20 @@ long long conv2d_wgrad_work_elems(int n, int h, int w, int cin, int cout) {
 
 // The GEMM over `slices` K ranges, the bias partials and the ordered reduction (3 or 2 launches).
 template <int KT, int KS, int S>
-static int run_wgrad(const float* dy, const void* x_hi, const void* x_lo, float* dw, float* db, float* work, int b, int t,
-                     int h_in, int w_in, int x_pitch, int x_lead, int cin, int h_o, int w_o, int cout, int pad, int slices,
+static int run_wgrad(const float* dy, const wgrad::Src& x, float* dw, float* db, float* work, int b, int t, int h_in,
+                     int w_in, int x_pitch, int x_lead, int h_o, int w_o, int cout, int groups, int pad, int slices,
                      bool bias_rows, cudaStream_t stream) {
   using namespace wgrad;
   constexpr int TAPS = KT * KS * KS;
   static DeviceOnce configured;
   if (const int e = configure_once(configured, SMEM, wgrad_mma_kernel<KT, KS, S>)) return e;
+  const int cin = x.cig[0] + x.cig[1];                 // input channels per group
   const long long n_w = static_cast<long long>(cout) * TAPS * cin;
   float* wsb = work + slices * n_w;
   const long long pixels = static_cast<long long>(b) * t * h_o * w_o;
-  const dim3 grid((TAPS * cin + NT - 1) / NT, (cout + MT - 1) / MT, slices);
-  wgrad_mma_kernel<KT, KS, S><<<grid, THREADS, SMEM, stream>>>(dy, static_cast<const __nv_bfloat16*>(x_hi),
-                                                               static_cast<const __nv_bfloat16*>(x_lo), work, b, t, h_in, w_in,
-                                                               x_pitch, x_lead, cin, h_o, w_o, cout, pad, slices);
+  const dim3 grid((TAPS * cin + NT - 1) / NT, groups * ((cout / groups + MT - 1) / MT), slices);
+  wgrad_mma_kernel<KT, KS, S><<<grid, THREADS, SMEM, stream>>>(dy, x, work, b, t, h_in, w_in, x_pitch, x_lead, h_o, w_o,
+                                                               cout, groups, pad, slices);
   count_launch();
   if (db) {
     if (bias_rows && cout <= 128)
@@ -285,9 +304,15 @@ static int run_wgrad(const float* dy, const void* x_hi, const void* x_lo, float*
   return static_cast<int>(cudaGetLastError());
 }
 
+// one source of cin channels, groups 1
+static wgrad::Src one_src(const void* x_hi, const void* x_lo, int cin) {
+  return wgrad::Src{{static_cast<const __nv_bfloat16*>(x_hi), nullptr}, {static_cast<const __nv_bfloat16*>(x_lo), nullptr},
+                    {cin, 0}, {cin, 0}};
+}
+
 int launch_dis_wgrad(const float* dy, const void* x_hi, const void* x_lo, float* dw, float* db, float* work, int b, int t,
                      int h_in, int w_in, int cin, int h_o, int w_o, int cout, int pad, cudaStream_t stream) {
-  return run_wgrad<3, 5, 2>(dy, x_hi, x_lo, dw, db, work, b, t, h_in, w_in, w_in, 0, cin, h_o, w_o, cout, pad,
+  return run_wgrad<3, 5, 2>(dy, one_src(x_hi, x_lo, cin), dw, db, work, b, t, h_in, w_in, w_in, 0, h_o, w_o, cout, 1, pad,
                             dis_wgrad_slices(b, t, h_o, w_o, cout, cin), false, stream);
 }
 
@@ -295,7 +320,40 @@ int launch_conv2d_wgrad(const float* dy, const void* x_hi, const void* x_lo, int
                         int n, int h, int w, int cin, int cout, cudaStream_t stream) {
   const int pitch = x_lead ? conv_rows_pitch(w, x_lead, cin) : w;
   const int slices = wgrad_slices(static_cast<long long>(n) * h * w, cout, C2D_TAPS * cin);
-  return run_wgrad<1, 7, 1>(dy, x_hi, x_lo, dw, db, work, n, 1, h, w, pitch, x_lead, cin, h, w, cout, 3, slices, true, stream);
+  return run_wgrad<1, 7, 1>(dy, one_src(x_hi, x_lo, cin), dw, db, work, n, 1, h, w, pitch, x_lead, h, w, cout, 1, 3, slices,
+                            true, stream);
+}
+
+// 3x3 / pad 1 convs, stride 1 or 2: the output is ((h_in - 1) / stride + 1) x ((w_in - 1) / stride + 1)
+static int c3_out(int s, int stride) { return (s - 1) / stride + 1; }
+
+int conv3x3_wgrad_slices(int n, int h_in, int w_in, int cig, int cout, int groups, int stride) {
+  return wgrad_slices(static_cast<long long>(n) * c3_out(h_in, stride) * c3_out(w_in, stride), cout, 9 * cig, groups);
+}
+
+long long conv3x3_wgrad_work_elems(int n, int h_in, int w_in, int cig, int cout, int groups, int stride) {
+  const long long s = conv3x3_wgrad_slices(n, h_in, w_in, cig, cout, groups, stride);
+  return s * (static_cast<long long>(cout) * 9 * cig + cout);
+}
+
+int launch_conv3x3_wgrad(const float* dy, int nsrc, const void* const* x_hi, const void* const* x_lo, const int* x_c,
+                         int x_lead, float* dw, float* db, float* work, int n, int h_in, int w_in, int cout, int groups,
+                         int stride, cudaStream_t stream) {
+  wgrad::Src x{};
+  for (int i = 0; i < nsrc; ++i) {
+    x.h[i] = static_cast<const __nv_bfloat16*>(x_hi[i]);
+    x.l[i] = static_cast<const __nv_bfloat16*>(x_lo[i]);
+    x.cs[i] = x_c[i];
+    x.cig[i] = x_c[i] / groups;
+  }
+  const int pitch = x_lead ? conv_rows_pitch(w_in, x_lead, x_c[0]) : w_in;
+  const int h_o = c3_out(h_in, stride), w_o = c3_out(w_in, stride);
+  const int slices = conv3x3_wgrad_slices(n, h_in, w_in, x.cig[0] + x.cig[1], cout, groups, stride);
+  if (stride == 1)
+    return run_wgrad<1, 3, 1>(dy, x, dw, db, work, n, 1, h_in, w_in, pitch, x_lead, h_o, w_o, cout, groups, 1, slices, true,
+                              stream);
+  return run_wgrad<1, 3, 2>(dy, x, dw, db, work, n, 1, h_in, w_in, pitch, x_lead, h_o, w_o, cout, groups, 1, slices, true,
+                            stream);
 }
 
 }  // namespace e2f

@@ -126,8 +126,9 @@ int launch_conv3x3(int nsrc, const void* const* src_hi, const void* const* src_l
                    void* out_hi, void* out_lo, int n, int h_in, int w_in, int cout, int groups, float slope, int ks,
                    int stride, int pad, int in_rows, int out_lead, cudaStream_t stream, const ConvGeom* geom = nullptr,
                    int epi_flags = 0,      // 1: tanh, 2: NCHW fp32 output (3-channel output conv only)
-                   const void* dact = nullptr, int dact_lead = 0);   // ReLU derivative at dact (bf16, Cout channels;
-                                                                     // row-gapped with that lead, or dense when 0)
+                   const void* dact = nullptr, int dact_lead = 0,    // LeakyReLU(dact_slope) derivative at dact (bf16,
+                   float dact_slope = 0.f);                          // Cout channels; row-gapped with that lead, or
+                                                                     // dense when 0); slope 0: ReLU
 int launch_conv_kxn(int nsrc, const void* const* src_hi, const void* const* src_lo, const int* src_c, const void* w_hi,
                     const void* w_lo, const float* bias, const float* residual, float* out, void* out_hi, void* out_lo, int n,
                     int h, int w, int cout, int groups, int co_pad, int ks, float slope, int flags, cudaStream_t stream);
@@ -151,7 +152,23 @@ int launch_dis_wgrad(const float* dy, const void* x_hi, const void* x_lo, float*
 long long conv2d_wgrad_work_elems(int n, int h, int w, int cin, int cout);
 int launch_conv2d_wgrad(const float* dy, const void* x_hi, const void* x_lo, int x_lead, float* dw, float* db, float* work,
                         int n, int h, int w, int cin, int cout, cudaStream_t stream);
-constexpr int I3D_STEM_TAIL = 16;          // zero pixels after the stem operand's last row (the last window's overrun)
+// Encoder / decoder backward (3x3 / pad 1 convs, stride 1 or 2): input gradient on the implicit-GEMM conv (conv.cu,
+// also the k = 7 / stride 1 case), weight gradient on the split-K GEMM (dis_wgrad.cu), element-wise adjoints
+// (encdec_grad.cu).  See include/e2fgvi_b200.h for the operand layouts.
+int launch_conv_dgrad(const void* dy_hi, const void* dy_lo, int dy_c, int dy_lead, const void* w_hi, const void* w_lo,
+                      const void* act, const float* residual, float* dx, void* dx_hi, void* dx_lo, int n, int h_in,
+                      int w_in, int cin, int groups, int ks, int stride, cudaStream_t stream);
+long long conv3x3_wgrad_work_elems(int n, int h_in, int w_in, int cig, int cout, int groups, int stride);
+int launch_conv3x3_wgrad(const float* dy, int nsrc, const void* const* x_hi, const void* const* x_lo, const int* x_c,
+                         int x_lead, float* dw, float* db, float* work, int n, int h_in, int w_in, int cout, int groups,
+                         int stride, cudaStream_t stream);
+int launch_upsample2x_backward(const float* dy, const float* act, float* dx, void* hi, void* lo, int n, int h, int w, int c,
+                               float slope, cudaStream_t stream);
+int launch_tanh_backward_rows(const float* dout, const float* out, float* dy32, void* hi, void* lo, int n, int c, int h, int w,
+                              int lead, cudaStream_t stream);
+int launch_leaky_backward(const float* dy, const float* act, float* dx, void* hi, void* lo, long long count, float slope,
+                          cudaStream_t stream);
+constexpr int I3D_STEM_TAIL = 16;         // zero pixels after the stem operand's last row (the last window's overrun)
 long long i3d_stem_elems(int b, int t, int h, int w);
 int launch_i3d_stem_pack(const void* x, int x_u8, void* hi, void* lo, int b, int t, int h, int w, cudaStream_t stream);
 int launch_i3d_stem_conv(const void* hi, const void* lo, const void* w_hi, const void* w_lo, const float* bias, float* out,

@@ -79,7 +79,25 @@ class Encoder(nn.Module):
         """All nine convs run on the wgmma implicit-GEMM kernel (stride 2 via TMA element strides) with LeakyReLU
         fused and the bf16 split operand handed from epilogue to the next conv; the group-wise concatenation of
         e2fgvi.py:103-108 is expressed as two TMA sources, never materialised.  ``last_out="both"`` also returns the
-        bf16 (hi, lo) split of the features (operand of the propagation convs and of SoftSplit)."""
+        bf16 (hi, lo) split of the features (operand of the propagation convs and of SoftSplit).
+
+        Trainable: with grad mode on, the default ``last_out`` and some encoder parameter requiring grad, the features
+        carry a ``grad_fn`` whose backward gives the parameters that require grad their gradients (``_EncoderGrad``);
+        the features are bit-identical to the untracked call.  Frames that require grad raise ``ValueError`` (no
+        gradient into the frames).  Other ``last_out`` values stay untracked."""
+        if last_out == "f32" and torch.is_grad_enabled():
+            params = [t for conv in self.layers[::2] for t in (conv.weight, conv.bias)]
+            if any(p.requires_grad for p in params):
+                if x.requires_grad:
+                    raise ValueError("Encoder: the gradient with respect to the frames is not implemented (detach them; "
+                                     "the features' gradient reaches the encoder's parameters)")
+                return _EncoderGrad.apply(self, x, *params)
+        return self._forward(x, last_out)
+
+    def _forward(self, x, last_out="f32", keep=None):
+        """The launch sequence of ``forward``; ``keep`` (a list or None) receives each conv's input operands (the stem's
+        row-gapped frames, then [SplitNHWC] or [x0, SplitNHWC] for the two-source convs): the LeakyReLU outputs the
+        backward reads."""
         out = x
         x0 = None
         last = len(_ENC) - 1
@@ -92,6 +110,8 @@ class Encoder(nn.Module):
                 out = ops.pack_rows(out, lead=conv.padding[0])
             if k == 4:
                 x0 = out
+            if keep is not None:
+                keep.append([x0, out] if k > 4 else [out])
             if k > 4 and conv.out_channels // conv.groups <= 32 and mode == "split":
                 # groups of 32 output channels (e2fgvi.py:97): the kx-in-N kernel, one tile per (pixels, group)
                 out = ops.conv_kxn([x0, out], conv.weight, conv.bias, negative_slope=0.2, out=mode, groups=conv.groups)
@@ -101,6 +121,75 @@ class Encoder(nn.Module):
             else:
                 out = ops.conv3x3([out], conv.weight, conv.bias, negative_slope=0.2, out=mode, stride=stride)
         return out
+
+
+def _encoder_backward(enc, frames, keep, feat, grad, need):
+    """Gradients of the encoder's parameters from ``grad`` = d loss / d features (N, 128, h, w).  need[k] = (weight,
+    bias) of conv k need a gradient.  Convs 8 -> 0: LeakyReLU's derivative at each conv's output is fused into the
+    input gradient that produces that output's gradient; x0 (conv 3's output, read by convs 4-8) collects the
+    contributions of convs 8, 7, 6, 5 through the residual epilogue, and conv 4's input gradient adds its own and
+    applies the derivative: (acc4 + (acc5 + (acc6 + (acc7 + acc8)))) * LeakyReLU'(x0).  The walk stops at the lowest
+    conv with a trainable parameter.  Returns [dW0, db0, dW1, ...] (None where not needed)."""
+    grads = [None] * (2 * len(_ENC))
+    active = [k for k in range(len(_ENC)) if any(need[k])]
+    if not active:
+        return grads
+    lowest = active[0]
+    convs = [enc.layers[2 * k] for k in range(len(_ENC))]
+    g = grad.permute(0, 2, 3, 1)                 # NHWC, a view for channels_last gradients
+    dy32, dy = ops.leaky_relu_backward(g, feat.permute(0, 2, 3, 1), 0.2, out="both")
+    dx0 = None
+    x0_c = _ENC[4][0]
+    for k in range(len(_ENC) - 1, lowest - 1, -1):
+        cin, cout, stride, groups = _ENC[k]
+        conv = convs[k]
+        nw, nb = need[k]
+        if nw or nb:
+            srcs = [ops.pack_rows(frames, lead=1, cin=8)] if k == 0 else keep[k]   # 8-channel copy of the frames
+            dw, db = ops.conv3x3_wgrad(dy32, srcs, groups=groups, stride=stride, with_bias=nb,
+                                       cin=cin // groups)
+            grads[2 * k] = dw if nw else None
+            grads[2 * k + 1] = db
+        if k == lowest:
+            break
+        if k > 4:
+            chans = [x0_c, cin - x0_c]
+            if lowest <= 3:
+                dx0 = ops.conv_dgrad(dy, conv.weight, groups=groups, src_channels=chans, source=0, residual=dx0)
+            dy32, dy = ops.conv_dgrad(dy, conv.weight, groups=groups, src_channels=chans, source=1, act=keep[k][1],
+                                      out="both")
+        else:
+            src = keep[k][0]
+            dy32, dy = ops.conv_dgrad(dy, conv.weight, stride=stride, in_size=src.shape[2:], act=src,
+                                      residual=dx0 if k == 4 else None, out="both")
+    return grads
+
+
+class _EncoderGrad(torch.autograd.Function):
+    """``Encoder.forward`` with a backward pass into the encoder's 18 parameters.  The forward is the inference launch
+    sequence, keeping the split operands it produces; the parameters are saved with ``save_for_backward`` (changing one
+    in place before the backward raises autograd's usual error).  The backward frees the kept operands: a second
+    backward (``retain_graph=True``) raises."""
+
+    @staticmethod
+    def forward(ctx, enc, frames, *params):
+        keep = []
+        feat = enc._forward(frames, "f32", keep)
+        ctx.enc, ctx.keep = enc, keep
+        ctx.save_for_backward(frames, feat, *params)
+        return feat
+
+    @staticmethod
+    def backward(ctx, grad):
+        if ctx.keep is None:
+            raise RuntimeError("Encoder: the backward frees the operands it keeps, so the features cannot be "
+                               "backpropagated a second time (retain_graph=True is not supported); run the forward again")
+        frames, feat = ctx.saved_tensors[:2]        # raises if a parameter was modified in place since the forward
+        needs = ctx.needs_input_grad[2:]
+        need = [(needs[2 * k], needs[2 * k + 1]) for k in range(len(_ENC))]
+        grads = _encoder_backward(ctx.enc, frames, ctx.keep, feat, grad, need)
+        ctx.keep = None
+        return (None, None) + tuple(grads)
 
 
 class deconv(nn.Module):
@@ -290,14 +379,91 @@ class InpaintGenerator(BaseNetwork):
         # tanh and the NCHW layout of the prediction are fused into the last decoder conv's epilogue
         return self._decode(enc_feat), pred_flows
 
-    def _decode(self, x):
-        """tanh(self.decoder(x)) (e2fgvi.py:143-150, :262) with the convs on the wgmma kernel, LeakyReLU(0.2) fused, and
-        tanh + the NCHW store fused into the output conv."""
+    def decode(self, feat):
+        """``tanh(self.decoder(feat))``, the decoder step of e2fgvi.py:262: feat (N, 128, h, w) -> prediction (N, 3, 4h, 4w)
+        fp32, on ``_decode``'s kernel sequence.  With grad mode on and ``feat`` or some decoder parameter requiring
+        grad, the prediction carries a ``grad_fn`` into both (``_DecodeGrad``); its values are the same bits."""
+        params = self._decoder_params()
+        if torch.is_grad_enabled() and (feat.requires_grad or any(p.requires_grad for p in params)):
+            return _DecodeGrad.apply(self, feat, *params)
+        return self._decode(feat)
+
+    def _decoder_params(self):
         d = self.decoder
-        y = ops.conv3x3([ops.upsample2x_split(x)], d[0].conv.weight, d[0].conv.bias, negative_slope=0.2, out="split")
-        y = ops.conv3x3([y], d[2].weight, d[2].bias, negative_slope=0.2)
-        y = ops.conv3x3([ops.upsample2x_split(y)], d[4].conv.weight, d[4].conv.bias, negative_slope=0.2, out="split")
-        return ops.conv3x3_tanh_nchw(y, d[6].weight, d[6].bias)
+        return [t for conv in (d[0].conv, d[2], d[4].conv, d[6]) for t in (conv.weight, conv.bias)]
+
+    def _decode(self, x, keep=None):
+        """tanh(self.decoder(x)) (e2fgvi.py:143-150, :262) with the convs on the wgmma kernel, LeakyReLU(0.2) fused, and
+        tanh + the NCHW store fused into the output conv.  ``keep`` (a list or None) receives the convs' operands: the
+        upsampled input, the first conv's output, the second's (fp32), its upsample and the third's output."""
+        d = self.decoder
+        u0 = ops.upsample2x_split(x)
+        y1 = ops.conv3x3([u0], d[0].conv.weight, d[0].conv.bias, negative_slope=0.2, out="split")
+        y2 = ops.conv3x3([y1], d[2].weight, d[2].bias, negative_slope=0.2)
+        u1 = ops.upsample2x_split(y2)
+        y3 = ops.conv3x3([u1], d[4].conv.weight, d[4].conv.bias, negative_slope=0.2, out="split")
+        if keep is not None:
+            keep += [u0, y1, y2, u1, y3]
+        return ops.conv3x3_tanh_nchw(y3, d[6].weight, d[6].bias)
+
+
+def _decode_backward(gen, keep, pred, grad, need, want_feat):
+    """Gradients of ``decode``: need[i] = (weight, bias) of decoder conv i (decoder[0].conv, [2], [4].conv, [6]) need a
+    gradient, ``want_feat`` the input's.  tanh's derivative feeds the output conv's gradients; each input gradient
+    fuses LeakyReLU's derivative at the activation it reaches (after the upsample adjoint for the deconvs).  Returns
+    ([dW0, db0, ...], d feat (N, 128, h, w) or None)."""
+    d = gen.decoder
+    convs = (d[0].conv, d[2], d[4].conv, d[6])
+    u0, y1, y2, u1, y3 = keep
+    srcs = (u0, y1, u1, y3)
+    grads = [None] * 8
+    active = [i for i in range(4) if any(need[i])]
+    lowest = 0 if want_feat else (active[0] if active else 4)
+    if lowest == 4:
+        return grads, None
+    dy32, dy = ops.tanh_backward_rows(grad, pred, lead=1)
+    cout = convs[3].out_channels
+    dfeat = None
+    for i in range(3, lowest - 1, -1):
+        nw, nb = need[i]
+        if nw or nb:
+            dw, db = ops.conv3x3_wgrad(dy32[..., :cout] if i == 3 else dy32, [srcs[i]], with_bias=nb)
+            grads[2 * i] = dw if nw else None
+            grads[2 * i + 1] = db
+        if i == 3 and lowest < 3:
+            dy32, dy = ops.conv_dgrad(dy, convs[3].weight, act=y3, out="both")
+        elif i == 2 and lowest < 2:
+            dy32, dy = ops.upsample2x_backward(ops.conv_dgrad(dy, convs[2].weight), act=y2, out="both")
+        elif i == 1 and lowest < 1:
+            dy32, dy = ops.conv_dgrad(dy, convs[1].weight, act=y1, out="both")
+        elif i == 0 and want_feat:
+            dfeat = ops.upsample2x_backward(ops.conv_dgrad(dy, convs[0].weight)).permute(0, 3, 1, 2)
+    return grads, dfeat
+
+
+class _DecodeGrad(torch.autograd.Function):
+    """``InpaintGenerator.decode`` with a backward pass into the four decoder convs and the features.  The forward is
+    ``_decode``'s launch sequence, keeping its operands; the backward frees them (no ``retain_graph``)."""
+
+    @staticmethod
+    def forward(ctx, gen, feat, *params):
+        keep = []
+        pred = gen._decode(feat, keep)
+        ctx.gen, ctx.keep = gen, keep
+        ctx.save_for_backward(pred, *params)
+        return pred
+
+    @staticmethod
+    def backward(ctx, grad):
+        if ctx.keep is None:
+            raise RuntimeError("decode: the backward frees the operands it keeps, so the prediction cannot be "
+                               "backpropagated a second time (retain_graph=True is not supported); run the forward again")
+        pred = ctx.saved_tensors[0]                # raises if a parameter was modified in place since the forward
+        needs = ctx.needs_input_grad[2:]
+        need = [(needs[2 * i], needs[2 * i + 1]) for i in range(4)]
+        grads, dfeat = _decode_backward(ctx.gen, ctx.keep, pred, grad, need, ctx.needs_input_grad[1])
+        ctx.keep = None
+        return (None, dfeat) + tuple(grads)
 
 
 class InpaintGeneratorHQ(InpaintGenerator):

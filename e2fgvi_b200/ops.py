@@ -1320,6 +1320,202 @@ def conv2d_wgrad(dy, x, cin, with_bias=True):
     return dw, db
 
 
+# ------------------------------------------------------------------------------------- encoder / decoder backward
+def conv_dgrad_s2_taps():
+    """(phase, ky, kx) of the stride-2 / pad-1 3x3 input gradient's taps in the kernel's order: phase ph = 2 (y % 2) +
+    (x % 2) of the output pixel (y, x) takes the taps with ky = y + 1 and kx = x + 1 (mod 2), in increasing order; tap
+    (ky, kx) of pixel (2 gy + oy, 2 gx + ox) reads dY at (gy + (oy + 1 - ky) / 2, gx + (ox + 1 - kx) / 2)."""
+    return [(ph, ky, kx) for ph in range(4) for ky in range(3) for kx in range(3)
+            if (ph // 2 + 1 - ky) % 2 == 0 and (ph % 2 + 1 - kx) % 2 == 0]
+
+
+def source_dgrad_weight(weight, groups=1, src_channels=None, source=0):
+    """The stride-1 input gradient's weight for one source of a (grouped, multi-source) conv: fp32 (Cout, Cin/G, k, k)
+    -> a conv weight (C_s, Cout/G, k, k), G groups, with Wt[g cig + ci][co][ky][kx] = W[g cog + co][off + ci][k-1-ky]
+    [k-1-kx] (cig = C_s / G, off = the source's offset in the group-wise concatenation)."""
+    cout, cin_g, k, _ = weight.shape
+    src_channels = [cin_g * groups] if src_channels is None else list(src_channels)
+    cig = src_channels[source] // groups
+    off = sum(c // groups for c in src_channels[:source])
+    w = weight.detach().float().view(groups, cout // groups, cin_g, k, k)[:, :, off: off + cig]
+    return w.transpose(1, 2).reshape(groups * cig, cout // groups, k, k).flip(2, 3).contiguous()
+
+
+def pack_conv_dgrad_s2_weight(weight, src_channels=None, source=0):
+    """The stride-2 input gradient's weight (groups 1): fp32 (Cout, Cin, 3, 3) -> (hi, lo) bf16 (C_s, 9 *
+    ceil(Cout / 64) * 64), taps in ``conv_dgrad_s2_taps`` order, Wt[ci][tap][co] = W[co][off + ci][ky][kx]."""
+    cout, cin = weight.shape[:2]
+    src_channels = [cin] if src_channels is None else list(src_channels)
+    off, cs = sum(src_channels[:source]), src_channels[source]
+    idx = torch.tensor([3 * ky + kx for _, ky, kx in conv_dgrad_s2_taps()], device=weight.device)
+    p = weight.detach().float()[:, off: off + cs].reshape(cout, cs, 9).index_select(2, idx).permute(1, 2, 0)
+    kc = -(-cout // 64) * 64
+    p = torch.nn.functional.pad(p, (0, kc - cout))
+    return split_bf16(p.reshape(cs, 9 * kc))
+
+
+def _dgrad_operand(weight, groups, src_channels, source, stride, rows_cin):
+    """(hi, lo, effective groups) of an input gradient's weight, the value of its ("dgrad", ...) ``_derived`` entry."""
+    if stride == 2:
+        return (*pack_conv_dgrad_s2_weight(weight, src_channels, source), 1)
+    wt = source_dgrad_weight(weight, groups, src_channels, source)
+    if rows_cin:
+        return (*pack_conv_rows_weight(wt, rows_cin), 1)
+    return _conv3x3_operand(wt, [weight.shape[0]], groups, 0)
+
+
+def conv_dgrad(dy, weight, groups=1, stride=1, in_size=None, src_channels=None, source=0, act=None, residual=None,
+               out="f32"):
+    """Input gradient of one source of a k x k conv (``e2f_conv_dgrad_bf16x3``): k = 3 or 7 at stride 1 (pad k // 2),
+    k = 3 at stride 2 (pad 1); groups 1 / 2 / 4 / 8; the forward read ``src_channels`` group-wise concatenated and this
+    is the gradient of source ``source``.  dy: the gradient of the conv's output as a dense ``SplitNHWC``, or a
+    ``RowsNHWC`` with lead k // 2 (stride 1, groups 1).  weight: the forward's nn.Conv2d weight.  in_size: the forward's
+    input (h, w) (default: dy's size, stride 1).  The result is (acc + residual) * LeakyReLU(0.2)'(act): ``residual``
+    fp32 (N, h, w, C_s) NHWC or None, ``act`` the source's ``SplitNHWC`` (its hi part decides) or None.
+    out = "f32": dx fp32 (N, h, w, C_s) NHWC; "split": its ``SplitNHWC``; "both": (dx, SplitNHWC)."""
+    cout, cin_g, ks, _ = weight.shape
+    src_channels = [cin_g * groups] if src_channels is None else list(src_channels)
+    cs = src_channels[source]
+    rows = isinstance(dy, RowsNHWC)
+    if dy.shape[1] != cout or sum(src_channels) != cin_g * groups:
+        raise ValueError(f"conv_dgrad: dy {dy.shape} / sources {src_channels} do not match the weight {tuple(weight.shape)}")
+    if rows and dy.lead != ks // 2:
+        raise ValueError(f"conv_dgrad: a row-gapped dy needs lead {ks // 2}")
+    n, _, h_o, w_o = dy.shape
+    h, w = in_size if in_size is not None else (h_o, w_o)
+    if ((h - 1) // stride + 1, (w - 1) // stride + 1) != (h_o, w_o):
+        raise ValueError(f"conv_dgrad: input size {(h, w)} does not give dy's {(h_o, w_o)} at stride {stride}")
+    _need_cuda(weight, dy.hi, residual)
+    dy_c = dy.cin if rows else dy.hi.shape[-1]
+    act_ptr = None
+    if act is not None:
+        if act.shape != (n, cs, h, w) or act.hi.shape[-1] != cs:
+            raise ValueError(f"conv_dgrad: act {act.shape} does not match ({n}, {cs}, {h}, {w})")
+        act_ptr = act.hi.data_ptr()
+    res = None
+    if residual is not None:
+        if tuple(residual.shape) != (n, h, w, cs):
+            raise ValueError(f"conv_dgrad: residual {tuple(residual.shape)} != {(n, h, w, cs)}")
+        res = residual.contiguous().float()
+    dx, ohi, olo = _outputs(out, ("f32", "split", "both"), (n, h, w, cs), weight.device)
+    rows_cin = dy_c if rows else 0
+    w_hi, w_lo, g_eff = _derived_one(weight, ("dgrad", tuple(src_channels), groups, source, stride, rows_cin),
+                                     _dgrad_operand, groups, src_channels, source, stride, rows_cin)
+    with _timed(f"conv_dgrad_c{cs}", 2.0 * n * h_o * w_o * cout * (cs // groups) * ks * ks):
+        st = _lib.load().e2f_conv_dgrad_bf16x3(dy.hi.data_ptr(), dy.lo.data_ptr(), dy_c, dy.lead if rows else 0,
+                                               w_hi.data_ptr(), w_lo.data_ptr(), act_ptr,
+                                               None if res is None else res.data_ptr(),
+                                               None if dx is None else dx.data_ptr(),
+                                               None if ohi is None else ohi.data_ptr(),
+                                               None if olo is None else olo.data_ptr(), n, h, w, cs, g_eff, ks, stride,
+                                               _stream())
+    _lib.check(st, "e2f_conv_dgrad_bf16x3")
+    return _result(out, dx, None if ohi is None else SplitNHWC(ohi, olo, (n, cs, h, w)))
+
+
+def conv3x3_wgrad(dy, sources, groups=1, stride=1, with_bias=True, cin=None):
+    """(dW fp32 (Cout, Cin/G, 3, 3), db fp32 (Cout,) or None) of a 3x3 / pad 1 conv (``e2f_conv3x3_wgrad_bf16x3``) from dy
+    fp32 (N, h_o, w_o, Cout) NHWC (Cout padded to a multiple of 8 here) and the forward's operands: a list of one or two
+    dense ``SplitNHWC`` read group-wise concatenated, or one ``RowsNHWC`` with lead 1.  ``cin``: keep the first cin input
+    channels (a row-gapped source's padding channels get their own, zero-valued, gradient)."""
+    sources = list(sources) if isinstance(sources, (list, tuple)) else [sources]
+    n, h_o, w_o, cout = dy.shape
+    _need_cuda(dy, *[s_.hi for s_ in sources])
+    rows = isinstance(sources[0], RowsNHWC)
+    if rows and (len(sources) != 1 or sources[0].lead != 1):
+        raise ValueError("conv3x3_wgrad: a row-gapped operand must be the only source and have lead 1")
+    h, w = sources[0].shape[2:]
+    for s_ in sources:
+        if s_.shape[0] != n or tuple(s_.shape[2:]) != (h, w):
+            raise ValueError("conv3x3_wgrad: sources must share N, H, W")
+    if ((h - 1) // stride + 1, (w - 1) // stride + 1) != (h_o, w_o):
+        raise ValueError(f"conv3x3_wgrad: dy {tuple(dy.shape)} is not the stride-{stride} output of {(h, w)}")
+    dy = dy.contiguous().float()
+    cpad = -(-cout // 8) * 8
+    if cpad != cout:
+        dy = torch.nn.functional.pad(dy, (0, cpad - cout))
+    lib = _lib.load()
+    x_c = [s_.cin if rows else s_.hi.shape[-1] for s_ in sources]
+    xc = sum(x_c)
+    elems = lib.e2f_conv3x3_wgrad_work_elems(n, h, w, xc, cpad, groups, stride)
+    if elems < 0:
+        _lib.check(int(elems), "e2f_conv3x3_wgrad_work_elems")
+    work = torch.empty(int(elems), dtype=torch.float32, device=dy.device)
+    dw = torch.empty(cpad, xc // groups, 3, 3, dtype=torch.float32, device=dy.device)
+    db = torch.empty(cpad, dtype=torch.float32, device=dy.device) if with_bias else None
+    hi_p, lo_p, c_p = _source_arrays(sources)
+    with _timed(f"conv3x3_wgrad_c{cout}", 2.0 * n * h_o * w_o * cout * (xc // groups) * 9):
+        st = lib.e2f_conv3x3_wgrad_bf16x3(dy.data_ptr(), len(sources), hi_p, lo_p, c_p, 1 if rows else 0, dw.data_ptr(),
+                                          None if db is None else db.data_ptr(), work.data_ptr(), n, h, w, cpad, groups,
+                                          stride, _stream())
+    _lib.check(st, "e2f_conv3x3_wgrad_bf16x3")
+    keep = xc // groups if cin is None else cin
+    if cpad != cout or keep != xc // groups:
+        dw = dw[:cout, :keep].contiguous()
+    if db is not None and cpad != cout:
+        db = db[:cout].contiguous()
+    return dw, db
+
+
+def upsample2x_backward(dy, act=None, out="f32"):
+    """Adjoint of ``upsample2x_split`` (x2 bilinear, align_corners=True): dy fp32 (N, 2H, 2W, C) NHWC -> dx (N, H, W, C)
+    NHWC, times LeakyReLU(0.2)'(act) when ``act`` (fp32 (N, C, H, W), the upsampled LeakyReLU output) is given.
+    out = "f32" | "split" | "both" as ``conv_dgrad``."""
+    _need_cuda(dy, act)
+    n, oh, ow, c = dy.shape
+    h, w = oh // 2, ow // 2
+    if (oh, ow) != (2 * h, 2 * w) or c % 8:
+        raise ValueError(f"upsample2x_backward: dy {tuple(dy.shape)} (even H, W and C % 8 == 0)")
+    a = None
+    if act is not None:
+        if tuple(act.shape) != (n, c, h, w):
+            raise ValueError(f"upsample2x_backward: act {tuple(act.shape)} != {(n, c, h, w)}")
+        a = act.permute(0, 2, 3, 1).contiguous().float()        # no-op for channels_last
+    dy = dy.contiguous().float()
+    dx, hi, lo = _outputs(out, ("f32", "split", "both"), (n, h, w, c), dy.device)
+    with _timed("upsample2x_backward", float(dy.numel() * 4 + n * h * w * c * 4 * (1 + (a is not None)))):
+        st = _lib.load().e2f_upsample2x_backward(dy.data_ptr(), None if a is None else a.data_ptr(),
+                                                 None if dx is None else dx.data_ptr(), None if hi is None else hi.data_ptr(),
+                                                 None if lo is None else lo.data_ptr(), n, h, w, c, _stream())
+    _lib.check(st, "e2f_upsample2x_backward")
+    return _result(out, dx, None if hi is None else SplitNHWC(hi, lo, (n, c, h, w)))
+
+
+def tanh_backward_rows(dout, out, lead=1):
+    """dY = dOut * (1 - out^2) of the prediction ``out = tanh(conv)`` (both fp32 (N, C, H, W), C <= 8): returns (dy fp32
+    (N, H, W, 8) NHWC, channels >= C zero — the weight gradient's operand; the row-gapped ``RowsNHWC`` of dy with
+    ``lead`` — the input gradient's operand)."""
+    _need_cuda(dout, out)
+    n, c, h, w = out.shape
+    if tuple(dout.shape) != (n, c, h, w):
+        raise ValueError(f"tanh_backward_rows: dout {tuple(dout.shape)} != out {tuple(out.shape)}")
+    dout, out = dout.contiguous().float(), out.contiguous().float()
+    dy = torch.empty((n, h, w, 8), dtype=torch.float32, device=out.device)
+    hi, lo = _rows_pair(n, h, w, lead, 8, out.device)
+    with _timed("tanh_backward_rows", float(out.numel() * 8 + dy.numel() * 4 + hi.numel() * 4)):
+        st = _lib.load().e2f_tanh_backward_rows(dout.data_ptr(), out.data_ptr(), dy.data_ptr(), hi.data_ptr(),
+                                                lo.data_ptr(), n, c, h, w, lead, _stream())
+    _lib.check(st, "e2f_tanh_backward_rows")
+    return dy, RowsNHWC(hi, lo, (n, c, h, w), lead, 8)
+
+
+def leaky_relu_backward(dy, act, slope=0.2, out="both"):
+    """dy * LeakyReLU(slope)'(act) for two fp32 NHWC tensors of one shape (N, H, W, C): out = "f32" | "split" | "both"
+    as ``conv_dgrad``."""
+    _need_cuda(dy, act)
+    if dy.shape != act.shape or dy.dim() != 4:
+        raise ValueError(f"leaky_relu_backward: dy {tuple(dy.shape)} and act {tuple(act.shape)} must be one (N, H, W, C)")
+    dy, act = dy.contiguous().float(), act.contiguous().float()
+    n, h, w, c = dy.shape
+    dx, hi, lo = _outputs(out, ("f32", "split", "both"), dy.shape, dy.device)
+    with _timed("leaky_relu_backward", float(dy.numel() * (8 + 4 * (dx is not None) + 4 * (hi is not None)))):
+        st = _lib.load().e2f_leaky_relu_backward(dy.data_ptr(), act.data_ptr(), None if dx is None else dx.data_ptr(),
+                                                 None if hi is None else hi.data_ptr(), None if lo is None else lo.data_ptr(),
+                                                 dy.numel(), float(slope), _stream())
+    _lib.check(st, "e2f_leaky_relu_backward")
+    return _result(out, dx, None if hi is None else SplitNHWC(hi, lo, (n, c, h, w)))
+
+
 def attention_flops(B, T, H, W, C, window_size, expand_size, focal_window, use_pooled=True):
     """Algorithmic FLOPs of one attention launch as the REFERENCE counts keys (SURVEY §8d): QK^T + PV over
     T*(own window + listed ring keys incl. duplicates + fh*fw pooled keys incl. masked ones) keys per query."""

@@ -549,6 +549,52 @@ int64_t e2f_conv2d_wgrad_work_elems(int n, int h, int w, int cin, int cout);
 int e2f_conv2d_wgrad_bf16x3(const float* dy, const void* x_hi, const void* x_lo, int x_lead, float* dw, float* db, float* work,
                             int n, int h, int w, int cin, int cout, void* stream);
 
+/* Gradients of the encoder's and decoder's convs (3x3 / pad 1, stride 1 or 2, groups 1 / 2 / 4 / 8, one or two sources
+ * read group-wise concatenated) and of the element-wise steps between them, bf16 three-term splits with fp32
+ * accumulation.  The forward conv reads X [n][h_in][w_in][cin] and writes Y [n][h_o][w_o][cout], h_o = (h_in - 1) /
+ * stride + 1.
+ *   e2f_conv_dgrad_bf16x3 : input gradient dX [n][h_in][w_in][cin] of one source of a k x k conv (k = 3 or 7 at stride 1
+ *       with pad k / 2, k = 3 at stride 2 with pad 1) from dY = (dy_hi, dy_lo) with dy_c channels: dense [n][h_o][w_o][dy_c],
+ *       or row-gapped with dy_lead = k / 2 (stride 1, groups 1, dy_c 8, 16 or 32; see e2f_conv_rows_pitch).  Stride 1:
+ *       the weight is that source's rows of the group weights rotated by 180 degrees with in / out swapped, a conv
+ *       weight [cin][dy_c / groups][k][k] with Wt[g cig + ci][co][ky][kx] = W[g cog + co][off + ci][k-1-ky][k-1-kx]
+ *       (cig = cin / groups, off = the source's offset in the group-wise concatenation), packed as
+ *       e2f_conv2d_rows_bf16x3 packs a weight for that dY layout.  Stride 2: four output phases ph = 2 (y % 2) + (x % 2);
+ *       phase ph lists the taps (ky, kx) with ky = y + 1 and kx = x + 1 (mod 2) in increasing order (1, 2, 2, 4 taps),
+ *       and the weight is [cin][9 taps in that order][ceil(dy_c / 64) * 64] with Wt[ci][tap][co] = W[co][ci][ky][kx].
+ *       The epilogue computes (acc + residual) * LeakyReLU(0.2)'(act): `residual` fp32 [n][h_in][w_in][cin] or NULL,
+ *       `act` (bf16 hi part of the LeakyReLU output that is the source, [n][h_in][w_in][cin]) or NULL.  Outputs: fp32 dx
+ *       and/or its split (the next input gradient's dY).  cin a multiple of 8 per group, <= 512.
+ *   e2f_conv3x3_wgrad_work_elems / e2f_conv3x3_wgrad_bf16x3 : dw fp32 [cout][cin / groups][3][3] (the torch layout) and,
+ *       if db is not NULL, db fp32 [cout] = the sum of dy over pixels, from dy fp32 [n][h_o][w_o][cout] and the forward's
+ *       operands: nsrc = 1 or 2 sources (x_hi[i], x_lo[i]) [n][h_in][w_in][x_c[i]], group g reading channels [g x_c[i] /
+ *       groups, (g + 1) x_c[i] / groups) of source 0, then of source 1 (cin = the sum of x_c); or one row-gapped source
+ *       with x_lead = 1 (x_c 8, 16 or 32, groups 1: the 3-channel frames packed to 8 channels).  Multiples of 8 channels
+ *       per group.  The split-K GEMM of e2f_dis_conv3d_wgrad: `work` holds e2f_conv3x3_wgrad_work_elems(...) floats
+ *       (negative = bad arguments) and the slices are added in a fixed order: bit-identical from run to run.
+ *   e2f_upsample2x_backward : adjoint of the x2 bilinear upsample with align_corners = True (e2f_upsample2x_split): dx
+ *       [n][h][w][c] from dy [n][2h][2w][c], fp32 NHWC; each input pixel sums the output pixels that sample it in a fixed
+ *       order (no atomics).  `act` (fp32 [n][h][w][c], the LeakyReLU(0.2) output that was upsampled) or NULL: times that
+ *       LeakyReLU's derivative.  Outputs: fp32 dx and/or its split.  c % 8 == 0.
+ *   e2f_tanh_backward_rows : dY = dOut * (1 - out^2) of out = tanh(conv) from dout, out fp32 NCHW [n][c][h][w] (c <= 8):
+ *       fp32 dy [n][h][w][8] (channels >= c zero: the weight gradient's operand) and the row-gapped split (dy_hi, dy_lo)
+ *       with `lead` zero pixels per row and 8 channels (the input gradient's operand; e2f_conv_rows_pitch / _tail).
+ *   e2f_leaky_relu_backward : dx = dy * LeakyReLU(slope)'(act) over `count` fp32 elements (count % 8 == 0): fp32 dx
+ *       and/or its split. */
+int e2f_conv_dgrad_bf16x3(const void* dy_hi, const void* dy_lo, int dy_c, int dy_lead, const void* wt_hi, const void* wt_lo,
+                          const void* act, const float* residual, float* dx, void* dx_hi, void* dx_lo, int n, int h_in,
+                          int w_in, int cin, int groups, int ks, int stride, void* stream);
+int64_t e2f_conv3x3_wgrad_work_elems(int n, int h_in, int w_in, int cin, int cout, int groups, int stride);
+int e2f_conv3x3_wgrad_bf16x3(const float* dy, int nsrc, const void* const* x_hi, const void* const* x_lo, const int* x_c,
+                             int x_lead, float* dw, float* db, float* work, int n, int h_in, int w_in, int cout, int groups,
+                             int stride, void* stream);
+int e2f_upsample2x_backward(const float* dy, const float* act, float* dx, void* dx_hi, void* dx_lo, int n, int h, int w, int c,
+                            void* stream);
+int e2f_tanh_backward_rows(const float* dout, const float* out, float* dy, void* dy_hi, void* dy_lo, int n, int c, int h, int w,
+                           int lead, void* stream);
+int e2f_leaky_relu_backward(const float* dy, const float* act, float* dx, void* dx_hi, void* dx_lo, int64_t count, float slope,
+                            void* stream);
+
 /* Number of kernel launches issued through this library since load (all threads); used by bench.py's
  * "gpu_launches" accounting. */
 int64_t e2f_launch_count(void);
