@@ -29,9 +29,12 @@ SIGNATURES = {
     "e2f_t2t_fold_nhwc": (_i, [_fp, _fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "e2f_t2t_unfold_nhwc": (_i, [_fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "e2f_t2t_fold_unfold": (_i, [_fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "e2f_t2t_fold_unfold_train": (_i, [_fp, _fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "e2f_t2t_fold": (_i, [_fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "e2f_split_bf16": (_i, [_fp, _vp, _vp, _c.c_int64, _vp]),
     "e2f_linear_bf16x3": (_i, [_vp, _vp, _vp, _vp, _fp, _fp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "e2f_linear_wgrad_work_elems": (_c.c_int64, [_i, _i, _i]),
+    "e2f_linear_wgrad_bf16x3": (_i, [_vp, _vp, _i, _vp, _vp, _i, _fp, _fp, _fp, _i, _i, _i, _vp]),
     "e2f_conv3x3_bf16x3": (_i, [_i, _c.POINTER(_vp), _c.POINTER(_vp), _c.POINTER(_i), _vp, _vp, _fp, _fp, _fp, _vp, _vp,
                                 _i, _i, _i, _i, _i, _f, _vp]),
     "e2f_conv2d_bf16x3": (_i, [_i, _c.POINTER(_vp), _c.POINTER(_vp), _c.POINTER(_i), _vp, _vp, _fp, _fp, _fp, _vp, _vp,

@@ -221,6 +221,24 @@ int e2f_t2t_fold_unfold(const float* tokens_in, float* tokens, void* tokens_hi, 
   return finish(st, "e2f_t2t_fold_unfold");
 }
 
+int e2f_t2t_fold_unfold_train(const float* tokens_in, float* u, float* tokens, void* tokens_hi, void* tokens_lo, int bt, int c,
+                              int h, int w, int k, int stride, int pad, int backward, int out_pitch, void* stream) {
+  const char* who = "e2f_t2t_fold_unfold_train";
+  if ((!tokens && !tokens_hi) || (!tokens_hi) != (!tokens_lo)) { set_error("%s: need tokens and/or both of tokens_hi/tokens_lo", who); return E2F_ERR_BAD_ARG; }
+  if (!u) { set_error("%s: null u", who); return E2F_ERR_BAD_ARG; }
+  if (backward != 0 && backward != 1) { set_error("%s: backward=%d (0 or 1)", who, backward); return E2F_ERR_BAD_ARG; }
+  int st = t2t_checks(who, tokens_in, tokens ? static_cast<const void*>(tokens) : tokens_hi, bt, c, h, w, k, stride, pad);
+  if (st) return st;
+  if (!aligned(u, 16) || (tokens_hi && (!aligned(tokens_hi, 16) || !aligned(tokens_lo, 16)))) { set_error("%s: 16-byte alignment required", who); return E2F_ERR_ALIGNMENT; }
+  if (out_pitch == 0) out_pitch = c * k * k;
+  if (out_pitch < c * k * k || out_pitch % 4) { set_error("%s: out_pitch=%d must be 0 or a multiple of 4 >= C*k*k=%d", who, out_pitch, c * k * k); return E2F_ERR_BAD_ARG; }
+  if (k != 7 || stride != 3 || pad != 3 || c % 4 || bt > 65535) { set_error("%s: only k=7 stride=3 pad=3 with C %% 4 == 0 and bt <= 65535 (k=%d s=%d p=%d c=%d)", who, k, stride, pad, c); return E2F_ERR_UNSUPPORTED; }
+  st = launch_t2t_fold_unfold(tokens_in, tokens, tokens_hi, tokens_lo, bt, c, h, w, k, stride, pad, 1, out_pitch,
+                              static_cast<cudaStream_t>(stream), backward ? u : nullptr, backward ? nullptr : u);
+  if (st == E2F_ERR_UNSUPPORTED) { set_error("%s: the image (w=%d) does not fit the fused kernel's shared memory", who, w); return st; }
+  return finish(st, who);
+}
+
 int e2f_layernorm_pool_split(const float* x, const float* gamma, const float* beta, const float* pool_w,
                              const float* pool_b, void* out_hi, void* out_lo, int bt, int h, int w, int c, int wh, int ww,
                              float eps, void* stream) {
@@ -794,6 +812,27 @@ int e2f_conv_dgrad_bf16x3(const void* dy_hi, const void* dy_lo, int dy_c, int dy
   if (n == 0) return 0;
   return finish(launch_conv_dgrad(dy_hi, dy_lo, dy_c, dy_lead, wt_hi, wt_lo, act, residual, dx, dx_hi, dx_lo, n, h_in, w_in,
                                   cin, groups, ks, stride, static_cast<cudaStream_t>(stream)), who);
+}
+
+static bool linear_wgrad_ok(const char* who, int m, int n, int k) {
+  if (m < 0 || n <= 0 || k <= 0) { set_error("%s: bad shape m=%d n=%d k=%d", who, m, n, k); return false; }
+  return true;
+}
+
+int64_t e2f_linear_wgrad_work_elems(int m, int n, int k) {
+  if (!linear_wgrad_ok("e2f_linear_wgrad_work_elems", m, n, k)) return E2F_ERR_BAD_ARG;
+  return static_cast<int64_t>(linear_wgrad_work_elems(m, n, k));
+}
+
+int e2f_linear_wgrad_bf16x3(const void* dy_hi, const void* dy_lo, int ldy, const void* x_hi, const void* x_lo, int ldx, float* dw,
+                            float* db, float* work, int m, int n, int k, void* stream) {
+  const char* who = "e2f_linear_wgrad_bf16x3";
+  if (!dy_hi || !dy_lo || !x_hi || !x_lo || !dw) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if (!linear_wgrad_ok(who, m, n, k)) return E2F_ERR_BAD_ARG;
+  if (ldy < n || ldx < k || ldy % 8 || ldx % 8) { set_error("%s: row pitches ldy=%d ldx=%d must be multiples of 8 >= n=%d / k=%d", who, ldy, ldx, n, k); return E2F_ERR_BAD_ARG; }
+  if (!work && linear_wgrad_work_elems(m, n, k) > 0) { set_error("%s: null workspace (e2f_linear_wgrad_work_elems floats needed)", who); return E2F_ERR_BAD_ARG; }
+  if (!aligned(dy_hi, 16) || !aligned(dy_lo, 16) || !aligned(x_hi, 16) || !aligned(x_lo, 16) || !aligned(dw, 4) || (db && !aligned(db, 4)) || (work && !aligned(work, 4))) { set_error("%s: alignment (operands 16 bytes)", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_linear_wgrad(dy_hi, dy_lo, ldy, x_hi, x_lo, ldx, dw, db, work, m, n, k, static_cast<cudaStream_t>(stream)), who);
 }
 
 static bool conv3x3_wgrad_ok(const char* who, int n, int h_in, int w_in, int cin, int cout, int groups, int stride) {

@@ -206,6 +206,16 @@ template <int N, bool F16>
 __device__ __forceinline__ void wgmma_ss(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
   WgmmaSS<N, F16>::run(d, adesc, bdesc, acc);
 }
+// D[64 x 128] (+)= A[64 x 16] . B[128 x 16]^T with BOTH operands MN-major (transposed) bf16 in shared memory: the
+// operands of a weight gradient, whose reduction runs over the outer (token) index of both.  A: one 64-element atom along
+// M; B: two atoms along N, LBO apart; 8-k groups SBO apart in both.
+__device__ __forceinline__ void wgmma_n128_bf16_tt(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {" E2F_WR0 E2F_WR1 E2F_WR2 E2F_WR3 E2F_WR4 E2F_WR5
+               E2F_WR6 E2F_WR7 "}, %64, %65, p, 1, 1, 1, 1;\n}\n"
+               : E2F_WD64(0)
+               : "l"(adesc), "l"(bdesc), "r"(acc));
+}
 // register-A variant (A fragment in registers, B transposed = MN-major in shared memory)
 __device__ __forceinline__ void wgmma_n64_f16_rs_tb(float* d, const uint32_t (&a)[4], uint64_t bdesc, uint32_t acc) {
   asm volatile(

@@ -94,8 +94,11 @@ int launch_layernorm_pool_split(const float* x, const float* gamma, const float*
                                 float eps, cudaStream_t stream);
 int launch_window_pool(const void* xh, const void* xl, const float* weight, const float* bias, float* out, void* out_hi,
                        void* out_lo, int bt, int h, int w, int c, int wh, int ww, cudaStream_t stream);
+// gu != nullptr: the adjoint of the training forward (tin = dz, gu = its saved u); u_out != nullptr (gelu only): the
+// training forward, which also writes u = the normalised values before GELU.  Both [BT][L][C*k*k] fp32.
 int launch_t2t_fold_unfold(const float* tin, float* tok, void* tok_hi, void* tok_lo, int bt, int c, int h, int w, int k,
-                           int s, int p, int gelu, int out_pitch, cudaStream_t stream);
+                           int s, int p, int gelu, int out_pitch, cudaStream_t stream, const float* gu = nullptr,
+                           float* u_out = nullptr);
 int launch_t2t_fold_nhwc(const float* tok, const float* bias, const float* residual, float* img, int bt, int c, int h,
                          int w, int k, int s, int p, int normalize, cudaStream_t stream);
 int launch_t2t_fold(const float* tok, const float* bias, float* img, int bt, int c, int h, int w, int k, int s,
@@ -104,6 +107,12 @@ int launch_t2t_fold(const float* tok, const float* bias, float* img, int bt, int
 int launch_split_bf16(const float* x, void* hi, void* lo, long long n, cudaStream_t stream);
 int launch_linear_bf16x3(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, const float* bias,
                          const float* residual, void* out, int m, int n, int k, int out_dtype, cudaStream_t stream);
+// Linear weight / bias gradient (linear_wgrad.cu): dW [n][k] = dY^T X, db [n] = column sums of dY, from the split
+// dY [m][ldy] and X [m][ldx]; split-K workspace of linear_wgrad_work_elems floats (0: none needed).
+int linear_wgrad_slices(int m, int n, int k);
+long long linear_wgrad_work_elems(int m, int n, int k);
+int launch_linear_wgrad(const void* dy_hi, const void* dy_lo, int ldy, const void* x_hi, const void* x_lo, int ldx, float* dw,
+                        float* db, float* work, int m, int n, int k, cudaStream_t stream);
 
 // Optional generalised geometry of the implicit-GEMM conv ("gather conv", see conv.cu Params): explicit tap offsets,
 // output phases and tile shape.  nullptr = the plain k x k / stride / pad conv.

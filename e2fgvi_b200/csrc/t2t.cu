@@ -13,6 +13,13 @@
 namespace e2f {
 
 __device__ __forceinline__ float gelu_exact(float v) { return 0.5f * v * (1.0f + erff(v * 0.70710678118654752f)); }
+// dz * GELU'(u), GELU'(u) = Phi(u) + u phi(u): the prologue of the fold/normalise/unfold adjoint
+__device__ __forceinline__ float gelu_grad(float dz, float u) {
+  return dz * (0.5f * (1.0f + erff(u * 0.70710678118654752f)) + u * 0.39894228040143268f * __expf(-0.5f * u * u));
+}
+__device__ __forceinline__ float4 gelu_grad4(float4 dz, float4 u) {
+  return make_float4(gelu_grad(dz.x, u.x), gelu_grad(dz.y, u.y), gelu_grad(dz.z, u.z), gelu_grad(dz.w, u.w));
+}
 
 // one thread per 4 consecutive token channels (float4 store); channel = c*k*k + ky*k + kx
 // KC/SC/PC: compile-time kernel / stride / padding (the div/mod by 49 and 7 become multiply-shifts); KC = 0 selects
@@ -154,13 +161,18 @@ __global__ void __launch_bounds__(256) t2t_unfold733_kernel(const float* __restr
 // Algorithmic bytes: tokens in (x (TR+4)/TR or (TR+2)/TR halo re-read, served by L2) + tokens / image out.
 // OUT_NHWC (fold only): the image is written channels_last, [BT][H][W][C], with an optional residual of the same
 // layout added (enc_feat + trans_feat of e2fgvi.py:263 folded into the store) — the layout the decoder's convs read.
-template <bool FUSED, bool GELU, int CC, bool OUT_NHWC = false>
+// Training (FUSED only): `u_out` non-null also writes the normalised values before GELU, [BT][L][C*49] fp32 (GELU is then
+// applied at the store); BWD reads `gu` (that u, same layout as tin) and folds tin * GELU'(gu) instead of tin: the
+// operator unfold . (/ fold(ones)) . fold is self-adjoint, so this is the input gradient of the training forward.
+template <bool FUSED, bool GELU, int CC, bool OUT_NHWC = false, bool BWD = false>
 __global__ void __launch_bounds__(256, 3) t2t_fold733_kernel(const float* __restrict__ tin, float* __restrict__ tok,
                                                           __nv_bfloat16* __restrict__ tok_hi,
                                                           __nv_bfloat16* __restrict__ tok_lo, float* __restrict__ img,
                                                           const float* __restrict__ bias, int normalize, int C, int H,
                                                           int W, int FH, int FW, int TR, int CKP,
-                                                          const float* __restrict__ residual = nullptr) {
+                                                          const float* __restrict__ residual = nullptr,
+                                                          const float* __restrict__ gu = nullptr,
+                                                          float* __restrict__ u_out = nullptr) {
   extern __shared__ float simg[];                  // [CC][ROWS][WP], x padded by 3 on both sides; then nx[WP]
   constexpr int RUN4 = CC * 49 / 4;
   const int WP = W + 6, ROWS = FUSED ? 3 * TR + 4 : 3 * TR;
@@ -226,6 +238,12 @@ __global__ void __launch_bounds__(256, 3) t2t_fold733_kernel(const float* __rest
         v[0] = __ldg(reinterpret_cast<const float4*>(gp));
         if (live1) v[1] = __ldg(reinterpret_cast<const float4*>(gp + gslot));
         if (live2) v[2] = __ldg(reinterpret_cast<const float4*>(gp + 2 * gslot));
+        if constexpr (BWD) {
+          const float* up = gu + (gp - tin);
+          v[0] = gelu_grad4(v[0], __ldg(reinterpret_cast<const float4*>(up)));
+          if (live1) v[1] = gelu_grad4(v[1], __ldg(reinterpret_cast<const float4*>(up + gslot)));
+          if (live2) v[2] = gelu_grad4(v[2], __ldg(reinterpret_cast<const float4*>(up + 2 * gslot)));
+        }
       };
       auto foldrow = [&](const float4 (&v)[U]) {
         if (r0 >= 0 && r0 + 7 <= ROWS) {                    // no per-element row checks
@@ -339,7 +357,7 @@ __global__ void __launch_bounds__(256, 3) t2t_fold733_kernel(const float* __rest
       const float rny = 1.0f / static_cast<float>(ny);
       for (int xx = lane; xx < WP; xx += 32) {
         float v = row[xx] * (rny * rnx[xx]);
-        if (GELU) v = gelu_exact(v);
+        if (GELU && !u_out) v = gelu_exact(v);
         row[xx] = v;
       }
     } else {
@@ -370,6 +388,12 @@ __global__ void __launch_bounds__(256, 3) t2t_fold733_kernel(const float* __rest
         for (int e = 0; e < 4; ++e) {
           v[e] = *pe[e];
           pe[e] += 3 * TSUB;
+        }
+        if (GELU && u_out) {
+          const long long du = (tok0 + static_cast<long long>(iy) * FW + tx) * CK + c0 * 49 + q4 * 4;
+          *reinterpret_cast<float4*>(u_out + du) = make_float4(v[0], v[1], v[2], v[3]);
+#pragma unroll
+          for (int e = 0; e < 4; ++e) v[e] = gelu_exact(v[e]);
         }
         if (tok) *reinterpret_cast<float4*>(tok + dst) = make_float4(v[0], v[1], v[2], v[3]);
         if (tok_hi) {
@@ -493,11 +517,14 @@ int launch_t2t_unfold(const float* img, float* tok, void* tok_hi_v, void* tok_lo
 // read-modify-writes suffice — no atomics, deterministic.
 constexpr int MID_CC = 4, MID_RUN4 = MID_CC * 49 / 4, MID_TSUB = 256 / MID_RUN4, MID_U = 4;
 
-template <bool GELU>
+// u_out / BWD / gu: the training forward and the adjoint, as in t2t_fold733_kernel.
+template <bool GELU, bool BWD = false>
 __global__ void __launch_bounds__(256, 2) t2t_ffn_mid_kernel(const float* __restrict__ tin, float* __restrict__ tok,
                                                              __nv_bfloat16* __restrict__ tok_hi,
                                                              __nv_bfloat16* __restrict__ tok_lo, int C, int H, int W, int FH,
-                                                             int FW, int TR, int TW, int XT, int CKP) {
+                                                             int FW, int TR, int TW, int XT, int CKP,
+                                                             const float* __restrict__ gu = nullptr,
+                                                             float* __restrict__ u_out = nullptr) {
   extern __shared__ float simg[];                  // [CC][R][WP] + int ny[R] + int nx[WP]
   const int chunk = blockIdx.x / XT, xt = blockIdx.x - chunk * XT;
   const int c0 = chunk * MID_CC;
@@ -558,6 +585,9 @@ __global__ void __launch_bounds__(256, 2) t2t_ffn_mid_kernel(const float* __rest
         if (t + u * MID_TSUB < ntok) {
           const int ty = fy + 3 * iy, tx = fx + 3 * ix;
           v4[u] = __ldg(reinterpret_cast<const float4*>(src + static_cast<long long>(ty * FW + tx) * CK));
+          if constexpr (BWD)
+            v4[u] = gelu_grad4(v4[u], __ldg(reinterpret_cast<const float4*>(gu + (src - tin) +
+                                                                              static_cast<long long>(ty * FW + tx) * CK)));
           base[u] = 3 * (ty - tyb) * WP + 3 * (tx - txb);
           advance();
         }
@@ -611,7 +641,7 @@ __global__ void __launch_bounds__(256, 2) t2t_ffn_mid_kernel(const float* __rest
       float v = 0.f;
       if (cnt) {
         v = row[xx] / static_cast<float>(cnt);
-        if (GELU) v = gelu_exact(v);
+        if (GELU && !u_out) v = gelu_exact(v);
       }
       row[xx] = v;
     }
@@ -628,6 +658,12 @@ __global__ void __launch_bounds__(256, 2) t2t_ffn_mid_kernel(const float* __rest
 #pragma unroll
       for (int e = 0; e < 4; ++e) v[e] = simg[base + off[e]];
       const long long dst = ((bt * FH + ty0 + iy) * static_cast<long long>(FW) + tx0 + ix) * CKP + c0 * 49 + q4 * 4;
+      if (GELU && u_out) {
+        const long long du = ((bt * FH + ty0 + iy) * static_cast<long long>(FW) + tx0 + ix) * CK + c0 * 49 + q4 * 4;
+        *reinterpret_cast<float4*>(u_out + du) = make_float4(v[0], v[1], v[2], v[3]);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) v[e] = gelu_exact(v[e]);
+      }
       if (tok) *reinterpret_cast<float4*>(tok + dst) = make_float4(v[0], v[1], v[2], v[3]);
       if (tok_hi) {
         const __nv_bfloat162 h0 = __floats2bfloat162_rn(v[0], v[1]), h1 = __floats2bfloat162_rn(v[2], v[3]);
@@ -685,7 +721,7 @@ static int fold733_configure() {
     return e;
   // three ~63 KB bands per SM need the large shared-memory carve-out (ncu: the default left room for two)
   return configure_once_carveout(fullwidth, 200 * 1024, cudaSharedmemCarveoutMaxShared, t2t_fold733_kernel<true, true, 4>,
-                                 t2t_fold733_kernel<true, false, 4>);
+                                 t2t_fold733_kernel<true, false, 4>, t2t_fold733_kernel<true, false, 4, false, true>);
 }
 
 // Fused fold/normalise/unfold(/GELU).  Returns -2 (unsupported) when the geometry is not 7/3/3 or no band fits in
@@ -693,7 +729,8 @@ static int fold733_configure() {
 // First-generation launch (whole image width per block): measured faster than the x-tiled kernel while the image is
 // narrow enough for >= 2 blocks per SM.
 static int launch_fold733_fullwidth(const float* tin, float* tok, void* tok_hi, void* tok_lo, int bt, int c, int h, int w,
-                                    int fh, int fw, int gelu, int out_pitch, cudaStream_t stream) {
+                                    int fh, int fw, int gelu, int out_pitch, const float* gu, float* u_out,
+                                    cudaStream_t stream) {
   constexpr int CC = 4;
   size_t smem = 0;
   const int tr = fold733_band(w, fh, 4, &smem, CC, static_cast<long long>(c / CC) * bt);
@@ -702,9 +739,12 @@ static int launch_fold733_fullwidth(const float* tin, float* tok, void* tok_hi, 
   auto* lo = static_cast<__nv_bfloat16*>(tok_lo);
   const dim3 grid(c / CC, (fh + tr - 1) / tr, bt);
   if (const int e = fold733_configure()) return e;
-  if (gelu)
+  if (gu)
+    t2t_fold733_kernel<true, false, CC, false, true><<<grid, 256, smem, stream>>>(tin, tok, hi, lo, nullptr, nullptr, 1, c, h, w,
+                                                                                  fh, fw, tr, out_pitch, nullptr, gu);
+  else if (gelu)
     t2t_fold733_kernel<true, true, CC><<<grid, 256, smem, stream>>>(tin, tok, hi, lo, nullptr, nullptr, 1, c, h, w, fh, fw, tr,
-                                                                    out_pitch);
+                                                                    out_pitch, nullptr, nullptr, u_out);
   else
     t2t_fold733_kernel<true, false, CC><<<grid, 256, smem, stream>>>(tin, tok, hi, lo, nullptr, nullptr, 1, c, h, w, fh, fw, tr,
                                                                      out_pitch);
@@ -713,12 +753,13 @@ static int launch_fold733_fullwidth(const float* tin, float* tok, void* tok_hi, 
 }
 
 int launch_t2t_fold_unfold(const float* tin, float* tok, void* tok_hi, void* tok_lo, int bt, int c, int h, int w, int k,
-                           int s, int p, int gelu, int out_pitch, cudaStream_t stream) {
+                           int s, int p, int gelu, int out_pitch, cudaStream_t stream, const float* gu, float* u_out) {
   if (k != 7 || s != 3 || p != 3 || c % MID_CC) return -2;
   const int fh = (h + 2 * p - k) / s + 1, fw = (w + 2 * p - k) / s + 1;
   if (bt == 0 || fh <= 0 || fw <= 0) return 0;
   if (bt > 65535) return -2;
-  if (fw <= 40) return launch_fold733_fullwidth(tin, tok, tok_hi, tok_lo, bt, c, h, w, fh, fw, gelu, out_pitch, stream);
+  if (fw <= 40)
+    return launch_fold733_fullwidth(tin, tok, tok_hi, tok_lo, bt, c, h, w, fh, fw, gelu, out_pitch, gu, u_out, stream);
   // tile: <= 36 token columns (x tiles evened out) and the tallest band of token rows that keeps two blocks per SM
   const int xt = (fw + 35) / 36, tw = (fw + xt - 1) / xt;
   const int wp = 3 * (tw + 4) + 4;
@@ -730,12 +771,17 @@ int launch_t2t_fold_unfold(const float* tin, float* tok, void* tok_hi, void* tok
   const size_t smem = smem_of(tr);
   if (smem > 200 * 1024 || bands > 65535) return -2;
   static DeviceOnce cfg;
-  if (const int e = configure_once(cfg, 200 * 1024, t2t_ffn_mid_kernel<true>, t2t_ffn_mid_kernel<false>)) return e;
+  if (const int e = configure_once(cfg, 200 * 1024, t2t_ffn_mid_kernel<true>, t2t_ffn_mid_kernel<false>,
+                                   t2t_ffn_mid_kernel<false, true>))
+    return e;
   auto* hi = static_cast<__nv_bfloat16*>(tok_hi);
   auto* lo = static_cast<__nv_bfloat16*>(tok_lo);
   const dim3 grid((c / MID_CC) * xt, bands, bt);
-  if (gelu)
-    t2t_ffn_mid_kernel<true><<<grid, 256, smem, stream>>>(tin, tok, hi, lo, c, h, w, fh, fw, tr, tw, xt, out_pitch);
+  if (gu)
+    t2t_ffn_mid_kernel<false, true><<<grid, 256, smem, stream>>>(tin, tok, hi, lo, c, h, w, fh, fw, tr, tw, xt, out_pitch, gu);
+  else if (gelu)
+    t2t_ffn_mid_kernel<true><<<grid, 256, smem, stream>>>(tin, tok, hi, lo, c, h, w, fh, fw, tr, tw, xt, out_pitch, nullptr,
+                                                          u_out);
   else
     t2t_ffn_mid_kernel<false><<<grid, 256, smem, stream>>>(tin, tok, hi, lo, c, h, w, fh, fw, tr, tw, xt, out_pitch);
   count_launch();

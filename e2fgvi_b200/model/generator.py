@@ -374,7 +374,7 @@ class InpaintGenerator(BaseNetwork):
         else:
             tokens = self.transformer(tokens)
         # enc_feat + trans_feat (e2fgvi.py:263) is fused into SoftComp's fold / conv epilogue
-        enc_feat = self.sc(tokens, t, fold_size if self.HQ else None, residual=enc_feat)
+        enc_feat = self.sc._forward(tokens, t, fold_size if self.HQ else None, residual=enc_feat)
 
         # tanh and the NCHW layout of the prediction are fused into the last decoder conv's epilogue
         return self._decode(enc_feat), pred_flows

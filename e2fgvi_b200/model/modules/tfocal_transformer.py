@@ -22,6 +22,17 @@ def _token_grid(output_size, kernel_size, stride, padding):
     return tuple((output_size[i] + 2 * padding[i] - (kernel_size[i] - 1) - 1) // stride[i] + 1 for i in range(2))
 
 
+def _tracked(inputs, params):
+    """Grad mode is on and a tensor input or a parameter requires grad: the call gets a ``grad_fn``."""
+    return torch.is_grad_enabled() and (any(isinstance(t, torch.Tensor) and t.requires_grad for t in inputs)
+                                        or any(p.requires_grad for p in params))
+
+
+def _second_backward(what):
+    return RuntimeError(f"{what}: the backward frees the operands it keeps, so the output cannot be backpropagated a "
+                        "second time (retain_graph=True is not supported); run the forward again")
+
+
 class SoftSplit(nn.Module):
     """unfold(7x7, s3, p3) + Linear(49*C -> hidden) (tfocal_transformer.py:19-46)."""
 
@@ -33,11 +44,49 @@ class SoftSplit(nn.Module):
         self.output_size = None if t2t_param is None else t2t_param.get("output_size")
 
     def forward(self, x, b, output_size=None):
+        """x (BT, C, H, W) fp32 (or the encoder's ``SplitNHWC``) -> tokens (b, T, fh, fw, hidden).  Trainable
+        (``_SoftSplitGrad``) when grad mode is on and the tensor x or a parameter requires grad; the tokens are the same
+        bits as the untracked call."""
         output_size = output_size or self.output_size
         f_h, f_w = _token_grid(output_size, self.kernel_size, self.stride, self.padding)
-        # unfold + Linear == a 7x7 / stride-3 conv: one implicit-GEMM launch, the 49x unfolded operand never exists
-        feat = ops.soft_split(x, self.embedding.weight, self.embedding.bias, self.kernel_size, self.stride, self.padding)
+        params = (self.embedding.weight, self.embedding.bias)
+        if isinstance(x, torch.Tensor) and _tracked([x], params):
+            feat = _SoftSplitGrad.apply(self, x, *params)
+        else:
+            # unfold + Linear == a 7x7 / stride-3 conv: one implicit-GEMM launch, the 49x unfolded operand never exists
+            feat = ops.soft_split(x, *params, self.kernel_size, self.stride, self.padding)
         return feat.view(b, -1, f_h, f_w, feat.size(2))
+
+
+class _SoftSplitGrad(torch.autograd.Function):
+    """``SoftSplit``'s launch with a backward into ``embedding`` and x: dW = dT^T . unfold(x) (the unfold materialised as
+    a split operand), db = the sum of dT, dx = fold(dT . W) on ``soft_comp``'s transposed-conv launch with W^T."""
+
+    @staticmethod
+    def forward(ctx, mod, x, weight, bias):
+        ctx.mod, ctx.live = mod, True
+        ctx.save_for_backward(x, weight, bias)
+        return ops.soft_split(x, weight, bias, mod.kernel_size, mod.stride, mod.padding)
+
+    @staticmethod
+    def backward(ctx, grad):
+        if not ctx.live:
+            raise _second_backward("SoftSplit")
+        x, weight, bias = ctx.saved_tensors
+        ctx.live = False
+        mod = ctx.mod
+        n, c, h, w = x.shape
+        _, need_x, need_w, need_b = ctx.needs_input_grad
+        dx = dw = db = None
+        if need_w or need_b:
+            cols = ops.t2t_unfold(x, mod.kernel_size, mod.stride, mod.padding, out="split")
+            dw, db = ops.linear_wgrad(grad, cols, with_bias=need_b)
+            dw = dw if need_w else None
+        if need_x:
+            fh, fw = _token_grid((h, w), mod.kernel_size, mod.stride, mod.padding)
+            dx = ops.soft_comp(grad.reshape(n, fh, fw, -1), weight, None, (h, w), mod.kernel_size, mod.stride,
+                               mod.padding, transpose=True)
+        return None, dx, dw, db
 
 
 class SoftComp(nn.Module):
@@ -54,20 +103,86 @@ class SoftComp(nn.Module):
         else:
             self.bias = nn.Parameter(torch.zeros((channel, output_size[0], output_size[1]), dtype=torch.float32))
 
+    def params(self):
+        """The parameters in ``_SoftCompGrad``'s order: embedding weight and bias, then the bias map (base) or
+        bias_conv's weight and bias (HQ)."""
+        tail = (self.bias_conv.weight, self.bias_conv.bias) if self.hq else (self.bias,)
+        return (self.embedding.weight, self.embedding.bias) + tail
+
     def forward(self, x, t, output_size=None, residual=None):
         """``residual`` (b*t, C, H, W), optional: added to the result by the fold kernel (base model) or the conv
-        epilogue (HQ) — the ``enc_feat + trans_feat`` of e2fgvi.py:263; the result is then channels_last."""
+        epilogue (HQ) — the ``enc_feat + trans_feat`` of e2fgvi.py:263; the result is then channels_last.  Trainable
+        (``_SoftCompGrad``) when grad mode is on and x, the residual or a parameter requires grad; the result is the
+        same bits as the untracked call."""
+        output_size = tuple(output_size or self.output_size)
+        if isinstance(x, torch.Tensor) and _tracked([x, residual], self.params()):
+            return _SoftCompGrad.apply(self, x, residual, output_size, *self.params())
+        return self._forward(x, t, output_size, residual)
+
+    def _forward(self, x, t, output_size=None, residual=None, keep=None):
+        """The launch sequence of ``forward`` (untracked); ``keep`` (a dict or None) receives the split tokens and, HQ,
+        the split operand of bias_conv."""
         output_size = output_size or self.output_size
         b_, t_, f_h, f_w, c_ = x.shape
         # Linear + fold == the transposed 7x7 / stride-3 conv: one implicit-GEMM launch over nine output phases; the
         # 6272-wide token matrix and the fold pass never exist
         tokens = x.view(b_ * t_, f_h, f_w, c_)
+        if keep is not None:
+            tokens = keep["tokens"] = ops.SplitMat(*ops.split_bf16(tokens))
         if self.hq:
             feat = ops.soft_comp(tokens, self.embedding.weight, self.embedding.bias, output_size, self.kernel_size,
                                  self.stride, self.padding, out="split")
+            if keep is not None:
+                keep["feat"] = feat
             return ops.conv3x3([feat], self.bias_conv.weight, self.bias_conv.bias, residual=residual)
         return ops.soft_comp(tokens, self.embedding.weight, self.embedding.bias, output_size, self.kernel_size,
                              self.stride, self.padding, bias_map_extra=self.bias, residual=residual)
+
+
+class _SoftCompGrad(torch.autograd.Function):
+    """``SoftComp``'s launches with a backward into its parameters, the tokens and the residual.  With dfeat = the
+    gradient of the folded features (HQ: bias_conv's input gradient on ``conv_dgrad``, its weight gradient on
+    ``conv3x3_wgrad``): the base bias map gets the sum of dfeat over BT, the embedding dW = unfold(dfeat)^T . tokens
+    and db = the sum of unfold(dfeat), the tokens unfold(dfeat) . W on ``soft_split``'s launch with W^T; the residual
+    receives the gradient unchanged."""
+
+    @staticmethod
+    def forward(ctx, mod, tokens, residual, output_size, *params):
+        keep = {}
+        out = mod._forward(tokens, tokens.shape[1], output_size, residual, keep)
+        ctx.mod, ctx.keep, ctx.output_size, ctx.shape = mod, keep, output_size, tokens.shape
+        ctx.save_for_backward(*params)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        if ctx.keep is None:
+            raise _second_backward("SoftComp")
+        params = ctx.saved_tensors
+        mod, keep = ctx.mod, ctx.keep
+        ctx.keep = None
+        need_tok, need_res = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+        needs = ctx.needs_input_grad[4:]
+        grads = [None] * len(params)
+        k, s, p = mod.kernel_size, mod.stride, mod.padding
+        dfeat = grad
+        if mod.hq:
+            if needs[2] or needs[3]:
+                dw, db = ops.conv3x3_wgrad(grad.permute(0, 2, 3, 1), [keep["feat"]], with_bias=needs[3])
+                grads[2], grads[3] = (dw if needs[2] else None), db
+            dfeat = None
+            if need_tok or needs[0] or needs[1]:
+                dfeat = ops.conv_dgrad(ops.split_nhwc(grad), params[2]).permute(0, 3, 1, 2)
+        elif needs[2]:
+            grads[2] = grad.sum(0)
+        if needs[0] or needs[1]:
+            cols = ops.t2t_unfold(dfeat, k, s, p, out="split")
+            dw, db = ops.linear_wgrad(cols, keep["tokens"], with_bias=needs[1])
+            grads[0], grads[1] = (dw if needs[0] else None), db
+        dtok = None
+        if need_tok:
+            dtok = ops.soft_split(dfeat, params[0], None, k, s, p, transpose=True).reshape(ctx.shape)
+        return (None, dtok, grad if need_res else None, None) + tuple(grads)
 
 
 class FusionFeedForward(nn.Module):
@@ -85,7 +200,13 @@ class FusionFeedForward(nn.Module):
 
     def forward(self, x, output_size=None, residual=None):
         """conv1 -> [fold / fold(ones) -> unfold -> GELU] (one fused kernel on the token-major layout) -> conv2
-        (+ residual, fused into the GEMM epilogue)."""
+        (+ residual, fused into the GEMM epilogue).  Trainable (``_FusionFeedForwardGrad``) when grad mode is on, x is
+        an fp32 tensor (B, N, 512) and x, the residual or a Linear's parameter requires grad; the output is the same
+        bits as the untracked call."""
+        params = (self.conv1[0].weight, self.conv1[0].bias, self.conv2[1].weight, self.conv2[1].bias)
+        if isinstance(x, torch.Tensor) and _tracked([x, residual], params):
+            p = self.t2t_params
+            return _FusionFeedForwardGrad.apply(self, x, residual, tuple(output_size or p.get("output_size")), *params)
         p = self.t2t_params
         output_size = output_size or p.get("output_size")
         f_h, f_w = _token_grid(output_size, p["kernel_size"], p["stride"], p["padding"])
@@ -98,6 +219,60 @@ class FusionFeedForward(nn.Module):
                                 gelu=True, out="split", pitch=(c + 63) // 64 * 64)
         x = x.view(b, n, x.shape[-1])
         return ops.linear(x, self.conv2[1].weight, self.conv2[1].bias, residual=residual)
+
+    def geometry(self, output_size):
+        p = self.t2t_params
+        return output_size, p["kernel_size"], p["stride"], p["padding"]
+
+
+class _FusionFeedForwardGrad(torch.autograd.Function):
+    """``FusionFeedForward``'s launches with a backward into both Linears, x and the residual.  The forward splits x
+    once (conv1's operand, kept for its weight gradient) and runs the fold/normalise/unfold kernel in its training mode,
+    which also keeps u, the normalised values before GELU.  Backward, with g = the output's gradient:
+      dz = g . W2 (``linear`` with W2^T), dW2 = g^T . GELU(u) (the kept split operand), db2 = sum g;
+      dh = U D F (dz * GELU'(u)) (the same kernel's adjoint mode, written as a split operand with the 1984 pitch);
+      dx = dh . W1 (``linear`` with W1^T, padded alike), dW1 = dh^T . x, db1 = sum dh; the residual receives g."""
+
+    @staticmethod
+    def forward(ctx, mod, x, residual, output_size, w1, b1, w2, b2):
+        geo = mod.geometry(output_size)
+        b, n, _ = x.shape
+        xs = ops.SplitMat(*ops.split_bf16(x.reshape(-1, x.shape[-1])))
+        h = ops.linear(xs, w1, b1)
+        hd = h.shape[-1]
+        f_h, f_w = _token_grid(*geo)
+        z, u = ops.t2t_fold_unfold_train(h.view(-1, f_h * f_w, hd), *geo, out="split", pitch=(hd + 63) // 64 * 64)
+        out = ops.linear(z.view(b * n, z.shape[-1]), w2, b2, residual=residual)
+        ctx.mod, ctx.geo, ctx.keep, ctx.shape = mod, geo, {"x": xs, "u": u, "z": z}, x.shape
+        ctx.save_for_backward(w1, w2)
+        return out.view(b, n, -1)
+
+    @staticmethod
+    def backward(ctx, grad):
+        if ctx.keep is None:
+            raise _second_backward("FusionFeedForward")
+        w1, w2 = ctx.saved_tensors
+        keep = ctx.keep
+        ctx.keep = None
+        need_x, need_res = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+        nw1, nb1, nw2, nb2 = ctx.needs_input_grad[4:]
+        z, u = keep["z"], keep["u"]
+        hd = w1.shape[0]
+        g = ops.SplitMat(*ops.split_bf16(grad.reshape(-1, grad.shape[-1])))
+        dw1 = db1 = dw2 = db2 = dx = None
+        if nw2 or nb2:
+            dw2, db2 = ops.linear_wgrad(g, z.view(-1, z.shape[-1]), with_bias=nb2, shape=tuple(w2.shape))
+            dw2 = dw2 if nw2 else None
+        if need_x or nw1 or nb1:
+            dz = ops.linear(g, w2, transpose=True)
+            dh = ops.t2t_fold_unfold_train(dz.view(u.shape), *ctx.geo, u=u, out="split", pitch=z.shape[-1])
+            dh = dh.view(-1, dh.shape[-1])
+            if nw1 or nb1:
+                dw1, db1 = ops.linear_wgrad(dh, keep["x"], with_bias=nb1, shape=tuple(w1.shape))
+                dw1 = dw1 if nw1 else None
+            if need_x:
+                dx = ops.linear(dh, w1, transpose=True).view(ctx.shape)
+        return None, dx, grad if need_res else None, None, dw1, db1, dw2, db2
 
 
 def window_partition(x, window_size):

@@ -401,6 +401,40 @@ def t2t_fold_unfold(tokens, output_size, kernel_size, stride, padding, gelu=Fals
     return tok if out == "f32" else SplitMat(hi, lo)
 
 
+def t2t_fold_unfold_train(tokens, output_size, kernel_size, stride, padding, u=None, out="split", pitch=None):
+    """The training modes of ``t2t_fold_unfold`` with GELU (``e2f_t2t_fold_unfold_train``), 7/3/3 only.
+
+    ``u=None``: the forward, returns ``(GELU(u), u)`` with u = unfold(fold(tokens) / fold(ones)) fp32 (BT, L, C*k*k) —
+    the first the same bits as ``t2t_fold_unfold(gelu=True)``.  ``u`` given (the forward's): the input gradient of that
+    forward at dz = ``tokens``, unfold(fold(dz * GELU'(u)) / fold(ones)).  Outputs as ``t2t_fold_unfold``."""
+    k, s, p = _square(kernel_size, stride, padding)
+    if (k, s, p) != (7, 3, 3):
+        raise NotImplementedError("t2t_fold_unfold_train: the 7/3/3 geometry only (the fused kernel)")
+    _need_cuda(tokens, u)
+    h, w = output_size
+    tokens = tokens.contiguous().float()
+    bt, n_tok, ck = tokens.shape
+    c = ck // 49
+    fh, fw = (h - 1) // 3 + 1, (w - 1) // 3 + 1
+    if n_tok != fh * fw or c * 49 != ck:
+        raise ValueError(f"t2t_fold_unfold_train: tokens {tuple(tokens.shape)} do not match output_size {output_size}")
+    backward = u is not None
+    if backward and tuple(u.shape) != tuple(tokens.shape):
+        raise ValueError(f"t2t_fold_unfold_train: u {tuple(u.shape)} != tokens {tuple(tokens.shape)}")
+    u = torch.empty_like(tokens) if u is None else u.contiguous()
+    pitch = ck if pitch is None else int(pitch)
+    tok, hi, lo = _outputs(out, ("f32", "split"), (bt, n_tok, pitch), tokens.device)
+    name = "t2t_fold_unfold_adjoint" if backward else "t2t_fold_unfold"
+    with _timed(name, float(tokens.numel() * (12 if backward else 8))):
+        st = _lib.load().e2f_t2t_fold_unfold_train(tokens.data_ptr(), u.data_ptr(), None if tok is None else tok.data_ptr(),
+                                                   None if hi is None else hi.data_ptr(),
+                                                   None if lo is None else lo.data_ptr(), bt, c, h, w, k, s, p,
+                                                   1 if backward else 0, pitch, _stream())
+    _lib.check(st, "e2f_t2t_fold_unfold_train")
+    res = tok if out == "f32" else SplitMat(hi, lo)
+    return res if backward else (res, u)
+
+
 def window_pool(x, weight, bias, window_size, out="split"):
     """pool_layers[0] (``nn.Linear(wh*ww, 1)`` across the tokens of each window, per channel; tfocal_transformer.py:
     508-516) in one kernel.  x: the split LayerNorm output as a ``SplitMat`` of shape (B,T,H,W,C); weight (1, wh*ww);
@@ -576,21 +610,34 @@ def _derived(params, tag, build):
     return hit[2]
 
 
-def _padded_split(weight, k):
+def transposed_linear_weight(weight, k):
+    """fp32 W^T of an (N, K) Linear weight as (K, k), k >= N: zero columns appended to match an operand whose rows are
+    padded to k — the weight operand of the input gradient dY . W."""
+    wt = weight.detach().reshape(weight.shape[0], -1).float().t()
+    return torch.nn.functional.pad(wt, (0, k - wt.shape[1])) if k > wt.shape[1] else wt.contiguous()
+
+
+def _padded_split(weight, k, transpose=False):
     """bf16 (hi, lo) split of an (N, K) or (N, K, 1, 1) weight as (N, k), k >= K: zero columns appended to match an
-    operand whose rows are padded to k."""
+    operand whose rows are padded to k.  ``transpose``: of ``transposed_linear_weight(weight, k)`` instead."""
+    if transpose:
+        return split_bf16(transposed_linear_weight(weight, k))
     w2 = weight.detach().reshape(weight.shape[0], -1)
     if k > w2.shape[1]:
         w2 = torch.nn.functional.pad(w2.float(), (0, k - w2.shape[1]))
     return split_bf16(w2)
 
 
-def linear(x, weight, bias=None, residual=None, out_dtype=torch.float32, tile_hint=0):
+def linear(x, weight, bias=None, residual=None, out_dtype=torch.float32, tile_hint=0, transpose=False):
     """``F.linear(x, weight, bias) (+ residual)`` on the bf16 tensor pipe with a 3-term split (fp32-level accuracy).
 
     x (..., K) fp32, weight (N, K) fp32 nn.Parameter (its bf16 split is cached per parameter object and refreshed
-    when the parameter changes), bias (N,), residual (..., N) fp32 -> (..., N) ``out_dtype``."""
+    when the parameter changes), bias (N,), residual (..., N) fp32 -> (..., N) ``out_dtype``.
+    ``transpose=True``: ``x . weight`` instead, x (..., N) -> (..., K) (the input gradient of the Linear; W^T's split is
+    cached under its own tag)."""
     n, k = weight.shape[:2]            # (N, K) Linear weight or (N, K, 1, 1) 1x1-conv weight
+    if transpose:
+        n, k = k, n
     lead = x.shape[:-1]
     k_pad = 0
     if isinstance(x, SplitMat):         # operand pair written by a fused producer
@@ -606,7 +653,7 @@ def linear(x, weight, bias=None, residual=None, out_dtype=torch.float32, tile_hi
         x2 = x.reshape(-1, k)
         m = x2.shape[0]
         a_hi, a_lo = split_bf16(x2)
-    w_hi, w_lo = _derived_one(weight, ("split", k_pad), _padded_split, k)
+    w_hi, w_lo = _derived_one(weight, ("split_t" if transpose else "split", k_pad), _padded_split, k, transpose)
     b32 = None if bias is None else bias.detach().float().contiguous()
     res = None
     if residual is not None:
@@ -619,6 +666,44 @@ def linear(x, weight, bias=None, residual=None, out_dtype=torch.float32, tile_hi
                                            _DT[out_dtype], tile_hint, _stream())
     _lib.check(st, "e2f_linear_bf16x3")
     return out.view(*lead, n)
+
+
+def linear_wgrad(dy, x, with_bias=True, shape=None):
+    """(dW fp32 (N, K), db fp32 (N,) or None) of a Linear: dW = dY^T . X, db = the sum of dY over rows
+    (``e2f_linear_wgrad_bf16x3``).  dy (..., N) and x (..., K): fp32 tensors or ``SplitMat`` operands (rows may be padded
+    with zero columns, e.g. ``t2t_fold_unfold``'s pitch); ``shape`` = the parameter's (N, K) when they are padded."""
+    ops_ = []
+    for t in (dy, x):
+        if isinstance(t, SplitMat):
+            _need_cuda(t.hi)
+            w = t.shape[-1]
+            ops_.append((t.hi.reshape(-1, w), t.lo.reshape(-1, w)))
+        else:
+            _need_cuda(t)
+            w = t.shape[-1]
+            if w % 8:
+                t = torch.nn.functional.pad(t.float(), (0, 8 - w % 8))
+            ops_.append(split_bf16(t.reshape(-1, t.shape[-1])))
+    (dy_hi, dy_lo), (x_hi, x_lo) = ops_
+    m, ldy, ldx = dy_hi.shape[0], dy_hi.shape[1], x_hi.shape[1]
+    if x_hi.shape[0] != m:
+        raise ValueError(f"linear_wgrad: dy has {m} rows, x {x_hi.shape[0]}")
+    n, k = shape if shape is not None else (dy.shape[-1], x.shape[-1])
+    if n > ldy or k > ldx:
+        raise ValueError(f"linear_wgrad: shape {(n, k)} exceeds the operands' widths {(ldy, ldx)}")
+    lib = _lib.load()
+    elems = int(lib.e2f_linear_wgrad_work_elems(m, n, k))
+    if elems < 0:
+        _lib.check(elems, "e2f_linear_wgrad_work_elems")
+    work = torch.empty(elems, dtype=torch.float32, device=dy_hi.device) if elems else None
+    dw = torch.empty((n, k), dtype=torch.float32, device=dy_hi.device)
+    db = torch.empty(n, dtype=torch.float32, device=dy_hi.device) if with_bias else None
+    with _timed("linear_wgrad_bf16x3", 2.0 * m * n * k):
+        st = lib.e2f_linear_wgrad_bf16x3(dy_hi.data_ptr(), dy_lo.data_ptr(), ldy, x_hi.data_ptr(), x_lo.data_ptr(), ldx,
+                                         dw.data_ptr(), None if db is None else db.data_ptr(),
+                                         None if work is None else work.data_ptr(), m, n, k, _stream())
+    _lib.check(st, "e2f_linear_wgrad_bf16x3")
+    return dw, db
 
 
 class SplitNHWC:
@@ -935,7 +1020,16 @@ def conv_frames(sources, weight, bias=None, negative_slope=1.0, residual=None, o
                         2.0 * n * h * w * cout * weight.shape[1] * ks * ks, slope=negative_slope, into=into)
 
 
-def soft_split(x, weight, bias, kernel_size, stride, padding):
+def soft_split_weight(weight, c, k, transpose=False):
+    """The conv weight (hidden, c, k, k) that ``soft_split`` runs: the Linear weight (hidden, c*k*k) viewed as a conv,
+    or with ``transpose`` that of W^T for a (c*k*k, hidden) weight — SoftComp's token gradient unfold(dfeat) . W_sc."""
+    w = weight.detach().float()
+    if transpose:
+        w = w.t()
+    return w.reshape(w.shape[0], c, k, k)
+
+
+def soft_split(x, weight, bias, kernel_size, stride, padding, transpose=False):
     """SoftSplit.forward (tfocal_transformer.py:39-46): ``Linear(unfold(x, k, s, p))`` evaluated as the k x k / stride-s
     convolution it is — an implicit GEMM whose A operand is fetched by TMA straight from the NHWC feature map; the
     k*k-times larger unfolded token matrix is never built.
@@ -945,13 +1039,13 @@ def soft_split(x, weight, bias, kernel_size, stride, padding):
     k, s, p = _square(kernel_size, stride, padding)
     src = split_nhwc(x)
     n, c, h, w = src.shape
-    hidden = weight.shape[0]
-    if weight.shape[1] != c * k * k or k * k > 64 or c % 8:
+    hidden, ck = (weight.shape[1], weight.shape[0]) if transpose else tuple(weight.shape)
+    if ck != c * k * k or k * k > 64 or c % 8:
         raise ValueError(f"soft_split: weight {tuple(weight.shape)} does not match C={c}, k={k}")
     _need_cuda(weight, bias)
     fh, fw = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
-    w_hi, w_lo = _derived_one(weight, ("soft_split", c, k),
-                              lambda wt: pack_conv3x3_weight(wt.detach().view(hidden, c, k, k), [c], 1))
+    w_hi, w_lo = _derived_one(weight, ("soft_split_t" if transpose else "soft_split", c, k),
+                              lambda wt: pack_conv3x3_weight(soft_split_weight(wt, c, k, transpose), [c], 1))
     taps = [(ky - p, kx - p) for ky in range(k) for kx in range(k)]
     tok = _conv_gather([src], w_hi, w_lo, bias, None, None, "f32", hidden, s, (fh, fw), taps, [(0, 0, 0)], 1,
                        (fh, fw), 2.0 * n * fh * fw * hidden * c * k * k)
@@ -976,8 +1070,22 @@ def _soft_comp_tables(k, s, p):
     return taps, phases, kpos
 
 
+def soft_comp_weight(weight, k, s, p, transpose=False):
+    """fp32 (C, k*k*hidden) operand of ``soft_comp``: the Linear weight (C*k*k, hidden) with its kernel positions in the
+    phase tap order of ``_soft_comp_tables``, or with ``transpose`` that of W^T for a (hidden, C*k*k) weight — SoftSplit's
+    input gradient fold(dT . W_ss)."""
+    w = weight.detach().float()
+    if transpose:
+        w = w.t()
+    hidden = w.shape[1]
+    c = w.shape[0] // (k * k)
+    _, _, kpos = _soft_comp_tables(k, s, p)
+    order = torch.tensor([ky * k + kx for ky, kx in kpos], device=w.device)
+    return w.reshape(c, k * k, hidden)[:, order, :].reshape(c, k * k * hidden)
+
+
 def soft_comp(tokens, weight, bias, output_size, kernel_size, stride, padding, bias_map_extra=None, residual=None,
-              out="f32"):
+              out="f32", transpose=False):
     """SoftComp.forward up to (and including) the fold (tfocal_transformer.py:65-72, _hq.py:67-79):
     ``fold(Linear(tokens))`` evaluated as the transposed convolution it is, one implicit-GEMM launch over the nine
     output phases; the (C*k*k)-wide token matrix and the fold pass never exist.
@@ -989,15 +1097,15 @@ def soft_comp(tokens, weight, bias, output_size, kernel_size, stride, padding, b
     k, s, p = _square(kernel_size, stride, padding)
     h, w = output_size
     fh, fw = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
-    hidden = weight.shape[1]
-    c = weight.shape[0] // (k * k)
+    hidden, ck = (weight.shape[0], weight.shape[1]) if transpose else (weight.shape[1], weight.shape[0])
+    c = ck // (k * k)
     if isinstance(tokens, SplitMat):
         hi, lo = tokens.hi, tokens.lo
     else:
         _need_cuda(tokens)
         hi, lo = split_bf16(tokens)
     n = hi.numel() // (fh * fw * hidden)
-    if hi.numel() != n * fh * fw * hidden or hidden % 64 or c * k * k != weight.shape[0]:
+    if hi.numel() != n * fh * fw * hidden or hidden % 64 or c * k * k != ck:
         raise ValueError(f"soft_comp: tokens {tuple(hi.shape)} / weight {tuple(weight.shape)} do not match output_size "
                          f"{output_size}")
     _need_cuda(weight, bias, bias_map_extra, residual)
@@ -1006,12 +1114,8 @@ def soft_comp(tokens, weight, bias, output_size, kernel_size, stride, padding, b
     taps, phases, kpos = _soft_comp_tables(k, s, p)
     src = SplitNHWC(hi.view(n, fh, fw, hidden), lo.view(n, fh, fw, hidden), (n, hidden, fh, fw))
 
-    def pack(weight):
-        order = torch.tensor([ky * k + kx for ky, kx in kpos], device=weight.device)
-        wp = weight.detach().float().view(c, k * k, hidden)[:, order, :].reshape(c, k * k * hidden)
-        return split_bf16(wp)
-
-    w_hi, w_lo = _derived_one(weight, ("soft_comp", k, s), pack)
+    w_hi, w_lo = _derived_one(weight, ("soft_comp_t" if transpose else "soft_comp", k, s),
+                              lambda wt: split_bf16(soft_comp_weight(wt, k, s, p, transpose)))
 
     def fold_bias():
         # fold of the Linear bias: every pixel receives b[c, ky, kx] from each token patch that covers it (border

@@ -146,6 +146,16 @@ int e2f_t2t_unfold_nhwc(const float* img_nhwc, float* tokens, void* tokens_hi, v
 int e2f_t2t_fold_unfold(const float* tokens_in, float* tokens, void* tokens_hi, void* tokens_lo, int bt, int c, int h,
                         int w, int k, int stride, int pad, int gelu, int out_pitch, void* stream);
 
+/* Training modes of e2f_t2t_fold_unfold with GELU (k=7, stride=3, pad=3, C % 4 == 0; E2F_ERR_UNSUPPORTED otherwise):
+ *   backward = 0: the forward, out = GELU(u) with u = unfold(fold(tokens_in) / fold(ones)); u is also written, fp32
+ *       [BT][L][C*k*k] with dense rows, for the backward;
+ *   backward = 1: the input gradient of that forward, out = unfold(fold(g) / fold(ones)) with g = tokens_in * GELU'(u)
+ *       (the operator unfold . / fold(ones) . fold is self-adjoint), tokens_in = dz and u = the forward's u, both fp32
+ *       [BT][L][C*k*k]; GELU'(u) = Phi(u) + u phi(u) of the exact (erf) GELU.
+ * Outputs and out_pitch as e2f_t2t_fold_unfold; the forward's outputs are the same bits as e2f_t2t_fold_unfold's. */
+int e2f_t2t_fold_unfold_train(const float* tokens_in, float* u, float* tokens, void* tokens_hi, void* tokens_lo, int bt, int c,
+                              int h, int w, int k, int stride, int pad, int backward, int out_pitch, void* stream);
+
 /* Window pooling of the focal attention's coarse level: pool_layers[0] = nn.Linear(wh*ww, 1) across the tokens of
  * every window, per channel (tfocal_transformer.py:508-516, the permute/Linear/squeeze chain):
  *   out[bt][wi][wj][c] = bias[0] + sum_{r<wh, q<ww} x[bt][wi*wh + r][wj*ww + q][c] * weight[r*ww + q]
@@ -190,6 +200,17 @@ int e2f_split_bf16(const float* x, void* hi_bf16, void* lo_bf16, int64_t n, void
 int e2f_linear_bf16x3(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, const float* bias,
                       const float* residual, void* out, int m, int n, int k, int out_dtype, int tile_hint,
                       void* stream);
+
+/* Weight and bias gradient of a Linear (e2f_linear_bf16x3): dw [n][k] fp32 = dY^T . X and, if db is not NULL, db [n]
+ * fp32 = the sum of dY over its m rows, from dY = (dy_hi, dy_lo) bf16 [m][ldy] and X = (x_hi, x_lo) bf16 [m][ldx]
+ * (e2f_split_bf16 pairs).  Columns past n / k are not read, so operands whose rows are padded with zero columns (the
+ * out_pitch of e2f_t2t_fold_unfold) are accepted; ldy and ldx are multiples of 8.  bf16 three-term split with fp32
+ * accumulation, split over m into slices (a function of the shape alone) whose partial sums are added in a fixed order:
+ * bit-identical from run to run.  `work` holds e2f_linear_wgrad_work_elems(m, n, k) floats (NULL allowed when that is 0;
+ * negative = bad arguments). */
+int64_t e2f_linear_wgrad_work_elems(int m, int n, int k);
+int e2f_linear_wgrad_bf16x3(const void* dy_hi, const void* dy_lo, int ldy, const void* x_hi, const void* x_lo, int ldx, float* dw,
+                            float* db, float* work, int m, int n, int k, void* stream);
 
 /* 3x3 / stride 1 / pad 1 convolution (nn.Conv2d at e2fgvi.py:75-94,143-150; feat_prop.py:20-28,73-77) as a wgmma
  * implicit GEMM with fp32-level accuracy (bf16 3-term split, like e2f_linear_bf16x3):
