@@ -23,6 +23,9 @@ SIGNATURES = {
     "e2f_deform_align_fused": (_i, [_vp, _fp, _fp, _fp, _vp, _fp, _vp, _i, _i, _i, _i, _i, _i, _f, _i, _i, _vp]),
     "e2f_deform_align_fused_split": (_i, [_vp, _fp, _fp, _fp, _vp, _fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _i, _vp]),
     "e2f_focal_window_attention": (_i, [_vp, _vp, _vp] + [_i] * 13 + [_f, _i, _vp]),
+    "e2f_focal_window_attention_backward_work_elems": (_c.c_int64, [_i] * 13),
+    "e2f_focal_window_attention_backward": (_i, [_vp, _vp, _fp, _fp, _fp, _fp] + [_i] * 13 + [_f, _vp]),
+    "e2f_focal_window_attention_key_sources": (_i, [_i] * 14 + [_c.POINTER(_i)] * 3 + [_i]),
     "e2f_t2t_unfold": (_i, [_fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "e2f_upsample2x_split": (_i, [_fp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "e2f_layernorm_split": (_i, [_fp, _fp, _fp, _fp, _vp, _vp, _c.c_int64, _i, _f, _vp]),

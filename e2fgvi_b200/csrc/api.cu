@@ -173,6 +173,46 @@ int e2f_focal_window_attention(const void* qkv, const void* qkv_pooled, void* ou
                 "e2f_focal_window_attention");
 }
 
+static int focal_grad_geometry_checks(const char* who, int b, int t, int h, int w, int heads, int head_dim, int wh,
+                                      int ww, int eh, int ew, int fh, int fw, int use_pooled) {
+  if (b < 0 || t <= 0 || h <= 0 || w <= 0 || heads <= 0 || wh <= 0 || ww <= 0 || eh < 0 || ew < 0) { set_error("%s: bad shape", who); return E2F_ERR_BAD_ARG; }
+  if (h % wh || w % ww) { set_error("%s: token grid %dx%d is not a multiple of the window %dx%d", who, h, w, wh, ww); return E2F_ERR_BAD_ARG; }
+  if (use_pooled != 0 && use_pooled != 1) { set_error("%s: use_pooled %d", who, use_pooled); return E2F_ERR_BAD_ARG; }
+  if (use_pooled && (fh <= 0 || fw <= 0 || !(fh & 1) || !(fw & 1))) { set_error("%s: pooled neighbourhood %dx%d must be odd", who, fh, fw); return E2F_ERR_BAD_ARG; }
+  if (head_dim != 128) { set_error("%s: head_dim %d unsupported (128 only)", who, head_dim); return E2F_ERR_UNSUPPORTED; }
+  return 0;
+}
+
+int64_t e2f_focal_window_attention_backward_work_elems(int b, int t, int h, int w, int heads, int head_dim, int wh,
+                                                       int ww, int eh, int ew, int fh, int fw, int use_pooled) {
+  const char* who = "e2f_focal_window_attention_backward_work_elems";
+  if (const int st = focal_grad_geometry_checks(who, b, t, h, w, heads, head_dim, wh, ww, eh, ew, fh, fw, use_pooled)) return st;
+  return static_cast<int64_t>(focal_attention_backward_work_elems(b, t, h, w, heads, wh, ww, eh, ew, fh, fw, use_pooled));
+}
+
+int e2f_focal_window_attention_key_sources(int t_count, int h, int w, int wh, int ww, int eh, int ew, int fh, int fw,
+                                           int use_pooled, int t, int pooled, int y, int x, int* win, int* slot,
+                                           int* mult, int cap) {
+  const char* who = "e2f_focal_window_attention_key_sources";
+  if (const int st = focal_grad_geometry_checks(who, 1, t_count, h, w, 1, 128, wh, ww, eh, ew, fh, fw, use_pooled)) return st;
+  if (!win || !slot || !mult || cap <= 0) { set_error("%s: null pointer or cap %d", who, cap); return E2F_ERR_BAD_ARG; }
+  if (t < 0 || t >= t_count || (pooled && !use_pooled) || y < 0 || x < 0 || y >= (pooled ? h / wh : h) || x >= (pooled ? w / ww : w)) { set_error("%s: key token (%d, %d, %d) outside the grid", who, t, y, x); return E2F_ERR_BAD_ARG; }
+  return focal_attention_key_sources(t_count, h, w, wh, ww, eh, ew, fh, fw, use_pooled, t, pooled, y, x, win, slot, mult, cap);
+}
+
+int e2f_focal_window_attention_backward(const void* qkv, const void* qkv_pooled, const float* dout, float* dqkv,
+                                        float* dqkv_pooled, float* work, int b, int t, int h, int w, int heads,
+                                        int head_dim, int wh, int ww, int eh, int ew, int fh, int fw, int use_pooled,
+                                        float scale, void* stream) {
+  const char* who = "e2f_focal_window_attention_backward";
+  if (!qkv || !dout || !dqkv || !work || (use_pooled && (!qkv_pooled || !dqkv_pooled))) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if (const int st = focal_grad_geometry_checks(who, b, t, h, w, heads, head_dim, wh, ww, eh, ew, fh, fw, use_pooled)) return st;
+  if (!(scale > 0.f)) { set_error("%s: scale must be positive", who); return E2F_ERR_BAD_ARG; }
+  if (!aligned(qkv, 16) || !aligned(dout, 16) || !aligned(dqkv, 16) || !aligned(work, 16) || (use_pooled && (!aligned(qkv_pooled, 16) || !aligned(dqkv_pooled, 16)))) { set_error("%s: 16-byte alignment required", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_focal_attention_backward(qkv, qkv_pooled, dout, dqkv, dqkv_pooled, work, b, t, h, w, heads, wh, ww,
+                                                eh, ew, fh, fw, use_pooled, scale, static_cast<cudaStream_t>(stream)), who);
+}
+
 int e2f_dcn_pack_input(const float* a, const float* b, void* xg, int n, int h, int w, int ca, int cb, void* stream) {
   if (!a || !b || !xg) { set_error("e2f_dcn_pack_input: null pointer"); return E2F_ERR_BAD_ARG; }
   if (n < 0 || h <= 0 || w <= 0 || ca <= 0 || cb <= 0 || ca % 16 || cb % 16) { set_error("e2f_dcn_pack_input: bad shape (channels must be multiples of 16)"); return E2F_ERR_BAD_ARG; }

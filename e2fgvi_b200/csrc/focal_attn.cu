@@ -24,6 +24,7 @@
 #include <type_traits>
 #include <cuda_bf16.h>
 #include "common.cuh"
+#include "focal_geom.cuh"
 #include "launch.h"
 
 namespace e2f {
@@ -42,7 +43,6 @@ constexpr int SOFTMAX_THREADS = SOFTMAX_WARPS * 32;
 constexpr int THREADS = (SOFTMAX_WARPS + LOADER_WARPS) * 32;   // 384
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr float RESCALE_THRESHOLD = 8.0f;      // log2 domain: P stays <= 2^8
-constexpr int MAX_RING = 256;                  // expanded-window positions (153 for the 5x9 window)
 constexpr int MAX_FRAME_KEYS = 384;            // ring + pooled keys of one frame (198 for 5x9 / 5x9)
 
 struct Smem {
@@ -73,29 +73,6 @@ struct Params {
   uint8_t ring_pos[MAX_RING];     // positions (er*EW + ec): the n1 single ones first, then the n2 multiple ones
   uint8_t ring_mult[MAX_RING];    // multiplicity of each entry
 };
-
-// how many times the reference lists expanded-window position (er, ec) as a key (tfocal_transformer.py:166-179,235-280)
-__host__ __device__ inline int key_multiplicity(int er, int ec, int wh, int ww, int eh, int ew) {
-  int m = 0;
-  if (er >= eh && er < eh + wh && ec >= ew && ec < ew + ww) m += 1;                      // own window
-  {  // tl: window pos (r,c) holds token (r+eh, c+ew) -> expanded (r+2eh, c+2ew); kept if r>=wh-eh or c>=ww-ew
-    const int r = er - 2 * eh, c = ec - 2 * ew;
-    if (r >= 0 && r < wh && c >= 0 && c < ww && (r >= wh - eh || c >= ww - ew)) m += 1;
-  }
-  {  // tr: expanded (r+2eh, c); kept if r>=wh-eh or c<ew
-    const int r = er - 2 * eh, c = ec;
-    if (r >= 0 && r < wh && c >= 0 && c < ww && (r >= wh - eh || c < ew)) m += 1;
-  }
-  {  // bl: expanded (r, c+2ew); kept if r<eh or c>=ww-ew
-    const int r = er, c = ec - 2 * ew;
-    if (r >= 0 && r < wh && c >= 0 && c < ww && (r < eh || c >= ww - ew)) m += 1;
-  }
-  {  // br: expanded (r, c); kept if r<eh or c<ew
-    const int r = er, c = ec;
-    if (r >= 0 && r < wh && c >= 0 && c < ww && (r < eh || c < ew)) m += 1;
-  }
-  return m;
-}
 
 __device__ __forceinline__ void loader_barrier() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 
@@ -462,17 +439,7 @@ int launch_focal_attention(const void* qkv, const void* qkv_pooled, void* out, i
   prm.use_pooled = use_pooled;
   prm.scale_log2 = scale * LOG2E;
   // order the expanded-window positions: single-listed first, multiply-listed last (positions never listed are dropped)
-  prm.n1 = prm.n2 = 0;
-  for (int pass = 0; pass < 2; ++pass)
-    for (int e = 0; e < EH * EW; ++e) {
-      const int m = key_multiplicity(e / EW, e % EW, wh, ww, eh, ew);
-      if ((pass == 0 && m == 1) || (pass == 1 && m > 1)) {
-        const int slot = prm.n1 + prm.n2;
-        prm.ring_pos[slot] = static_cast<uint8_t>(e);
-        prm.ring_mult[slot] = static_cast<uint8_t>(m);
-        (pass == 0 ? prm.n1 : prm.n2)++;
-      }
-    }
+  order_ring(wh, ww, eh, ew, prm.ring_pos, prm.ring_mult, prm.n1, prm.n2);
   const long long nwin = static_cast<long long>(b) * prm.nWh * prm.nWw;
   if (nwin > 65535 || heads > 65535) {
     set_error("focal attention: grid too large (B*nW=%lld)", nwin);

@@ -107,6 +107,16 @@ int launch_t2t_fold(const float* tok, const float* bias, float* img, int bt, int
 int launch_split_bf16(const float* x, void* hi, void* lo, long long n, cudaStream_t stream);
 int launch_linear_bf16x3(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, const float* bias,
                          const float* residual, void* out, int m, int n, int k, int out_dtype, cudaStream_t stream);
+// Focal attention backward (focal_attn_grad.cu): workspace size in floats (negative: argument error), the (window, key
+// slot, multiplicity) sources of one key token, and the launch.
+long long focal_attention_backward_work_elems(int b, int t, int h, int w, int heads, int wh, int ww, int eh, int ew,
+                                              int fh, int fw, int use_pooled);
+int focal_attention_key_sources(int t_count, int h, int w, int wh, int ww, int eh, int ew, int fh, int fw,
+                                int use_pooled, int t, int pooled, int y, int x, int* win, int* slot, int* mult, int cap);
+int launch_focal_attention_backward(const void* qkv, const void* qkv_pooled, const float* dout, float* dqkv,
+                                    float* dqkv_pooled, float* work, int b, int t, int h, int w, int heads, int wh,
+                                    int ww, int eh, int ew, int fh, int fw, int use_pooled, float scale,
+                                    cudaStream_t stream);
 // Linear weight / bias gradient (linear_wgrad.cu): dW [n][k] = dY^T X, db [n] = column sums of dY, from the split
 // dY [m][ldy] and X [m][ldx]; split-K workspace of linear_wgrad_work_elems floats (0: none needed).
 int linear_wgrad_slices(int m, int n, int k);

@@ -342,7 +342,13 @@ class WindowAttention(nn.Module):
         """x (B,T,H,W,C) normed tokens (tensor or ops.SplitMat), pooled (B,nWh,nWw,T,C) tensor or the SplitMat of
         ops.window_pool (already (B,T,nWh,nWw,C)) -> (B,T,H,W,C) after proj (+ residual).
         ``joint_shape`` = (B,T,H,W): x is the SplitMat of ``ops.layer_norm_pool`` (token rows followed by pooled rows) and
-        ONE qkv GEMM serves both."""
+        ONE qkv GEMM serves both.  Trainable (``_WindowAttentionGrad``) when grad mode is on, x is a tensor, no
+        ``joint_shape`` is given and x, pooled, the residual or a parameter of ``qkv`` / ``proj`` requires grad; the result
+        is the same bits as the untracked call."""
+        params = self.params()
+        if (joint_shape is None and isinstance(x, torch.Tensor) and not isinstance(pooled, ops.SplitMat)
+                and _tracked([x, pooled if self.uses_pooled else None, residual], [p for p in params if p is not None])):
+            return _WindowAttentionGrad.apply(self, x, pooled if self.uses_pooled else None, residual, *params)
         if joint_shape is not None:
             B, T, H, W = joint_shape
             wh, ww = self.window_size
@@ -361,11 +367,81 @@ class WindowAttention(nn.Module):
                                          self.pooled_kernel(), self.scale, out_dtype="split")
         return ops.linear(out, self.proj.weight, self.proj.bias, residual=residual)
 
+    def params(self):
+        """The parameters in ``_WindowAttentionGrad``'s order: qkv weight and bias (None without qkv_bias), proj weight
+        and bias."""
+        return self.qkv.weight, self.qkv.bias, self.proj.weight, self.proj.bias
+
     def forward(self, x_all, mask_all=None):
         """Reference boundary: x_all = [x (B,T,H,W,C), pooled (B,nWh,nWw,T,C)] -> (B*nW, T*wh*ww, C)."""
         del mask_all  # always [None, None] on the path (tfocal_transformer.py:475)
         out = self.attend(x_all[0], x_all[1] if len(x_all) > 1 else None)
         return window_partition(out, self.window_size)
+
+
+class _WindowAttentionGrad(torch.autograd.Function):
+    """``WindowAttention.attend``'s launches with a backward into qkv, proj, x, pooled and the residual.  The forward
+    splits the token rows and the pooled rows once, into one operand (kept for qkv's weight gradient), and runs the
+    same qkv, attention and proj launches as the untracked call.  Backward, with g = the output's gradient:
+      dW_proj = g^T . O (the attention's kept split output), db_proj = sum g;  dO = g . W_proj (``linear`` with W^T);
+      dqkv = the attention backward (token rows and pooled rows in one buffer);
+      dW_qkv = dqkv^T . [x; pooled] and db_qkv = sum dqkv over both sets of rows in one reduction;
+      [dx; dpooled] = dqkv . W_qkv (``linear`` with W^T); the residual receives g."""
+
+    @staticmethod
+    def forward(ctx, mod, x, pooled, residual, wq, bq, wp, bp):
+        B, T, H, W, C = x.shape
+        wh, ww = mod.window_size
+        n_tok = B * T * H * W
+        rows = x.reshape(n_tok, C)
+        if pooled is not None:                                  # reference layout (B,nWh,nWw,T,C) -> (B,T,nWh,nWw,C)
+            rows = torch.cat([rows, pooled.permute(0, 3, 1, 2, 4).reshape(-1, C)])
+        xs = ops.SplitMat(*ops.split_bf16(rows))
+        qkv = ops.linear(ops.SplitMat(xs.hi[:n_tok], xs.lo[:n_tok]), wq, bq, out_dtype=torch.float16).view(B, T, H, W, -1)
+        qkv_pooled = None
+        if pooled is not None:
+            qkv_pooled = ops.linear(ops.SplitMat(xs.hi[n_tok:], xs.lo[n_tok:]), wq, bq, out_dtype=torch.float16)
+            qkv_pooled = qkv_pooled.view(B, T, H // wh, W // ww, -1)
+        out = ops.focal_window_attention(qkv, qkv_pooled, mod.num_heads, mod.window_size, mod.expand_size,
+                                         mod.pooled_kernel(), mod.scale, out_dtype="split")
+        ctx.mod, ctx.keep, ctx.shape = mod, {"x": xs, "qkv": qkv, "qkv_pooled": qkv_pooled, "out": out}, x.shape
+        ctx.save_for_backward(wq, wp)
+        return ops.linear(out, wp, bp, residual=residual)
+
+    @staticmethod
+    def backward(ctx, grad):
+        if ctx.keep is None:
+            raise _second_backward("WindowAttention")
+        wq, wp = ctx.saved_tensors
+        keep, mod = ctx.keep, ctx.mod
+        ctx.keep = None
+        need_x, need_pool, need_res = ctx.needs_input_grad[1:4]
+        nwq, nbq, nwp, nbp = ctx.needs_input_grad[4:]
+        B, T, H, W, C = ctx.shape
+        dx = dpool = dwq = dbq = dwp = dbp = None
+        need_attn = need_x or need_pool or nwq or nbq
+        if nwp or nbp or need_attn:
+            g = ops.SplitMat(*ops.split_bf16(grad.reshape(-1, C)))
+        if nwp or nbp:
+            out = keep["out"]
+            dwp, dbp = ops.linear_wgrad(g, out.view(-1, C), with_bias=nbp)
+            dwp = dwp if nwp else None
+        if need_attn:
+            dout = ops.linear(g, wp, transpose=True).view(B, T, H, W, C)
+            dqkv = ops.focal_window_attention_backward(keep["qkv"], keep["qkv_pooled"], dout, mod.num_heads,
+                                                       mod.window_size, mod.expand_size, mod.pooled_kernel(), mod.scale)
+            dqkv = ops.SplitMat(*ops.split_bf16(dqkv))        # one split serves qkv's weight and input gradients
+            if nwq or nbq:
+                dwq, dbq = ops.linear_wgrad(dqkv, keep["x"], with_bias=nbq)
+                dwq = dwq if nwq else None
+            if need_x or need_pool:
+                n_tok = B * T * H * W
+                drows = ops.linear(dqkv, wq, transpose=True)
+                dx = drows[:n_tok].view(B, T, H, W, C) if need_x else None
+                if need_pool:
+                    wh, ww = mod.window_size
+                    dpool = drows[n_tok:].view(B, T, H // wh, W // ww, C).permute(0, 2, 3, 1, 4).contiguous()
+        return None, dx, dpool, grad if need_res else None, dwq, dbq, dwp, dbp
 
 
 class TemporalFocalTransformerBlock(nn.Module):

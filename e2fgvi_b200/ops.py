@@ -8,6 +8,7 @@
 Same names / argument meaning / error behaviour as the reference operators; every call goes through the C ABI of
 ``libe2fgvi_b200.so`` on the current CUDA stream.  There is no CPU path: CPU tensors raise.
 """
+import ctypes
 import weakref
 
 import torch
@@ -324,6 +325,56 @@ def focal_window_attention(qkv, qkv_pooled, num_heads, window_size, expand_size,
             1 if use_pooled else 0, float(scale), 2 if split else _DT[out_dtype], _stream())
     _lib.check(st, "e2f_focal_window_attention")
     return SplitMat(out[0], out[1]) if split else out
+
+
+def focal_window_attention_backward(qkv, qkv_pooled, dout, num_heads, window_size, expand_size, focal_window, scale):
+    """Gradients of ``focal_window_attention`` (``e2f_focal_window_attention_backward``): qkv / qkv_pooled the fp16
+    operands the forward read, dout (B,T,H,W,C) fp32 -> one fp32 buffer (B*T*H*W + B*T*nWh*nWw, 3C): the token rows'
+    dq | dk | dv, then the pooled rows' 0 | dk | dv (none without qkv_pooled) — the qkv Linear's output gradient for
+    the token rows and pooled rows together."""
+    _need_cuda(qkv, qkv_pooled, dout)
+    B, T, H, W, C3 = qkv.shape
+    C = C3 // 3
+    wh, ww = window_size
+    use_pooled = qkv_pooled is not None
+    if qkv.dtype != torch.float16 or not qkv.is_contiguous():
+        raise ValueError("focal_window_attention_backward: qkv must be the contiguous fp16 tensor the forward read")
+    if use_pooled and (qkv_pooled.dtype != torch.float16 or not qkv_pooled.is_contiguous()
+                       or qkv_pooled.shape != (B, T, H // wh, W // ww, C3)):
+        raise ValueError("focal_window_attention_backward: qkv_pooled must be the contiguous fp16 tensor the forward read")
+    if dout.shape != (B, T, H, W, C):
+        raise ValueError(f"focal_window_attention_backward: dout shape {tuple(dout.shape)} != {(B, T, H, W, C)}")
+    dout = dout.contiguous().float()
+    geo = (B, T, H, W, num_heads, C // num_heads, wh, ww, expand_size[0], expand_size[1], focal_window[0],
+           focal_window[1], 1 if use_pooled else 0)
+    lib = _lib.load()
+    elems = int(lib.e2f_focal_window_attention_backward_work_elems(*geo))
+    if elems < 0:
+        _lib.check(elems, "e2f_focal_window_attention_backward_work_elems")
+    n_tok, n_pool = B * T * H * W, (B * T * (H // wh) * (W // ww) if use_pooled else 0)
+    d = torch.empty((n_tok + n_pool, C3), dtype=torch.float32, device=qkv.device)
+    work = torch.empty(max(elems, 4), dtype=torch.float32, device=qkv.device)
+    # the backward's algorithmic products: S, dP, dV, dQ, dK
+    with _timed("focal_window_attention_backward",
+                2.5 * attention_flops(B, T, H, W, C, window_size, expand_size, focal_window, use_pooled)):
+        st = lib.e2f_focal_window_attention_backward(
+            qkv.data_ptr(), qkv_pooled.data_ptr() if use_pooled else None, dout.data_ptr(), d.data_ptr(),
+            d[n_tok:].data_ptr() if use_pooled else None, work.data_ptr(), *geo[:12], geo[12], float(scale), _stream())
+    _lib.check(st, "e2f_focal_window_attention_backward")
+    return d
+
+
+def focal_attention_key_sources(t_count, grid, window_size, expand_size, focal_window, use_pooled, t, pooled, y, x):
+    """The backward's gather list of one key token: [(window index, key slot, multiplicity), ...] in the order the
+    backward adds them (``e2f_focal_window_attention_key_sources``; host only)."""
+    cap = 256
+    win, slot, mult = (ctypes.c_int * cap)(), (ctypes.c_int * cap)(), (ctypes.c_int * cap)()
+    n = _lib.load().e2f_focal_window_attention_key_sources(
+        t_count, grid[0], grid[1], window_size[0], window_size[1], expand_size[0], expand_size[1], focal_window[0],
+        focal_window[1], 1 if use_pooled else 0, t, 1 if pooled else 0, y, x, win, slot, mult, cap)
+    if n < 0:
+        _lib.check(n, "e2f_focal_window_attention_key_sources")
+    return [(win[i], slot[i], mult[i]) for i in range(n)]
 
 
 class SplitMat:

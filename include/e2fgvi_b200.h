@@ -113,6 +113,31 @@ int e2f_focal_window_attention(const void* qkv, const void* qkv_pooled, void* ou
                                int heads, int head_dim, int wh, int ww, int eh, int ew, int fh, int fw,
                                int use_pooled, float scale, int out_dtype, void* stream);
 
+/* Backward of e2f_focal_window_attention: the exact-softmax gradients of the attention core with respect to q, k, v of
+ * the token rows and k, v of the pooled rows, given the fp16 qkv / qkv_pooled the forward read and
+ *   dout        [B][T][H][W][C] fp32     gradient of the forward's output
+ *   dqkv        [B][T][H][W][3*C] fp32   dq | dk | dv (every element written)
+ *   dqkv_pooled [B][T][nWh][nWw][3*C] fp32 (use_pooled = 1): 0 | dk | dv
+ *   work        e2f_focal_window_attention_backward_work_elems(...) floats: 2 floats per query row and head, and
+ *               per-(window, key slot) dK | dV and per-window dQ fp32 partials of at most 32M floats (128 MB) per
+ *               chunk of (clip, head) pairs (at least one pair).
+ * A key the reference lists m times (the duplicated ring tokens, the wrap on small grids, every pooled neighbourhood
+ * holding a pooled token) gets the sum over its copies.  Every product on wgmma with the bf16 three-term split and fp32
+ * accumulation, no atomics: the results are bit-identical from run to run.  Shapes and arguments as e2f_focal_window_attention. */
+int64_t e2f_focal_window_attention_backward_work_elems(int b, int t, int h, int w, int heads, int head_dim, int wh,
+                                                       int ww, int eh, int ew, int fh, int fw, int use_pooled);
+int e2f_focal_window_attention_backward(const void* qkv, const void* qkv_pooled, const float* dout, float* dqkv,
+                                        float* dqkv_pooled, float* work, int b, int t, int h, int w, int heads,
+                                        int head_dim, int wh, int ww, int eh, int ew, int fh, int fw, int use_pooled,
+                                        float scale, void* stream);
+/* The gather list of the backward for one key token of a clip with t_count frames: token (t, y, x) of the token grid
+ * (pooled = 0) or pooled token (t, y = window row, x = window column) (pooled = 1).  Writes up to `cap` entries of
+ * (window index wi * nWw + wj, key slot in that window's key list, multiplicity = how many times the reference lists
+ * the token there) in the order the backward adds them; returns the count.  Host only, no CUDA call. */
+int e2f_focal_window_attention_key_sources(int t_count, int h, int w, int wh, int ww, int eh, int ew, int fh, int fw,
+                                           int use_pooled, int t, int pooled, int y, int x, int* win, int* slot,
+                                           int* mult, int cap);
+
 /* T2T token <-> image transforms, replacing F.unfold / F.fold as used by SoftSplit (tfocal_transformer.py:39-43),
  * SoftComp (:65-72) and FusionFeedForward (:89-96).  img [BT][C][H][W] fp32 (NCHW), tokens [BT][L][C*k*k] fp32 with
  * L = fh*fw, fh = (H+2p-k)/s+1, channel = c*k*k + ky*k + kx (torch.nn.Unfold order), i.e. the token-major layout
