@@ -34,6 +34,10 @@ SIGNATURES = {
     "e2f_t2t_fold_unfold": (_i, [_fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "e2f_t2t_fold_unfold_train": (_i, [_fp, _fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "e2f_t2t_fold": (_i, [_fp, _fp, _fp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "e2f_layernorm_backward_work_elems": (_c.c_int64, [_c.c_int64, _i]),
+    "e2f_layernorm_backward": (_i, [_fp, _fp, _fp, _fp, _fp, _vp, _vp, _fp, _fp, _fp, _c.c_int64, _i, _f, _vp]),
+    "e2f_layernorm_pool_backward_work_elems": (_c.c_int64, [_i] * 6),
+    "e2f_layernorm_pool_backward": (_i, [_fp] * 12 + [_i] * 6 + [_f, _vp]),
     "e2f_split_bf16": (_i, [_fp, _vp, _vp, _c.c_int64, _vp]),
     "e2f_linear_bf16x3": (_i, [_vp, _vp, _vp, _vp, _fp, _fp, _vp, _i, _i, _i, _i, _i, _vp]),
     "e2f_linear_wgrad_work_elems": (_c.c_int64, [_i, _i, _i]),

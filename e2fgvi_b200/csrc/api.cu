@@ -317,6 +317,53 @@ int e2f_layernorm_split(const float* x, const float* gamma, const float* beta, f
   return finish(launch_layernorm_split(x, gamma, beta, out, out_hi, out_lo, rows, c, eps, static_cast<cudaStream_t>(stream)), "e2f_layernorm_split");
 }
 
+int64_t e2f_layernorm_backward_work_elems(int64_t rows, int c) {
+  if (rows < 0 || c != 512) { set_error("e2f_layernorm_backward_work_elems: rows=%lld c=%d (512 channels only)", static_cast<long long>(rows), c); return c != 512 && rows >= 0 ? E2F_ERR_UNSUPPORTED : E2F_ERR_BAD_ARG; }
+  return static_cast<int64_t>(layernorm_backward_work_elems(rows));
+}
+
+int e2f_layernorm_backward(const float* x, const float* dy, const float* gamma, const float* residual, float* dx,
+                           void* dx_hi, void* dx_lo, float* dgamma, float* dbeta, float* work, int64_t rows, int c,
+                           float eps, void* stream) {
+  const char* who = "e2f_layernorm_backward";
+  const bool params = dgamma || dbeta;
+  if (!x || !dy || !gamma) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if ((!dx && !dx_hi && !params) || (!dx_hi) != (!dx_lo)) { set_error("%s: need dx, both of dx_hi/dx_lo, or a parameter gradient", who); return E2F_ERR_BAD_ARG; }
+  if (params && !work && rows > 0) { set_error("%s: null workspace (e2f_layernorm_backward_work_elems floats needed)", who); return E2F_ERR_BAD_ARG; }
+  if (rows < 0 || c <= 0) { set_error("%s: bad shape rows=%lld c=%d", who, static_cast<long long>(rows), c); return E2F_ERR_BAD_ARG; }
+  if (c != 512) { set_error("%s: specialised for 512 channels (got %d)", who, c); return E2F_ERR_UNSUPPORTED; }
+  if (!aligned(x, 16) || !aligned(dy, 16) || (residual && !aligned(residual, 16)) || (dx && !aligned(dx, 16)) || (dx_hi && (!aligned(dx_hi, 16) || !aligned(dx_lo, 16))) || !aligned(gamma, 4) || (dgamma && !aligned(dgamma, 4)) || (dbeta && !aligned(dbeta, 4)) || (work && !aligned(work, 16))) { set_error("%s: 16-byte alignment required", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_layernorm_backward(x, dy, gamma, residual, dx, dx_hi, dx_lo, dgamma, dbeta, params ? work : nullptr, rows, c, eps, static_cast<cudaStream_t>(stream)), who);
+}
+
+static int layernorm_pool_geometry_checks(const char* who, int bt, int h, int w, int c, int wh, int ww) {
+  if (bt < 0 || h <= 0 || w <= 0 || c <= 0 || wh <= 0 || ww <= 0) { set_error("%s: bad shape bt=%d h=%d w=%d c=%d window=%dx%d", who, bt, h, w, c, wh, ww); return E2F_ERR_BAD_ARG; }
+  if (h % wh || w % ww) { set_error("%s: token grid %dx%d is not a multiple of the window %dx%d", who, h, w, wh, ww); return E2F_ERR_BAD_ARG; }
+  if (c != 512) { set_error("%s: specialised for 512 channels (got %d)", who, c); return E2F_ERR_UNSUPPORTED; }
+  if (bt > 65535) { set_error("%s: at most 65535 frames per launch (got %d)", who, bt); return E2F_ERR_UNSUPPORTED; }
+  return 0;
+}
+
+int64_t e2f_layernorm_pool_backward_work_elems(int bt, int h, int w, int c, int wh, int ww) {
+  if (const int st = layernorm_pool_geometry_checks("e2f_layernorm_pool_backward_work_elems", bt, h, w, c, wh, ww)) return st;
+  return static_cast<int64_t>(layernorm_pool_backward_work_elems(bt, h, w, wh, ww));
+}
+
+int e2f_layernorm_pool_backward(const float* x, const float* gamma, const float* beta, const float* pool_w,
+                                const float* drows, const float* dx1, float* dx, float* dgamma, float* dbeta,
+                                float* dpool_w, float* dpool_b, float* work, int bt, int h, int w, int c, int wh, int ww,
+                                float eps, void* stream) {
+  const char* who = "e2f_layernorm_pool_backward";
+  const bool params = dgamma || dbeta || dpool_w || dpool_b;
+  if (!x || !gamma || !beta || !pool_w || !drows) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if (!dx && !params) { set_error("%s: need dx or a parameter gradient", who); return E2F_ERR_BAD_ARG; }
+  if (dx && !dx1) { set_error("%s: dx needs dx1", who); return E2F_ERR_BAD_ARG; }
+  if (params && !work && bt > 0) { set_error("%s: null workspace (e2f_layernorm_pool_backward_work_elems floats needed)", who); return E2F_ERR_BAD_ARG; }
+  if (const int st = layernorm_pool_geometry_checks(who, bt, h, w, c, wh, ww)) return st;
+  if (!aligned(x, 16) || !aligned(drows, 16) || (dx && (!aligned(dx, 16) || !aligned(dx1, 16))) || !aligned(gamma, 4) || !aligned(beta, 4) || !aligned(pool_w, 4) || (work && !aligned(work, 16))) { set_error("%s: 16-byte alignment required", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_layernorm_pool_backward(x, gamma, beta, pool_w, drows, dx1, dx, dgamma, dbeta, dpool_w, dpool_b, params ? work : nullptr, bt, h, w, c, wh, ww, eps, static_cast<cudaStream_t>(stream)), who);
+}
+
 int e2f_t2t_fold(const float* tokens, const float* bias, float* img, int bt, int c, int h, int w, int k, int stride,
                  int pad, int normalize, void* stream) {
   int st = t2t_checks("e2f_t2t_fold", tokens, img, bt, c, h, w, k, stride, pad);

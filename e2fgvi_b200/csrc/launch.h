@@ -92,6 +92,17 @@ int launch_layernorm_split(const float* x, const float* gamma, const float* beta
 int launch_layernorm_pool_split(const float* x, const float* gamma, const float* beta, const float* pool_w,
                                 const float* pool_b, void* hi, void* lo, int bt, int h, int w, int c, int wh, int ww,
                                 float eps, cudaStream_t stream);
+// LayerNorm / LayerNorm + window pooling backward (layernorm_grad.cu): per-CTA partial rows of the parameter gradients
+// in `work` (the *_work_elems floats), added in a fixed order by a second launch.
+long long layernorm_backward_work_elems(long long rows);
+long long layernorm_pool_backward_work_elems(int bt, int h, int w, int wh, int ww);
+int launch_layernorm_backward(const float* x, const float* dy, const float* gamma, const float* res, float* out, void* hi,
+                              void* lo, float* dgamma, float* dbeta, float* work, long long rows, int c, float eps,
+                              cudaStream_t stream);
+int launch_layernorm_pool_backward(const float* x, const float* gamma, const float* beta, const float* pool_w,
+                                   const float* drows, const float* dx1, float* out, float* dgamma, float* dbeta,
+                                   float* dpool_w, float* dpool_b, float* work, int bt, int h, int w, int c, int wh,
+                                   int ww, float eps, cudaStream_t stream);
 int launch_window_pool(const void* xh, const void* xl, const float* weight, const float* bias, float* out, void* out_hi,
                        void* out_lo, int bt, int h, int w, int c, int wh, int ww, cudaStream_t stream);
 // gu != nullptr: the adjoint of the training forward (tin = dz, gu = its saved u); u_out != nullptr (gelu only): the

@@ -369,10 +369,9 @@ class InpaintGenerator(BaseNetwork):
 
         fold_size = (h, w)
         tokens = self.ss(enc_sp, b, fold_size if self.HQ else None)
-        if self.HQ:
-            tokens = self.transformer([tokens, fold_size])[0]
-        else:
-            tokens = self.transformer(tokens)
+        # the blocks' untracked launches: a tracked block would keep its backward operands inside an inference call
+        for blk in self.transformer:
+            tokens = blk._forward(tokens, fold_size if self.HQ else None)
         # enc_feat + trans_feat (e2fgvi.py:263) is fused into SoftComp's fold / conv epilogue
         enc_feat = self.sc._forward(tokens, t, fold_size if self.HQ else None, residual=enc_feat)
 

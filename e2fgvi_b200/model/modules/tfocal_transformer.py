@@ -225,25 +225,54 @@ class FusionFeedForward(nn.Module):
         return output_size, p["kernel_size"], p["stride"], p["padding"]
 
 
-class _FusionFeedForwardGrad(torch.autograd.Function):
-    """``FusionFeedForward``'s launches with a backward into both Linears, x and the residual.  The forward splits x
-    once (conv1's operand, kept for its weight gradient) and runs the fold/normalise/unfold kernel in its training mode,
-    which also keeps u, the normalised values before GELU.  Backward, with g = the output's gradient:
+def _ffn_forward(mod, xs, output_size, w1, b1, w2, b2, residual):
+    """``FusionFeedForward``'s training launches on the split operand xs (rows, 512): conv1, the fold/normalise/unfold
+    kernel in its training mode (which also keeps u, the normalised values before GELU), conv2 (+ residual).  Returns
+    (out (rows, 512), the dict ``_ffn_backward`` reads)."""
+    geo = mod.geometry(output_size)
+    h = ops.linear(xs, w1, b1)
+    hd = h.shape[-1]
+    f_h, f_w = _token_grid(*geo)
+    z, u = ops.t2t_fold_unfold_train(h.view(-1, f_h * f_w, hd), *geo, out="split", pitch=(hd + 63) // 64 * 64)
+    out = ops.linear(z.view(-1, z.shape[-1]), w2, b2, residual=residual)
+    return out, {"x": xs, "u": u, "z": z, "geo": geo}
+
+
+def _ffn_backward(keep, grad, w1, w2, need_x, nw1, nb1, nw2, nb2):
+    """The backward of ``_ffn_forward`` at g = grad (rows, 512) fp32: (dx (rows, 512) or None, dW1, db1, dW2, db2), each
+    None when not asked for.
       dz = g . W2 (``linear`` with W2^T), dW2 = g^T . GELU(u) (the kept split operand), db2 = sum g;
-      dh = U D F (dz * GELU'(u)) (the same kernel's adjoint mode, written as a split operand with the 1984 pitch);
-      dx = dh . W1 (``linear`` with W1^T, padded alike), dW1 = dh^T . x, db1 = sum dh; the residual receives g."""
+      dh = U D F (dz * GELU'(u)) (the fold/normalise/unfold kernel's adjoint mode, a split operand with the 1984 pitch);
+      dx = dh . W1 (``linear`` with W1^T, padded alike), dW1 = dh^T . x, db1 = sum dh."""
+    z, u = keep["z"], keep["u"]
+    g = ops.SplitMat(*ops.split_bf16(grad.reshape(-1, grad.shape[-1])))
+    dw1 = db1 = dw2 = db2 = dx = None
+    if nw2 or nb2:
+        dw2, db2 = ops.linear_wgrad(g, z.view(-1, z.shape[-1]), with_bias=nb2, shape=tuple(w2.shape))
+        dw2 = dw2 if nw2 else None
+    if need_x or nw1 or nb1:
+        dz = ops.linear(g, w2, transpose=True)
+        dh = ops.t2t_fold_unfold_train(dz.view(u.shape), *keep["geo"], u=u, out="split", pitch=z.shape[-1])
+        dh = dh.view(-1, dh.shape[-1])
+        if nw1 or nb1:
+            dw1, db1 = ops.linear_wgrad(dh, keep["x"], with_bias=nb1, shape=tuple(w1.shape))
+            dw1 = dw1 if nw1 else None
+        if need_x:
+            dx = ops.linear(dh, w1, transpose=True)
+    return dx, dw1, db1, dw2, db2
+
+
+class _FusionFeedForwardGrad(torch.autograd.Function):
+    """``FusionFeedForward``'s launches with a backward into both Linears, x and the residual: the forward splits x
+    once (conv1's operand, kept for its weight gradient) and runs ``_ffn_forward``; the backward is ``_ffn_backward``,
+    and the residual receives the output's gradient."""
 
     @staticmethod
     def forward(ctx, mod, x, residual, output_size, w1, b1, w2, b2):
-        geo = mod.geometry(output_size)
         b, n, _ = x.shape
         xs = ops.SplitMat(*ops.split_bf16(x.reshape(-1, x.shape[-1])))
-        h = ops.linear(xs, w1, b1)
-        hd = h.shape[-1]
-        f_h, f_w = _token_grid(*geo)
-        z, u = ops.t2t_fold_unfold_train(h.view(-1, f_h * f_w, hd), *geo, out="split", pitch=(hd + 63) // 64 * 64)
-        out = ops.linear(z.view(b * n, z.shape[-1]), w2, b2, residual=residual)
-        ctx.mod, ctx.geo, ctx.keep, ctx.shape = mod, geo, {"x": xs, "u": u, "z": z}, x.shape
+        out, ctx.keep = _ffn_forward(mod, xs, output_size, w1, b1, w2, b2, residual)
+        ctx.shape = x.shape
         ctx.save_for_backward(w1, w2)
         return out.view(b, n, -1)
 
@@ -255,24 +284,8 @@ class _FusionFeedForwardGrad(torch.autograd.Function):
         keep = ctx.keep
         ctx.keep = None
         need_x, need_res = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
-        nw1, nb1, nw2, nb2 = ctx.needs_input_grad[4:]
-        z, u = keep["z"], keep["u"]
-        hd = w1.shape[0]
-        g = ops.SplitMat(*ops.split_bf16(grad.reshape(-1, grad.shape[-1])))
-        dw1 = db1 = dw2 = db2 = dx = None
-        if nw2 or nb2:
-            dw2, db2 = ops.linear_wgrad(g, z.view(-1, z.shape[-1]), with_bias=nb2, shape=tuple(w2.shape))
-            dw2 = dw2 if nw2 else None
-        if need_x or nw1 or nb1:
-            dz = ops.linear(g, w2, transpose=True)
-            dh = ops.t2t_fold_unfold_train(dz.view(u.shape), *ctx.geo, u=u, out="split", pitch=z.shape[-1])
-            dh = dh.view(-1, dh.shape[-1])
-            if nw1 or nb1:
-                dw1, db1 = ops.linear_wgrad(dh, keep["x"], with_bias=nb1, shape=tuple(w1.shape))
-                dw1 = dw1 if nw1 else None
-            if need_x:
-                dx = ops.linear(dh, w1, transpose=True).view(ctx.shape)
-        return None, dx, grad if need_res else None, None, dw1, db1, dw2, db2
+        dx, dw1, db1, dw2, db2 = _ffn_backward(keep, grad, w1, w2, need_x, *ctx.needs_input_grad[4:])
+        return None, None if dx is None else dx.view(ctx.shape), grad if need_res else None, None, dw1, db1, dw2, db2
 
 
 def window_partition(x, window_size):
@@ -338,15 +351,16 @@ class WindowAttention(nn.Module):
         """Neighbourhood of pooled windows each query window attends (unfold kernel, tfocal_transformer.py:186-196)."""
         return tuple(2 * (i // 2) + 1 for i in self.focal_window)
 
-    def attend(self, x, pooled, residual=None, joint_shape=None):
+    def attend(self, x, pooled, residual=None, joint_shape=None, keep=None):
         """x (B,T,H,W,C) normed tokens (tensor or ops.SplitMat), pooled (B,nWh,nWw,T,C) tensor or the SplitMat of
         ops.window_pool (already (B,T,nWh,nWw,C)) -> (B,T,H,W,C) after proj (+ residual).
         ``joint_shape`` = (B,T,H,W): x is the SplitMat of ``ops.layer_norm_pool`` (token rows followed by pooled rows) and
         ONE qkv GEMM serves both.  Trainable (``_WindowAttentionGrad``) when grad mode is on, x is a tensor, no
         ``joint_shape`` is given and x, pooled, the residual or a parameter of ``qkv`` / ``proj`` requires grad; the result
-        is the same bits as the untracked call."""
+        is the same bits as the untracked call.  ``keep`` (a dict or None; untracked calls on a SplitMat x without pooled
+        only) receives what ``_attention_backward`` reads: x, the fp16 qkv / qkv_pooled and the split attention output."""
         params = self.params()
-        if (joint_shape is None and isinstance(x, torch.Tensor) and not isinstance(pooled, ops.SplitMat)
+        if (keep is None and joint_shape is None and isinstance(x, torch.Tensor) and not isinstance(pooled, ops.SplitMat)
                 and _tracked([x, pooled if self.uses_pooled else None, residual], [p for p in params if p is not None])):
             return _WindowAttentionGrad.apply(self, x, pooled if self.uses_pooled else None, residual, *params)
         if joint_shape is not None:
@@ -365,6 +379,8 @@ class WindowAttention(nn.Module):
                 qkv_pooled = ops.linear(pooled, self.qkv.weight, self.qkv.bias, out_dtype=torch.float16)
         out = ops.focal_window_attention(qkv, qkv_pooled, self.num_heads, self.window_size, self.expand_size,
                                          self.pooled_kernel(), self.scale, out_dtype="split")
+        if keep is not None:
+            keep.update(x=x, qkv=qkv, qkv_pooled=qkv_pooled, out=out)
         return ops.linear(out, self.proj.weight, self.proj.bias, residual=residual)
 
     def params(self):
@@ -418,30 +434,46 @@ class _WindowAttentionGrad(torch.autograd.Function):
         need_x, need_pool, need_res = ctx.needs_input_grad[1:4]
         nwq, nbq, nwp, nbp = ctx.needs_input_grad[4:]
         B, T, H, W, C = ctx.shape
-        dx = dpool = dwq = dbq = dwp = dbp = None
-        need_attn = need_x or need_pool or nwq or nbq
-        if nwp or nbp or need_attn:
+        g = None
+        if nwp or nbp or need_x or need_pool or nwq or nbq:
             g = ops.SplitMat(*ops.split_bf16(grad.reshape(-1, C)))
-        if nwp or nbp:
-            out = keep["out"]
-            dwp, dbp = ops.linear_wgrad(g, out.view(-1, C), with_bias=nbp)
-            dwp = dwp if nwp else None
-        if need_attn:
-            dout = ops.linear(g, wp, transpose=True).view(B, T, H, W, C)
-            dqkv = ops.focal_window_attention_backward(keep["qkv"], keep["qkv_pooled"], dout, mod.num_heads,
-                                                       mod.window_size, mod.expand_size, mod.pooled_kernel(), mod.scale)
-            dqkv = ops.SplitMat(*ops.split_bf16(dqkv))        # one split serves qkv's weight and input gradients
-            if nwq or nbq:
-                dwq, dbq = ops.linear_wgrad(dqkv, keep["x"], with_bias=nbq)
-                dwq = dwq if nwq else None
-            if need_x or need_pool:
-                n_tok = B * T * H * W
-                drows = ops.linear(dqkv, wq, transpose=True)
-                dx = drows[:n_tok].view(B, T, H, W, C) if need_x else None
-                if need_pool:
-                    wh, ww = mod.window_size
-                    dpool = drows[n_tok:].view(B, T, H // wh, W // ww, C).permute(0, 2, 3, 1, 4).contiguous()
+        drows, dwq, dbq, dwp, dbp = _attention_backward(mod, keep, g, wq, wp, ctx.shape, need_x or need_pool, nwq, nbq,
+                                                        nwp, nbp)
+        dx = dpool = None
+        n_tok = B * T * H * W
+        if need_x:
+            dx = drows[:n_tok].view(B, T, H, W, C)
+        if need_pool:
+            wh, ww = mod.window_size
+            dpool = drows[n_tok:].view(B, T, H // wh, W // ww, C).permute(0, 2, 3, 1, 4).contiguous()
         return None, dx, dpool, grad if need_res else None, dwq, dbq, dwp, dbp
+
+
+def _attention_backward(mod, keep, g, wq, wp, shape, need_rows, nwq, nbq, nwp, nbp):
+    """The backward of ``WindowAttention.attend``'s launches at the split output gradient g (B*T*H*W, C), with ``keep``
+    = the kept joint split input "x" (token rows, then pooled rows ordered (B,T,nWh,nWw)), the fp16 "qkv" /
+    "qkv_pooled" and the attention's split output "out".  Returns (drows, dW_qkv, db_qkv, dW_proj, db_proj), each None
+    when not asked for; drows (rows of x, C) fp32 = [dx; dpooled] in x's joint layout (``need_rows``).
+      dW_proj = g^T . O, db_proj = sum g;  dO = g . W_proj (``linear`` with W^T);
+      dqkv = the attention backward (token rows and pooled rows in one buffer), split once for both of its uses;
+      dW_qkv = dqkv^T . [x; pooled] and db_qkv = sum dqkv over both sets of rows in one reduction;
+      [dx; dpooled] = dqkv . W_qkv (``linear`` with W^T)."""
+    B, T, H, W, C = shape
+    drows = dwq = dbq = dwp = dbp = None
+    if nwp or nbp:
+        dwp, dbp = ops.linear_wgrad(g, keep["out"].view(-1, C), with_bias=nbp)
+        dwp = dwp if nwp else None
+    if need_rows or nwq or nbq:
+        dout = ops.linear(g, wp, transpose=True).view(B, T, H, W, C)
+        dqkv = ops.focal_window_attention_backward(keep["qkv"], keep["qkv_pooled"], dout, mod.num_heads,
+                                                   mod.window_size, mod.expand_size, mod.pooled_kernel(), mod.scale)
+        dqkv = ops.SplitMat(*ops.split_bf16(dqkv))        # one split serves qkv's weight and input gradients
+        if nwq or nbq:
+            dwq, dbq = ops.linear_wgrad(dqkv, keep["x"], with_bias=nbq)
+            dwq = dwq if nwq else None
+        if need_rows:
+            drows = ops.linear(dqkv, wq, transpose=True)
+    return drows, dwq, dbq, dwp, dbp
 
 
 class TemporalFocalTransformerBlock(nn.Module):
@@ -470,9 +502,21 @@ class TemporalFocalTransformerBlock(nn.Module):
         self.norm2 = norm_layer(dim)
         self.mlp = FusionFeedForward(dim, n_vecs=n_vecs, t2t_params=t2t_params)
 
-    def _forward(self, x, output_size):
+    def params(self):
+        """The parameters in ``_TransformerBlockGrad``'s order: norm1 weight and bias, pool_layers[0] weight and bias
+        (None without pooling), attn.qkv weight and bias (None without qkv_bias), attn.proj weight and bias, norm2
+        weight and bias, mlp.conv1[0] weight and bias, mlp.conv2[1] weight and bias."""
+        pool = (self.pool_layers[0].weight, self.pool_layers[0].bias) if self.attn.uses_pooled else (None, None)
+        return ((self.norm1.weight, self.norm1.bias) + pool + self.attn.params() + (self.norm2.weight, self.norm2.bias)
+                + (self.mlp.conv1[0].weight, self.mlp.conv1[0].bias, self.mlp.conv2[1].weight, self.mlp.conv2[1].bias))
+
+    def _forward(self, x, output_size, keep=None):
+        """The launch sequence of ``forward`` (untracked); ``keep`` (a dict or None) receives what
+        ``_TransformerBlockGrad.backward`` reads: x1 = the attention's output (+ x), the attention's operands and the
+        feed-forward's (which then runs its training forward: the same bits)."""
         shortcut = x
         B, T, H, W, C = x.shape
+        attn_keep = None if keep is None else keep.setdefault("attn", {})
         if self.attn.uses_pooled:
             if H % self.window_size[0] or W % self.window_size[1]:
                 raise ValueError(f"token grid {H}x{W} must be a multiple of the window {self.window_size}")
@@ -481,15 +525,100 @@ class TemporalFocalTransformerBlock(nn.Module):
             lin = self.pool_layers[0]
             rows, _ = ops.layer_norm_pool(x, self.norm1.weight, self.norm1.bias, self.norm1.eps, lin.weight, lin.bias,
                                           self.window_size)
-            x = self.attn.attend(rows, None, residual=shortcut, joint_shape=(B, T, H, W))
+            x = self.attn.attend(rows, None, residual=shortcut, joint_shape=(B, T, H, W), keep=attn_keep)
         else:
             xn_split = ops.layer_norm(x, self.norm1.weight, self.norm1.bias, self.norm1.eps, out="split")
-            x = self.attn.attend(xn_split, None, residual=shortcut)
+            x = self.attn.attend(xn_split, None, residual=shortcut, keep=attn_keep)
         y = ops.layer_norm(x, self.norm2.weight, self.norm2.bias, self.norm2.eps, out="split")
-        return self.mlp(y.view(B, T * H * W, C), output_size, residual=x.view(B, T * H * W, C)).view(B, T, H, W, C)
+        if keep is None:
+            return self.mlp(y.view(B, T * H * W, C), output_size, residual=x.view(B, T * H * W, C)).view(B, T, H, W, C)
+        mlp = self.mlp
+        size = tuple(output_size or mlp.t2t_params["output_size"])
+        out, keep["mlp"] = _ffn_forward(mlp, y.view(B * T * H * W, C), size, mlp.conv1[0].weight, mlp.conv1[0].bias,
+                                        mlp.conv2[1].weight, mlp.conv2[1].bias, x)
+        keep["x1"] = x
+        return out.view(B, T, H, W, C)
 
     def forward(self, x):
+        """tokens (B,T,H,W,C) -> (B,T,H,W,C); HQ: [tokens, output_size] -> (tokens, output_size).  Trainable
+        (``_TransformerBlockGrad``) when grad mode is on and the tokens or a parameter requires grad; the result is the
+        same bits as the untracked call."""
         if self.hq:  # x = [tokens, (h, w)] -> (tokens, (h, w))   (_hq.py:492-495,562-565)
             tokens, output_size = x[0], x[1]
-            return self._forward(tokens, output_size), output_size
-        return self._forward(x, None)
+        else:
+            tokens, output_size = x, None
+        params = self.params()
+        if _tracked([tokens], [p for p in params if p is not None]):
+            out = _TransformerBlockGrad.apply(self, tokens, output_size, *params)
+        else:
+            out = self._forward(tokens, output_size)
+        return (out, output_size) if self.hq else out
+
+
+class _TransformerBlockGrad(torch.autograd.Function):
+    """``TemporalFocalTransformerBlock``'s launches (``_forward`` with ``keep``) with a backward into every parameter
+    and the tokens x.  With g = the output's gradient and x1 = x + attention(LN1(x)):
+      1. the feed-forward's backward (``_ffn_backward``) gives dy = the gradient of LN2's output and both Linears';
+      2. dx1 = g + LN2'(x1; dy) (``layer_norm_backward``, fp32 and split), dgamma2, dbeta2;
+      3. the attention's backward (``_attention_backward``) at dx1 gives [dxn; dpooled] and qkv's and proj's gradients;
+      4. dx = dx1 + LN1'(x; dxn + w_pool dpooled) (``layer_norm_pool_backward``; without pooling ``layer_norm_backward``
+         with the residual dx1), dgamma1, dbeta1, d w_pool, d b_pool.
+    The walk stops at the lowest part that needs a gradient; a frozen part launches no weight gradient."""
+
+    @staticmethod
+    def forward(ctx, mod, x, output_size, *params):
+        keep = {}
+        out = mod._forward(x, output_size, keep)
+        ctx.mod, ctx.keep = mod, keep
+        ctx.save_for_backward(x, *[p for p in params if p is not None])
+        ctx.have = [p is not None for p in params]
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        if ctx.keep is None:
+            raise _second_backward("TemporalFocalTransformerBlock")
+        saved = list(ctx.saved_tensors)
+        x = saved.pop(0)
+        params = [saved.pop(0) if h else None for h in ctx.have]
+        keep = ctx.keep
+        ctx.keep = None
+        dx, grads = _block_backward(ctx.mod, keep, x, params, grad, ctx.needs_input_grad[1], ctx.needs_input_grad[3:])
+        return (None, dx, None) + tuple(grads)
+
+
+def _block_backward(mod, keep, x, params, grad, need_x, needs):
+    """The backward of ``TemporalFocalTransformerBlock._forward(x, output_size, keep)`` at the output's gradient grad:
+    (dx or None, the 14 parameter gradients in ``params()`` order, None where ``needs`` is False)."""
+    n1w, n1b, pw, pb, wq, bq, wp, bp, n2w, n2b, w1, b1, w2, b2 = params
+    (nn1w, nn1b, npw, npb, nwq, nbq, nwp, nbp, nn2w, nn2b, nw1, nb1, nw2, nb2) = needs
+    grads = [None] * 14
+    B, T, H, W, C = x.shape
+    need_norm1 = nn1w or nn1b or npw or npb
+    need_rows = need_x or need_norm1                         # [dxn; dpooled]: the attention's input gradient
+    need_dx1 = need_rows or nwq or nbq or nwp or nbp         # the gradient of x1 past LN2 (the attention's output)
+    need_dy = need_dx1 or nn2w or nn2b
+    dy, *grads[10:14] = _ffn_backward(keep["mlp"], grad, w1, w2, need_dy, nw1, nb1, nw2, nb2)
+    if not need_dy:
+        return None, grads
+    dx1, grads[8], grads[9] = ops.layer_norm_backward(keep["x1"].view(-1, C), dy, n2w, mod.norm2.eps,
+                                                      residual=grad.reshape(-1, C), out="both" if need_dx1 else None,
+                                                      need_weight=nn2w, need_bias=nn2b)
+    if not need_dx1:
+        return None, grads
+    dx1_32, dx1_split = dx1
+    drows, grads[4], grads[5], grads[6], grads[7] = _attention_backward(mod.attn, keep["attn"], dx1_split, wq, wp,
+                                                                        x.shape, need_rows, nwq, nbq, nwp, nbp)
+    if not need_rows:
+        return None, grads
+    if mod.attn.uses_pooled:
+        dx, grads[0], grads[1], dpw, grads[3] = ops.layer_norm_pool_backward(
+            x, drows, dx1_32.view(x.shape), n1w, n1b, mod.norm1.eps, pw, mod.window_size, need_x=need_x,
+            need_norm=nn1w or nn1b, need_pool=npw or npb)
+        grads[2] = None if dpw is None else dpw.view(pw.shape)
+    else:
+        dx, grads[0], grads[1] = ops.layer_norm_backward(x.view(-1, C), drows, n1w, mod.norm1.eps, residual=dx1_32,
+                                                         out="f32" if need_x else None, need_weight=nn1w,
+                                                         need_bias=nn1b)
+    grads = [gr if need else None for gr, need in zip(grads, needs)]
+    return (None if dx is None else dx.view(x.shape)), grads

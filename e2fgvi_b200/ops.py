@@ -573,6 +573,98 @@ def layer_norm_pool(x, weight, bias, eps, pool_weight, pool_bias, window_size):
     return SplitMat(hi, lo), n_tok
 
 
+def layer_norm_backward(x, dy, weight, eps=1e-5, residual=None, out="f32", need_weight=True, need_bias=True):
+    """Gradients of ``layer_norm`` (``e2f_layernorm_backward``, C = 512): x the forward's fp32 input, dy the output's
+    gradient, both (..., C) -> ``(dx, dweight, dbias)``.  dx = residual + LN'(x; dy) (``residual`` of x's shape or
+    None) as an fp32 tensor (out="f32"), a ``SplitMat`` ("split"), both ("both") or None (out=None; then a parameter
+    gradient must be asked for).  dweight / dbias (C,) fp32, or None when not asked for — neither: no partial sums."""
+    c = x.shape[-1]
+    if tuple(dy.shape) != tuple(x.shape):
+        raise ValueError(f"layer_norm_backward: dy {tuple(dy.shape)} != x {tuple(x.shape)}")
+    if residual is not None and tuple(residual.shape) != tuple(x.shape):
+        raise ValueError(f"layer_norm_backward: residual {tuple(residual.shape)} != x {tuple(x.shape)}")
+    if c != 512 or tuple(weight.shape) != (c,):
+        raise ValueError(f"layer_norm_backward: 512 channels and a (512,) weight only (x {tuple(x.shape)}, weight "
+                         f"{tuple(weight.shape)})")
+    if out is None and not (need_weight or need_bias):
+        raise ValueError("layer_norm_backward: nothing to compute")
+    _need_cuda(x, dy, weight, residual)
+    o32, hi, lo = _outputs(out, ("f32", "split", "both"), x.shape, x.device) if out is not None else (None, None, None)
+    xc, dyc = x.contiguous().float(), dy.contiguous().float()
+    res = None if residual is None else residual.contiguous().float()
+    rows = xc.numel() // c
+    g32 = weight.detach().float().contiguous()
+    lib = _lib.load()
+    dw = torch.empty(c, dtype=torch.float32, device=x.device) if need_weight else None
+    db = torch.empty(c, dtype=torch.float32, device=x.device) if need_bias else None
+    work = None
+    if need_weight or need_bias:
+        elems = int(lib.e2f_layernorm_backward_work_elems(rows, c))
+        if elems < 0:
+            _lib.check(elems, "e2f_layernorm_backward_work_elems")
+        work = torch.empty(max(elems, 4), dtype=torch.float32, device=x.device)
+    n_out = (o32 is not None) + (hi is not None)
+    with _timed("layernorm_backward", float(xc.numel() * 4 * (2 + (res is not None) + n_out))):
+        st = lib.e2f_layernorm_backward(xc.data_ptr(), dyc.data_ptr(), g32.data_ptr(),
+                                        None if res is None else res.data_ptr(),
+                                        None if o32 is None else o32.data_ptr(), None if hi is None else hi.data_ptr(),
+                                        None if lo is None else lo.data_ptr(), None if dw is None else dw.data_ptr(),
+                                        None if db is None else db.data_ptr(),
+                                        None if work is None else work.data_ptr(), rows, c, float(eps), _stream())
+    _lib.check(st, "e2f_layernorm_backward")
+    dx = None if out is None else _result(out, o32, None if hi is None else SplitMat(hi, lo))
+    return dx, dw, db
+
+
+def layer_norm_pool_backward(x, drows, dx1, weight, bias, eps, pool_weight, window_size, need_x=True, need_norm=True,
+                             need_pool=True):
+    """Gradients of ``layer_norm_pool`` (``e2f_layernorm_pool_backward``): x (B,T,H,W,C) the forward's fp32 input, drows
+    (B*T*H*W + B*T*nWh*nWw, C) fp32 the gradient of its joint output (token rows, then pooled rows ordered
+    (B,T,nWh,nWw)), dx1 (B,T,H,W,C) the gradient x already receives past the LayerNorm (the block's residual).
+    Returns ``(dx, dweight, dbias, dpool_weight (1, wh*ww), dpool_bias (1,))``: dx = dx1 + LN'(x; dxn + w_pool *
+    dpooled) when ``need_x``, the norm's gradients when ``need_norm``, the pooling's when ``need_pool``; None otherwise."""
+    B, T, H, W, C = x.shape
+    wh, ww = window_size
+    if H % wh or W % ww:
+        raise ValueError(f"token grid {H}x{W} must be a multiple of the window {wh}x{ww}")
+    n_tok, n_pool = B * T * H * W, B * T * (H // wh) * (W // ww)
+    if C != 512 or tuple(weight.shape) != (C,) or tuple(bias.shape) != (C,):
+        raise ValueError(f"layer_norm_pool_backward: 512 channels only (x {tuple(x.shape)})")
+    if tuple(drows.shape) != (n_tok + n_pool, C):
+        raise ValueError(f"layer_norm_pool_backward: drows {tuple(drows.shape)} != {(n_tok + n_pool, C)}")
+    if pool_weight.numel() != wh * ww:
+        raise ValueError(f"layer_norm_pool_backward: pool weight has {pool_weight.numel()} entries, the window {wh * ww}")
+    if need_x and (dx1 is None or tuple(dx1.shape) != tuple(x.shape)):
+        raise ValueError(f"layer_norm_pool_backward: dx needs dx1 of x's shape {tuple(x.shape)}")
+    if not (need_x or need_norm or need_pool):
+        raise ValueError("layer_norm_pool_backward: nothing to compute")
+    _need_cuda(x, drows, dx1, weight, bias, pool_weight)
+    xc, dr = x.contiguous().float(), drows.contiguous().float()
+    d1 = dx1.contiguous().float() if need_x else None
+    g32, b32 = weight.detach().float().contiguous(), bias.detach().float().contiguous()
+    pw = pool_weight.detach().float().contiguous()
+    dev = x.device
+    dx = torch.empty((B, T, H, W, C), dtype=torch.float32, device=dev) if need_x else None
+    dw = torch.empty(C, dtype=torch.float32, device=dev) if need_norm else None
+    db = torch.empty(C, dtype=torch.float32, device=dev) if need_norm else None
+    dpw = torch.empty((1, wh * ww), dtype=torch.float32, device=dev) if need_pool else None
+    dpb = torch.empty(1, dtype=torch.float32, device=dev) if need_pool else None
+    lib = _lib.load()
+    work = None
+    if need_norm or need_pool:
+        elems = int(lib.e2f_layernorm_pool_backward_work_elems(B * T, H, W, C, wh, ww))
+        if elems < 0:
+            _lib.check(elems, "e2f_layernorm_pool_backward_work_elems")
+        work = torch.empty(max(elems, 4), dtype=torch.float32, device=dev)
+    ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+    with _timed("layernorm_pool_backward", float(xc.numel() * 4 * (2 + 2 * need_x) + n_pool * C * 4)):
+        st = lib.e2f_layernorm_pool_backward(xc.data_ptr(), g32.data_ptr(), b32.data_ptr(), pw.data_ptr(), dr.data_ptr(),
+                                             ptr(d1), ptr(dx), ptr(dw), ptr(db), ptr(dpw), ptr(dpb), ptr(work), B * T, H,
+                                             W, C, wh, ww, float(eps), _stream())
+    _lib.check(st, "e2f_layernorm_pool_backward")
+    return dx, dw, db, dpw, dpb
+
+
 def t2t_fold(tokens, output_size, kernel_size, stride, padding, normalize=False, bias=None, residual=None,
              channels_last=False):
     """``F.fold(tokens.permute(0, 2, 1), output_size, k, padding=p, stride=s)`` (tfocal_transformer.py:65-72,

@@ -212,6 +212,35 @@ int e2f_upsample2x_split(const float* x, void* out_hi, void* out_lo, int n, int 
 int e2f_layernorm_split(const float* x, const float* gamma, const float* beta, float* out, void* out_hi, void* out_lo,
                         int64_t rows, int c, float eps, void* stream);
 
+/* Backward of e2f_layernorm_split (C = 512): per row, with mean and rstd recomputed from the kept fp32 x in the forward's
+ * order, x^ = (x - mean) * rstd and g = gamma * dy,
+ *   dx = residual + rstd * (g - mean(g) - x^ * mean(g * x^))        (residual [rows][C] fp32 or NULL = 0),
+ * written to dx fp32 [rows][C] and/or its bf16 (dx_hi, dx_lo) split.  dgamma [C] = sum over rows of dy * x^ and dbeta
+ * [C] = sum of dy (either may be NULL; both NULL: no partials).  Every 64 rows leave one partial row of both in `work`
+ * (e2f_layernorm_backward_work_elems(rows, c) floats; NULL allowed when no parameter gradient is asked for), added
+ * in a fixed order by a second launch: no atomics, bit-identical from run to run.  At least one of the outputs. */
+int64_t e2f_layernorm_backward_work_elems(int64_t rows, int c);
+int e2f_layernorm_backward(const float* x, const float* dy, const float* gamma, const float* residual, float* dx,
+                           void* dx_hi, void* dx_lo, float* dgamma, float* dbeta, float* work, int64_t rows, int c,
+                           float eps, void* stream);
+
+/* Backward of e2f_layernorm_pool_split (C = 512, H % wh == W % ww == 0), one CTA per (frame, window):
+ *   drows [(BT*H*W + BT*(H/wh)*(W/ww))][C] fp32: the gradient of the forward's joint output, token rows (dxn) then pooled
+ *         rows (dpooled) ordered (bt, wi, wj);
+ *   dx    [BT][H][W][C] fp32 (or NULL) = dx1 + LN'(x; dxn + pool_w[token] * dpooled[window]), dx1 same shape fp32
+ *         (needed with dx);
+ *   dgamma, dbeta [C]: sums over tokens of dy * x^ and dy with dy = dxn + pool_w * dpooled;
+ *   dpool_w [wh*ww] = sum over frames, windows and channels of dpooled * LN(x)[token] (the fp32 affine LayerNorm output),
+ *   dpool_b [1] = sum of dpooled.
+ * Any of the four parameter gradients may be NULL; each CTA writes one partial row to `work`
+ * (e2f_layernorm_pool_backward_work_elems floats; NULL allowed when no parameter gradient is asked for), added in a fixed
+ * order by a second launch: bit-identical from run to run.  At least one output; bt <= 65535. */
+int64_t e2f_layernorm_pool_backward_work_elems(int bt, int h, int w, int c, int wh, int ww);
+int e2f_layernorm_pool_backward(const float* x, const float* gamma, const float* beta, const float* pool_w,
+                                const float* drows, const float* dx1, float* dx, float* dgamma, float* dbeta,
+                                float* dpool_w, float* dpool_b, float* work, int bt, int h, int w, int c, int wh, int ww,
+                                float eps, void* stream);
+
 /* fp32 -> two-term bf16 split (x = hi + lo, hi = bf16(x), lo = bf16(x - hi)); n must be a multiple of 8. */
 int e2f_split_bf16(const float* x, void* hi_bf16, void* lo_bf16, int64_t n, void* stream);
 
