@@ -22,6 +22,9 @@ SIGNATURES = {
     "e2f_dcn_pack_input": (_i, [_fp, _fp, _vp, _i, _i, _i, _i, _i, _vp]),
     "e2f_deform_align_fused": (_i, [_vp, _fp, _fp, _fp, _vp, _fp, _vp, _i, _i, _i, _i, _i, _i, _f, _i, _i, _vp]),
     "e2f_deform_align_fused_split": (_i, [_vp, _fp, _fp, _fp, _vp, _fp, _fp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _i, _vp]),
+    "e2f_deform_align_backward_work_elems": (_c.c_int64, [_i] * 5),
+    "e2f_deform_align_backward_sample": (_i, [_vp, _fp, _fp, _fp, _fp, _fp, _fp, _vp, _vp, _vp] + [_i] * 5 + [_f, _vp]),
+    "e2f_deform_align_backward_scatter": (_i, [_fp, _vp, _fp] + [_i] * 5 + [_vp]),
     "e2f_focal_window_attention": (_i, [_vp, _vp, _vp] + [_i] * 13 + [_f, _i, _vp]),
     "e2f_focal_window_attention_backward_work_elems": (_c.c_int64, [_i] * 13),
     "e2f_focal_window_attention_backward": (_i, [_vp, _vp, _fp, _fp, _fp, _fp] + [_i] * 13 + [_f, _vp]),

@@ -2,6 +2,7 @@
 // strings, launch accounting, TMA tensor-map encoding.  No torch types, no allocation; the only process-wide state is per-device-ordinal caches
 // of immutable facts (SM count, "function attributes already set on device d", cluster occupancy; launch.h DeviceOnce).
 #include <atomic>
+#include <climits>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -156,6 +157,44 @@ int e2f_deform_align_fused_split(const void* x, const float* head, const float* 
   if (x_layout != E2F_X_NHWC && x_layout != E2F_X_GROUPED) { set_error("%s: x_layout %d", who, x_layout); return E2F_ERR_BAD_ARG; }
   return finish(launch_dcn(x, nullptr, nullptr, head, flow1, flow2, w_packed, bias, out, n, h, w, cin, cout,
                            deform_groups, max_residue, E2F_F32, x_layout, static_cast<cudaStream_t>(stream), out_hi, out_lo), who);
+}
+
+static int dcn_backward_shape_checks(const char* who, int n, int h, int w, int cin, int deform_groups) {
+  if (n < 0 || h <= 0 || w <= 0) { set_error("%s: bad shape n=%d h=%d w=%d", who, n, h, w); return E2F_ERR_BAD_ARG; }
+  if (cin != 256 || deform_groups != 16) { set_error("%s: specialised for Cin=256, deform_groups=16 (got %d, %d)", who, cin, deform_groups); return E2F_ERR_UNSUPPORTED; }
+  if (static_cast<long long>(n) * h * w * 576 > INT_MAX) { set_error("%s: N*H*W=%lld too large (N*H*W*576 must fit in int)", who, static_cast<long long>(n) * h * w); return E2F_ERR_UNSUPPORTED; }
+  return 0;
+}
+
+int64_t e2f_deform_align_backward_work_elems(int n, int h, int w, int cin, int deform_groups) {
+  if (const int st = dcn_backward_shape_checks("e2f_deform_align_backward_work_elems", n, h, w, cin, deform_groups)) return st;
+  return static_cast<int64_t>(dcn_backward_work_elems(n, h, w));
+}
+
+int e2f_deform_align_backward_sample(const void* x, const float* head, const float* flow1, const float* flow2,
+                                     const float* da, float* dhead, float* dflow, void* a_hi, void* a_lo, void* work,
+                                     int n, int h, int w, int cin, int deform_groups, float max_residue, void* stream) {
+  const char* who = "e2f_deform_align_backward_sample";
+  if (!x || !head || !flow1 || !flow2) { set_error("%s: null x/head/flow", who); return E2F_ERR_BAD_ARG; }
+  if ((!a_hi) != (!a_lo)) { set_error("%s: a_hi and a_lo go together", who); return E2F_ERR_BAD_ARG; }
+  if (!dhead && !a_hi && !work) { set_error("%s: nothing to compute (need dhead, a_hi/a_lo or the scatter workspace)", who); return E2F_ERR_BAD_ARG; }
+  if (dhead && !da) { set_error("%s: dhead needs da", who); return E2F_ERR_BAD_ARG; }
+  if (dflow && !dhead) { set_error("%s: dflow goes with dhead", who); return E2F_ERR_BAD_ARG; }
+  if (const int st = dcn_backward_shape_checks(who, n, h, w, cin, deform_groups)) return st;
+  if (!aligned(x, 32) || !aligned(head, 16) || !aligned(flow1, 8) || !aligned(flow2, 8) || (da && !aligned(da, 16)) ||
+      (dhead && !aligned(dhead, 16)) || (dflow && !aligned(dflow, 16)) || (a_hi && (!aligned(a_hi, 16) || !aligned(a_lo, 16))) ||
+      (work && !aligned(work, 256))) { set_error("%s: x needs 32-byte, head / da / dhead / dflow / a 16-byte, flow 8-byte, work 256-byte alignment", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_dcn_sample_backward(x, head, flow1, flow2, da, dhead, dflow, a_hi, a_lo, work, n, h, w, max_residue,
+                                           static_cast<cudaStream_t>(stream)), who);
+}
+
+int e2f_deform_align_backward_scatter(const float* da, void* work, float* dx, int n, int h, int w, int cin,
+                                      int deform_groups, void* stream) {
+  const char* who = "e2f_deform_align_backward_scatter";
+  if (!da || !work || !dx) { set_error("%s: null pointer", who); return E2F_ERR_BAD_ARG; }
+  if (const int st = dcn_backward_shape_checks(who, n, h, w, cin, deform_groups)) return st;
+  if (!aligned(da, 16) || !aligned(dx, 16) || !aligned(work, 256)) { set_error("%s: da / dx need 16-byte, work 256-byte alignment", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_dcn_scatter_backward(da, work, dx, n, h, w, static_cast<cudaStream_t>(stream)), who);
 }
 
 int e2f_focal_window_attention(const void* qkv, const void* qkv_pooled, void* out, int b, int t, int h, int w,

@@ -14,6 +14,7 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include "common.cuh"
+#include "dcn_math.cuh"
 #include "launch.h"
 
 namespace e2f {
@@ -39,12 +40,6 @@ constexpr int TMA_WARP = PRODUCER_WARPS;
 constexpr int THREADS = (PRODUCER_WARPS + 1) * 32;
 constexpr int SMEM_BYTES = STAGES * (A_BYTES + B_BYTES) + 256 + 1024;  // + barriers + alignment slack
 
-__device__ __forceinline__ float fast_tanh(float v) {
-  // 1 - 2/(e^{2v}+1): abs error ~1e-7, saturates cleanly for |v| large
-  const float e = __expf(2.f * v);
-  return 1.f - __fdividef(2.f, e + 1.f);
-}
-__device__ __forceinline__ float fast_sigmoid(float v) { return __fdividef(1.f, 1.f + __expf(-v)); }
 
 // GROUPED: x is [N][G][H][W][16] (group-major; the two horizontally adjacent bilinear corners of a sample are one
 // contiguous 64 B run -> about half the distinct L1 lines per sample of the NHWC layout [N][H][W][256]).

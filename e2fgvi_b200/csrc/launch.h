@@ -79,6 +79,13 @@ int launch_dcn(const void* x, const float* offset, const float* mask, const floa
                void* out_hi = nullptr, void* out_lo = nullptr);   // optional bf16 split of the fp32 result
 int launch_dcn_pack_input(const float* a, const float* b, void* xg, int n, int h, int w, int ca, int cb,
                           cudaStream_t stream);
+// Deformable alignment backward (dcn_grad.cu): the sampler's adjoint (d head / offset part of d flow, the split sample
+// rows A, the dx scatter list in `work`) and the sort + gather of dx; workspace of dcn_backward_work_elems 32-bit words.
+long long dcn_backward_work_elems(int n, int h, int w);
+int launch_dcn_sample_backward(const void* x, const float* head, const float* flow1, const float* flow2, const float* da,
+                               float* dhead, float* dflow, void* a_hi, void* a_lo, void* work, int n, int h, int w,
+                               float max_residue, cudaStream_t stream);
+int launch_dcn_scatter_backward(const float* da, void* work, float* dx, int n, int h, int w, cudaStream_t stream);
 
 int launch_focal_attention(const void* qkv, const void* qkv_pooled, void* out, int b, int t, int h, int w, int heads,
                            int head_dim, int wh, int ww, int eh, int ew, int fh, int fw, int use_pooled, float scale,

@@ -97,9 +97,118 @@ class SecondOrderDeformableAlignment(nn.Module):
                                            self.bias, self.stride, self.padding, self.dilation, self.groups,
                                            self.deform_groups)
 
+    def transposed_weight(self):
+        """bf16 split of W16^T, the weight operand of the backward's dA = dY . W16, cached like ``packed_weight``."""
+        return ops._derived_one(self.weight, ("dcn_t", self.deform_groups),
+                                lambda w, g: ops.dcn_transposed_split(w, g), self.deform_groups)
+
+    def _flows_dgrad_weight(self):
+        """conv_offset.0's weight with 4 zero input channels after the flows' 4: its flows source is read as 8
+        channels (the split pads it), and the input-gradient kernel takes 8-channel sources."""
+        return ops._derived_one(self.conv_offset[0].weight, ("dcn_head_flows8",),
+                                lambda w: F.pad(w.detach().float(), (0, 0, 0, 0, 0, 4)))
+
+    def _params(self):
+        co = self.conv_offset
+        return [self.weight, self.bias] + [t for k in (0, 2, 4, 6) for t in (co[k].weight, co[k].bias)]
+
+    def _forward_keep(self, x, extra_feat, flow_1, flow_2, keep):
+        """``align(x, [extra_feat], flow_1, flow_2)``'s launches, keeping the operands of the backward: the fp16 x,
+        the head convs' split inputs (the LeakyReLU outputs also in fp32, for the activation's derivative), the raw head
+        and the flows.  The same kernels compute the same bits; the head convs also store their fp32 outputs."""
+        co = self.conv_offset
+        if x.dtype != torch.float16 or not ops._is_cl(x):
+            x = x.to(dtype=torch.float16, memory_format=torch.channels_last)
+        srcs = [ops.split_nhwc(extra_feat), ops.split_nhwc(torch.cat([flow_1, flow_2], dim=1))]
+        y1_32, y1 = ops.conv3x3(srcs, co[0].weight, co[0].bias, negative_slope=0.1, out="both")
+        y2_32, y2 = ops.conv3x3([y1], co[2].weight, co[2].bias, negative_slope=0.1, out="both")
+        y3_32, y3 = ops.conv3x3([y2], co[4].weight, co[4].bias, negative_slope=0.1, out="both")
+        head = ops.conv3x3([y3], co[6].weight, co[6].bias)
+        keep.update(x=x, head=head, flow_1=flow_1, flow_2=flow_2, srcs=[srcs, [y1], [y2], [y3]],
+                    acts=[None, y1_32, y2_32, y3_32])
+        return ops.deform_align_fused(x, head, flow_1, flow_2, self.packed_weight(), self.bias, self.deform_groups,
+                                      self.max_residue_magnitude)
+
     def forward(self, x, extra_feat, flow_1, flow_2):
-        """Reference boundary (feat_prop.py:35): extra_feat is the already concatenated condition tensor."""
+        """Reference boundary (feat_prop.py:35): extra_feat is the already concatenated condition tensor.  Under grad
+        mode, with the fused kernel, and when x, extra_feat, a flow or a parameter requires grad, the result carries a
+        ``grad_fn`` (``_AlignGrad``); it is bit-identical to the untracked call."""
+        if self.fused and torch.is_grad_enabled() and (
+                any(t.requires_grad for t in (x, extra_feat, flow_1, flow_2)) or
+                any(p.requires_grad for p in self._params())):
+            return _AlignGrad.apply(self, x, extra_feat, flow_1, flow_2, *self._params())
         return self.align(x, [extra_feat], flow_1, flow_2)
+
+
+def _align_backward(mod, keep, grad, need_in, need):
+    """Gradients of ``SecondOrderDeformableAlignment.forward``.  need_in = (x, extra_feat, flow_1, flow_2) need a
+    gradient; need = the 10 parameters of ``_params()``.  The DCN backward (``ops.deform_align_backward``) gives dx, dW,
+    db and d head with the offsets' share of d flow; the walk down the offset head (convs 6, 4, 2, 0) then runs each
+    conv's weight gradient where needed and its input gradient times LeakyReLU(0.1)'s derivative, and stops at the
+    lowest conv that needs something.  conv 0's flows input gradient adds the offsets' share (its residual).
+    Returns (dx, d extra_feat, d flow_1, d flow_2, *parameter gradients)."""
+    nx, ne, nf1, nf2 = need_in
+    nf = nf1 or nf2
+    head_need = [(need[2 + 2 * i], need[3 + 2 * i]) for i in range(4)]
+    active = [i for i in range(4) if any(head_need[i])]
+    lowest = 0 if (ne or nf) else (active[0] if active else 4)
+    need_head = lowest < 4
+    dx, dhead, dflow, dw, db = ops.deform_align_backward(
+        keep["x"], keep["head"], keep["flow_1"], keep["flow_2"], mod.packed_weight(), grad, mod.deform_groups,
+        mod.max_residue_magnitude, need_x=nx, need_head=need_head, need_flow=nf, need_weight=need[0],
+        need_bias=need[1], wt_split=mod.transposed_weight() if (nx or need_head) else None)
+    grads = [dw, db] + [None] * 8
+    dextra = dflow1 = dflow2 = None
+    if need_head:
+        co = mod.conv_offset
+        convs = [co[0], co[2], co[4], co[6]]
+        srcs, acts = keep["srcs"], keep["acts"]
+        g32 = dhead.permute(0, 2, 3, 1)                       # NHWC, a view
+        gsp = ops.SplitNHWC(*ops.split_bf16(g32), dhead.shape)
+        extra_c = srcs[0][0].shape[1]
+        chans = [extra_c, 4]
+        for i in range(3, lowest - 1, -1):
+            nw_i, nb_i = head_need[i]
+            if nw_i or nb_i:
+                dw_i, db_i = ops.conv3x3_wgrad(g32, srcs[i], with_bias=nb_i, cin=extra_c + 4 if i == 0 else None)
+                grads[2 + 2 * i] = dw_i if nw_i else None
+                grads[3 + 2 * i] = db_i
+            if i > lowest:
+                d = ops.conv_dgrad(gsp, convs[i].weight)
+                g32, gsp = ops.leaky_relu_backward(d, acts[i].permute(0, 2, 3, 1), 0.1, out="both")
+        if ne:
+            dextra = ops.conv_dgrad(gsp, convs[0].weight, src_channels=chans, source=0).permute(0, 3, 1, 2)
+        if nf:
+            d8 = ops.conv_dgrad(gsp, mod._flows_dgrad_weight(), src_channels=[extra_c, 8], source=1, residual=dflow)
+            dflow1 = d8[..., 0:2].permute(0, 3, 1, 2) if nf1 else None
+            dflow2 = d8[..., 2:4].permute(0, 3, 1, 2) if nf2 else None
+    return (dx, dextra, dflow1, dflow2, *grads)
+
+
+class _AlignGrad(torch.autograd.Function):
+    """``SecondOrderDeformableAlignment.forward`` with a backward pass into x, extra_feat, both flows, the DCN weight
+    and bias and the four offset-head convs.  The forward is ``align``'s launch sequence, keeping its operands; the
+    parameters are saved with ``save_for_backward`` (changing one in place before the backward raises autograd's usual
+    error).  The backward frees the kept operands: a second backward (``retain_graph=True``) raises."""
+
+    @staticmethod
+    def forward(ctx, mod, x, extra_feat, flow_1, flow_2, *params):
+        keep = {}
+        out = mod._forward_keep(x, extra_feat, flow_1, flow_2, keep)
+        ctx.mod, ctx.keep = mod, keep
+        ctx.save_for_backward(*params)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        if ctx.keep is None:
+            raise RuntimeError("SecondOrderDeformableAlignment: the backward frees the operands it keeps, so the output "
+                               "cannot be backpropagated a second time (retain_graph=True is not supported); run the "
+                               "forward again")
+        ctx.saved_tensors                       # raises if a parameter was modified in place since the forward
+        grads = _align_backward(ctx.mod, ctx.keep, grad, ctx.needs_input_grad[1:5], ctx.needs_input_grad[5:])
+        ctx.keep = None
+        return (None,) + tuple(grads)
 
 
 class BidirectionalPropagation(nn.Module):

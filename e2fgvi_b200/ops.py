@@ -290,6 +290,101 @@ def deform_align_fused(x, head, flow_1, flow_2, w_packed, bias, deform_groups, m
     return out
 
 
+def dcn_transposed_split(weight, deform_groups):
+    """bf16 (hi, lo) split of W16^T, the packed fp16 DCN weight transposed to (9*Cin, Cout): the weight operand of
+    dA = dY . W16 on ``e2f_linear_bf16x3``.  fp16 is exact as two bf16 terms.  ``weight``: the fp32 (Cout, Cin, 3, 3)
+    parameter or an already packed fp16 (Cout, 9*Cin) operand."""
+    w16 = weight if weight.dtype == torch.float16 and weight.dim() == 2 else pack_dcn_weight(weight, deform_groups)
+    return split_bf16(w16.float().t().contiguous())
+
+
+def deform_align_backward_work_elems(n, h, w, cin=256, deform_groups=16):
+    """32-bit words of the dx scatter workspace of ``deform_align_backward`` (``e2f_deform_align_backward_work_elems``)."""
+    elems = int(_lib.load().e2f_deform_align_backward_work_elems(n, h, w, cin, deform_groups))
+    if elems < 0:
+        _lib.check(elems, "e2f_deform_align_backward_work_elems")
+    return elems
+
+
+def deform_align_backward(x, head, flow_1, flow_2, w_packed, dy, deform_groups=16, max_residue_magnitude=10.0,
+                          need_x=True, need_head=True, need_flow=True, need_weight=True, need_bias=True, wt_split=None):
+    """Gradients of ``deform_align_fused`` (NHWC x) from dy = d loss / d out (n, Cout, h, w):
+
+    1. dA = dY . W16 (fp32 (M, 9*Cin)) on ``e2f_linear_bf16x3`` with ``wt_split`` = ``dcn_transposed_split`` (built from
+       ``w_packed`` when None); dY is split to bf16 once and serves steps 1 and 3.
+    2. the sampler's adjoint (``e2f_deform_align_backward_sample``): d head, the offsets' share of d flow, the split
+       sample rows A and the dx scatter list, each only when asked for.
+    3. dW = dY^T . A and db on ``e2f_linear_wgrad_bf16x3``, unpacked from the sampler's K order to (Cout, Cin, 3, 3).
+    4. dx by sorting the scatter list and gathering each destination in source order
+       (``e2f_deform_align_backward_scatter``).
+
+    x: (n, Cin, h, w) (the forward's fp16 input; converted like the forward does), head: the raw (n, 27*dg, h, w) fp32
+    head, flow_k (n, 2, h, w).  Returns (dx (n, Cin, h, w) fp32 channels_last, d head (n, 27*dg, h, w) fp32
+    channels_last, d flow (n, h, w, 8) fp32 = [d flow_1 (u, v), d flow_2 (u, v), 0 x 4], dW, db), None where not asked
+    for; d flow needs ``need_head``."""
+    _need_cuda(x, head, flow_1, flow_2, w_packed, dy)
+    n, cin, h, w = x.shape
+    cout = w_packed.shape[0]
+    kt = w_packed.shape[1]
+    if tuple(head.shape) != (n, 27 * deform_groups, h, w) or tuple(flow_1.shape) != (n, 2, h, w) or \
+            tuple(flow_2.shape) != (n, 2, h, w) or tuple(dy.shape) != (n, cout, h, w) or kt != 9 * cin:
+        raise ValueError(f"deform_align_backward: shapes x {tuple(x.shape)}, head {tuple(head.shape)}, flows "
+                         f"{tuple(flow_1.shape)} / {tuple(flow_2.shape)}, w_packed {tuple(w_packed.shape)}, dy "
+                         f"{tuple(dy.shape)} do not match")
+    if need_flow and not need_head:
+        raise ValueError("deform_align_backward: the flows' gradient goes with the head's")
+    lib = _lib.load()
+    m = n * h * w
+    if x.dtype != torch.float16 or not _is_cl(x):
+        x = x.to(dtype=torch.float16, memory_format=torch.channels_last)
+    if head.dtype != torch.float32 or not _is_cl(head):
+        head = head.to(dtype=torch.float32, memory_format=torch.channels_last)
+    f1 = flow_1.permute(0, 2, 3, 1).contiguous().float()
+    f2 = flow_2.permute(0, 2, 3, 1).contiguous().float()
+    dy_hi, dy_lo = split_bf16(dy.permute(0, 2, 3, 1).reshape(m, cout))
+    dev = head.device
+    da = None
+    if need_x or need_head:
+        wt_hi, wt_lo = wt_split if wt_split is not None else dcn_transposed_split(w_packed, deform_groups)
+        da = torch.empty((m, kt), dtype=torch.float32, device=dev)
+        with _timed("linear_bf16x3", 2.0 * m * kt * cout):
+            st = lib.e2f_linear_bf16x3(dy_hi.data_ptr(), dy_lo.data_ptr(), wt_hi.data_ptr(), wt_lo.data_ptr(), None, None,
+                                       da.data_ptr(), m, kt, cout, _DT[torch.float32], 0, _stream())
+        _lib.check(st, "e2f_linear_bf16x3")
+    dhead = torch.empty((n, h, w, 27 * deform_groups), dtype=torch.float32, device=dev) if need_head else None
+    dflow = torch.empty((n, h, w, 8), dtype=torch.float32, device=dev) if need_flow else None
+    need_a = need_weight or need_bias
+    a_hi = torch.empty((m, kt), dtype=torch.bfloat16, device=dev) if need_a else None
+    a_lo = torch.empty((m, kt), dtype=torch.bfloat16, device=dev) if need_a else None
+    work = None
+    if need_x:
+        work = torch.empty(deform_align_backward_work_elems(n, h, w, cin, deform_groups), dtype=torch.int32, device=dev)
+    if need_head or need_a or need_x:
+        with _timed("deform_align_backward_sample", float(m * kt * 2 * (need_head * 2 + need_a * 2) + m * 576 * 12 * need_x)):
+            st = lib.e2f_deform_align_backward_sample(
+                x.data_ptr(), head.data_ptr(), f1.data_ptr(), f2.data_ptr(), None if da is None else da.data_ptr(),
+                None if dhead is None else dhead.data_ptr(), None if dflow is None else dflow.data_ptr(),
+                None if a_hi is None else a_hi.data_ptr(), None if a_lo is None else a_lo.data_ptr(),
+                None if work is None else work.data_ptr(), n, h, w, cin, deform_groups, float(max_residue_magnitude),
+                _stream())
+        _lib.check(st, "e2f_deform_align_backward_sample")
+    dw = db = None
+    if need_a:
+        dw, db = linear_wgrad(SplitMat(dy_hi, dy_lo), SplitMat(a_hi, a_lo), with_bias=need_bias, shape=(cout, kt))
+        # packed K order k = (g*9 + tap)*cpg + c  ->  (Cout, Cin, 3, 3)
+        cpg = cin // deform_groups
+        dw = dw.view(cout, deform_groups, 9, cpg).transpose(2, 3).reshape(cout, cin, 3, 3) if need_weight else None
+    dx = None
+    if need_x:
+        dx = torch.empty((n, h, w, cin), dtype=torch.float32, device=dev)
+        with _timed("deform_align_backward_scatter", float(m * 576 * 40)):
+            st = lib.e2f_deform_align_backward_scatter(da.data_ptr(), work.data_ptr(), dx.data_ptr(), n, h, w, cin,
+                                                       deform_groups, _stream())
+        _lib.check(st, "e2f_deform_align_backward_scatter")
+        dx = dx.permute(0, 3, 1, 2)
+    return dx, None if dhead is None else dhead.permute(0, 3, 1, 2), dflow, dw, db
+
+
 def focal_window_attention(qkv, qkv_pooled, num_heads, window_size, expand_size, focal_window, scale,
                            out_dtype=torch.float16):
     """softmax(q k_all^T) v_all of tfocal_transformer.py:226-396, un-partitioned output.

@@ -99,6 +99,26 @@ int e2f_deform_align_fused_split(const void* x, const float* head, const float* 
                                  int h, int w, int cin, int cout, int deform_groups, float max_residue, int x_layout,
                                  void* stream);
 
+/* Backward of e2f_deform_align_fused (NHWC x, Cin = 256, 16 deform groups; E2F_ERR_UNSUPPORTED otherwise), in two calls
+ * around GEMMs the caller runs on e2f_linear_bf16x3 / e2f_linear_wgrad_bf16x3, with M = N*H*W:
+ *   da = dY . W16   fp32 [M][2304] in the packed K order of e2f_dcn_pack_weight (k = (g*9 + tap)*16 + c)
+ * e2f_deform_align_backward_sample recomputes the forward's offsets, masks and bilinear corners and writes, each if
+ * its pointer is not NULL:
+ *   dhead [M][432] fp32   gradient of the raw head (needs da)
+ *   dflow [M][8]   fp32   [d flow_1 (u, v), d flow_2 (u, v), 0 x 4]: the offsets' share of the flows' gradient,
+ *                         summed over each half's 72 sample points in a fixed order (needs dhead)
+ *   a_hi, a_lo [M][2304] bf16: the split of the fp32 samples x mask before the forward's fp16 rounding (the X of dW)
+ *   work                  the dx scatter list, consumed by e2f_deform_align_backward_scatter
+ * e2f_deform_align_backward_scatter sorts the list by destination (stable radix sort) and adds each destination's
+ * coefficient x da terms in source order: dx [N][H][W][256] fp32, bit-identical from run to run, no float atomics.
+ * work: e2f_deform_align_backward_work_elems 32-bit words, 256-byte aligned (negative = bad arguments). */
+int64_t e2f_deform_align_backward_work_elems(int n, int h, int w, int cin, int deform_groups);
+int e2f_deform_align_backward_sample(const void* x, const float* head, const float* flow1, const float* flow2,
+                                     const float* da, float* dhead, float* dflow, void* a_hi, void* a_lo, void* work,
+                                     int n, int h, int w, int cin, int deform_groups, float max_residue, void* stream);
+int e2f_deform_align_backward_scatter(const float* da, void* work, float* dx, int n, int h, int w, int cin,
+                                      int deform_groups, void* stream);
+
 /* Temporal focal window attention core — replaces model/modules/tfocal_transformer.py:226-396 (everything in
  * WindowAttention.forward between the qkv Linear and the proj Linear): window partition of q, the own-window keys,
  * the 4 circularly rolled ring key sets (with their duplicated tokens), the pooled-window keys with the -100
