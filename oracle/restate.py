@@ -358,20 +358,44 @@ def inpaint_generator_forward(sd, masked_frames, num_local_frames, hq=None, taps
     prop_taps = [] if taps is not None else None
     local = bidirectional_propagation(sd, "feat_prop_module", enc[:, :l_t], pred_flows[0], pred_flows[1], prop_taps)
     enc = torch.cat((local, enc[:, l_t:]), dim=1)
-    # SoftSplit (tfocal_transformer.py:39-46)
-    f_h, f_w = (h + 6 - 7) // 3 + 1, (w + 6 - 7) // 3 + 1
-    tok = F.unfold(enc.reshape(-1, c, h, w), (7, 7), padding=(3, 3), stride=(3, 3)).permute(0, 2, 1)
-    tok = _linear(sd, "ss.embedding", tok).view(b, -1, f_h, f_w, 512)
     blk_taps = [] if taps is not None else None
-    for i in range(8):
-        tok = transformer_block(sd, f"transformer.{i}", tok, (h, w), taps=blk_taps)
-    # SoftComp (tfocal_transformer.py:65-72; HQ _hq.py:67-79)
-    feat = _linear(sd, "sc.embedding", tok.view(b, -1, 512))
-    feat = feat.view(b * t, -1, feat.size(2)).permute(0, 2, 1)
-    feat = F.fold(feat, (h, w), (7, 7), padding=(3, 3), stride=(3, 3))
-    feat = _conv(sd, "sc.bias_conv", feat) if hq else feat + sd["sc.bias"][None]
-    enc = enc + feat.view(b, t, -1, h, w)
+    tok = transformer(sd, soft_split(sd, enc.reshape(-1, c, h, w), b), (h, w), blk_taps)
+    enc = enc + soft_comp(sd, tok, t, (h, w), hq).view(b, t, -1, h, w)
     out = torch.tanh(decoder(sd, enc.reshape(b * t, c, h, w)))
     if taps is not None:
         taps.update({"propagation": prop_taps, "blocks": blk_taps, "local_feat": local, "tokens": tok})
     return out, pred_flows
+
+
+def soft_split(sd, x, b):
+    """SoftSplit.forward, tfocal_transformer.py:39-46 (HQ _hq.py:32-46): x (b*t, c, h, w) -> tokens (b, t, fh, fw, 512)."""
+    h, w = x.shape[-2:]
+    f_h, f_w = (h + 6 - 7) // 3 + 1, (w + 6 - 7) // 3 + 1
+    tok = F.unfold(x, (7, 7), padding=(3, 3), stride=(3, 3)).permute(0, 2, 1)
+    return _linear(sd, "ss.embedding", tok).view(b, -1, f_h, f_w, 512)
+
+
+def transformer(sd, tok, output_size, taps=None):
+    """The eight TemporalFocalTransformerBlocks (e2fgvi.py:188-198, :255)."""
+    for i in range(8):
+        tok = transformer_block(sd, f"transformer.{i}", tok, output_size, taps=taps)
+    return tok
+
+
+def soft_comp(sd, tok, t, output_size, hq):
+    """SoftComp.forward, tfocal_transformer.py:65-72 (HQ _hq.py:67-79): tokens (b, t, fh, fw, 512) -> (b*t, c, h, w)."""
+    b = tok.shape[0]
+    feat = _linear(sd, "sc.embedding", tok.reshape(b, -1, 512))
+    feat = feat.view(b * t, -1, feat.size(2)).permute(0, 2, 1)
+    feat = F.fold(feat, output_size, (7, 7), padding=(3, 3), stride=(3, 3))
+    return _conv(sd, "sc.bias_conv", feat) if hq else feat + sd["sc.bias"][None]
+
+
+def generator_trunk(sd, frames, b, t, hq):
+    """tanh(decoder(enc + sc(transformer(ss(enc, b)), t))) with enc = encoder(frames): InpaintGenerator.forward
+    (e2fgvi.py:245-263, HQ e2fgvi_hq.py) with the flow completion and the propagation left out (the propagation taken
+    as the identity).  frames (b*t, 3, H, W) -> prediction (b*t, 3, H, W)."""
+    enc = encoder(sd, frames)
+    h, w = enc.shape[-2:]
+    tok = transformer(sd, soft_split(sd, enc, b), (h, w))
+    return torch.tanh(decoder(sd, enc + soft_comp(sd, tok, t, (h, w), hq)))
