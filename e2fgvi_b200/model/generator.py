@@ -13,6 +13,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from .. import ops
+from ._kept import KeptLaunches, tracked
 from .modules.flow_comp import SPyNet
 from .modules.feat_prop import BidirectionalPropagation, SecondOrderDeformableAlignment
 from .modules.tfocal_transformer import SoftComp, SoftSplit, TemporalFocalTransformerBlock
@@ -82,16 +83,16 @@ class Encoder(nn.Module):
         bf16 (hi, lo) split of the features (operand of the propagation convs and of SoftSplit).
 
         Trainable: with grad mode on, the default ``last_out`` and some encoder parameter requiring grad, the features
-        carry a ``grad_fn`` whose backward gives the parameters that require grad their gradients (``_EncoderGrad``);
-        the features are bit-identical to the untracked call.  Frames that require grad raise ``ValueError`` (no
-        gradient into the frames).  Other ``last_out`` values stay untracked."""
-        if last_out == "f32" and torch.is_grad_enabled():
+        carry a ``grad_fn`` whose backward gives the parameters that require grad their gradients
+        (``_encoder_backward``); the features are bit-identical to the untracked call.  Frames that require grad raise
+        ``ValueError`` (no gradient into the frames).  Other ``last_out`` values stay untracked."""
+        if last_out == "f32":
             params = [t for conv in self.layers[::2] for t in (conv.weight, conv.bias)]
-            if any(p.requires_grad for p in params):
+            if tracked((), params):
                 if x.requires_grad:
                     raise ValueError("Encoder: the gradient with respect to the frames is not implemented (detach them; "
                                      "the features' gradient reaches the encoder's parameters)")
-                return _EncoderGrad.apply(self, x, *params)
+                return KeptLaunches.apply("Encoder", _encoder_run, _encoder_backward, self, x, *params)
         return self._forward(x, last_out)
 
     def _forward(self, x, last_out="f32", keep=None):
@@ -123,17 +124,28 @@ class Encoder(nn.Module):
         return out
 
 
-def _encoder_backward(enc, frames, keep, feat, grad, need):
-    """Gradients of the encoder's parameters from ``grad`` = d loss / d features (N, 128, h, w).  need[k] = (weight,
-    bias) of conv k need a gradient.  Convs 8 -> 0: LeakyReLU's derivative at each conv's output is fused into the
-    input gradient that produces that output's gradient; x0 (conv 3's output, read by convs 4-8) collects the
-    contributions of convs 8, 7, 6, 5 through the residual epilogue, and conv 4's input gradient adds its own and
-    applies the derivative: (acc4 + (acc5 + (acc6 + (acc7 + acc8)))) * LeakyReLU'(x0).  The walk stops at the lowest
-    conv with a trainable parameter.  Returns [dW0, db0, dW1, ...] (None where not needed)."""
+def _encoder_run(keep, enc, frames, *params):
+    """``Encoder.forward``'s tracked launches: ``_forward`` keeping each conv's input operands; saves the frames, the
+    features and the 18 parameters."""
+    keep["enc"], keep["inputs"] = enc, []
+    feat = enc._forward(frames, "f32", keep["inputs"])
+    return feat, (frames, feat, *params)
+
+
+def _encoder_backward(keep, saved, needs, grad):
+    """Gradients of the encoder's parameters from ``grad`` = d loss / d features (N, 128, h, w).  Convs 8 -> 0:
+    LeakyReLU's derivative at each conv's output is fused into the input gradient that produces that output's
+    gradient; x0 (conv 3's output, read by convs 4-8) collects the contributions of convs 8, 7, 6, 5 through the
+    residual epilogue, and conv 4's input gradient adds its own and applies the derivative:
+    (acc4 + (acc5 + (acc6 + (acc7 + acc8)))) * LeakyReLU'(x0).  The walk stops at the lowest conv with a trainable
+    parameter.  Returns (None, None, dW0, db0, dW1, ...) (None where not needed)."""
+    enc, inputs = keep["enc"], keep["inputs"]
+    frames, feat = saved[:2]
+    need = list(zip(needs[2::2], needs[3::2]))         # (weight, bias) of conv k need a gradient
     grads = [None] * (2 * len(_ENC))
     active = [k for k in range(len(_ENC)) if any(need[k])]
     if not active:
-        return grads
+        return (None, None, *grads)
     lowest = active[0]
     convs = [enc.layers[2 * k] for k in range(len(_ENC))]
     g = grad.permute(0, 2, 3, 1)                 # NHWC, a view for channels_last gradients
@@ -145,7 +157,7 @@ def _encoder_backward(enc, frames, keep, feat, grad, need):
         conv = convs[k]
         nw, nb = need[k]
         if nw or nb:
-            srcs = [ops.pack_rows(frames, lead=1, cin=8)] if k == 0 else keep[k]   # 8-channel copy of the frames
+            srcs = [ops.pack_rows(frames, lead=1, cin=8)] if k == 0 else inputs[k]   # 8-channel copy of the frames
             dw, db = ops.conv3x3_wgrad(dy32, srcs, groups=groups, stride=stride, with_bias=nb,
                                        cin=cin // groups)
             grads[2 * k] = dw if nw else None
@@ -156,40 +168,13 @@ def _encoder_backward(enc, frames, keep, feat, grad, need):
             chans = [x0_c, cin - x0_c]
             if lowest <= 3:
                 dx0 = ops.conv_dgrad(dy, conv.weight, groups=groups, src_channels=chans, source=0, residual=dx0)
-            dy32, dy = ops.conv_dgrad(dy, conv.weight, groups=groups, src_channels=chans, source=1, act=keep[k][1],
+            dy32, dy = ops.conv_dgrad(dy, conv.weight, groups=groups, src_channels=chans, source=1, act=inputs[k][1],
                                       out="both")
         else:
-            src = keep[k][0]
+            src = inputs[k][0]
             dy32, dy = ops.conv_dgrad(dy, conv.weight, stride=stride, in_size=src.shape[2:], act=src,
                                       residual=dx0 if k == 4 else None, out="both")
-    return grads
-
-
-class _EncoderGrad(torch.autograd.Function):
-    """``Encoder.forward`` with a backward pass into the encoder's 18 parameters.  The forward is the inference launch
-    sequence, keeping the split operands it produces; the parameters are saved with ``save_for_backward`` (changing one
-    in place before the backward raises autograd's usual error).  The backward frees the kept operands: a second
-    backward (``retain_graph=True``) raises."""
-
-    @staticmethod
-    def forward(ctx, enc, frames, *params):
-        keep = []
-        feat = enc._forward(frames, "f32", keep)
-        ctx.enc, ctx.keep = enc, keep
-        ctx.save_for_backward(frames, feat, *params)
-        return feat
-
-    @staticmethod
-    def backward(ctx, grad):
-        if ctx.keep is None:
-            raise RuntimeError("Encoder: the backward frees the operands it keeps, so the features cannot be "
-                               "backpropagated a second time (retain_graph=True is not supported); run the forward again")
-        frames, feat = ctx.saved_tensors[:2]        # raises if a parameter was modified in place since the forward
-        needs = ctx.needs_input_grad[2:]
-        need = [(needs[2 * k], needs[2 * k + 1]) for k in range(len(_ENC))]
-        grads = _encoder_backward(ctx.enc, frames, ctx.keep, feat, grad, need)
-        ctx.keep = None
-        return (None, None) + tuple(grads)
+    return (None, None, *grads)
 
 
 class deconv(nn.Module):
@@ -252,8 +237,7 @@ class InpaintGenerator(BaseNetwork):
         ``forward(masked_frames, l_t)[1]`` bit for bit when masked_local_frames = (masked_frames[:, :l_t] + 1) / 2.
         Frames that require grad raise ``ValueError`` there (no gradient into the frames)."""
         b, l_t, c, h, w = masked_local_frames.size()
-        if (masked_local_frames.is_cuda and l_t > 1 and torch.is_grad_enabled()
-                and any(p.requires_grad for p in self.update_spynet.parameters())):
+        if masked_local_frames.is_cuda and l_t > 1 and tracked((), self.update_spynet.parameters()):
             return self.update_spynet.bidirect_flows(masked_local_frames, l_t, unit=True)
         small = F.interpolate(masked_local_frames.reshape(-1, c, h, w), scale_factor=1 / 4, mode="bilinear",
                               align_corners=True, recompute_scale_factor=True)
@@ -381,10 +365,10 @@ class InpaintGenerator(BaseNetwork):
     def decode(self, feat):
         """``tanh(self.decoder(feat))``, the decoder step of e2fgvi.py:262: feat (N, 128, h, w) -> prediction (N, 3, 4h, 4w)
         fp32, on ``_decode``'s kernel sequence.  With grad mode on and ``feat`` or some decoder parameter requiring
-        grad, the prediction carries a ``grad_fn`` into both (``_DecodeGrad``); its values are the same bits."""
+        grad, the prediction carries a ``grad_fn`` into both (``_decode_backward``); its values are the same bits."""
         params = self._decoder_params()
-        if torch.is_grad_enabled() and (feat.requires_grad or any(p.requires_grad for p in params)):
-            return _DecodeGrad.apply(self, feat, *params)
+        if tracked([feat], params):
+            return KeptLaunches.apply("decode", _decode_run, _decode_backward, self, feat, *params)
         return self._decode(feat)
 
     def _decoder_params(self):
@@ -406,20 +390,30 @@ class InpaintGenerator(BaseNetwork):
         return ops.conv3x3_tanh_nchw(y3, d[6].weight, d[6].bias)
 
 
-def _decode_backward(gen, keep, pred, grad, need, want_feat):
-    """Gradients of ``decode``: need[i] = (weight, bias) of decoder conv i (decoder[0].conv, [2], [4].conv, [6]) need a
-    gradient, ``want_feat`` the input's.  tanh's derivative feeds the output conv's gradients; each input gradient
-    fuses LeakyReLU's derivative at the activation it reaches (after the upsample adjoint for the deconvs).  Returns
-    ([dW0, db0, ...], d feat (N, 128, h, w) or None)."""
-    d = gen.decoder
+def _decode_run(keep, gen, feat, *params):
+    """``decode``'s tracked launches: ``_decode`` keeping its operands; saves the prediction and the 8 parameters."""
+    keep["gen"], keep["ops"] = gen, []
+    pred = gen._decode(feat, keep["ops"])
+    return pred, (pred, *params)
+
+
+def _decode_backward(keep, saved, needs, grad):
+    """Gradients of ``decode`` into the features and the decoder convs (decoder[0].conv, [2], [4].conv, [6]).  tanh's
+    derivative feeds the output conv's gradients; each input gradient fuses LeakyReLU's derivative at the activation it
+    reaches (after the upsample adjoint for the deconvs).  Returns (None, d feat (N, 128, h, w), dW0, db0, ...), None
+    where not needed."""
+    d = keep["gen"].decoder
+    pred = saved[0]
+    want_feat = needs[1]
+    need = list(zip(needs[2::2], needs[3::2]))         # (weight, bias) of decoder conv i need a gradient
     convs = (d[0].conv, d[2], d[4].conv, d[6])
-    u0, y1, y2, u1, y3 = keep
+    u0, y1, y2, u1, y3 = keep["ops"]
     srcs = (u0, y1, u1, y3)
     grads = [None] * 8
     active = [i for i in range(4) if any(need[i])]
     lowest = 0 if want_feat else (active[0] if active else 4)
     if lowest == 4:
-        return grads, None
+        return (None, None, *grads)
     dy32, dy = ops.tanh_backward_rows(grad, pred, lead=1)
     cout = convs[3].out_channels
     dfeat = None
@@ -437,32 +431,7 @@ def _decode_backward(gen, keep, pred, grad, need, want_feat):
             dy32, dy = ops.conv_dgrad(dy, convs[1].weight, act=y1, out="both")
         elif i == 0 and want_feat:
             dfeat = ops.upsample2x_backward(ops.conv_dgrad(dy, convs[0].weight)).permute(0, 3, 1, 2)
-    return grads, dfeat
-
-
-class _DecodeGrad(torch.autograd.Function):
-    """``InpaintGenerator.decode`` with a backward pass into the four decoder convs and the features.  The forward is
-    ``_decode``'s launch sequence, keeping its operands; the backward frees them (no ``retain_graph``)."""
-
-    @staticmethod
-    def forward(ctx, gen, feat, *params):
-        keep = []
-        pred = gen._decode(feat, keep)
-        ctx.gen, ctx.keep = gen, keep
-        ctx.save_for_backward(pred, *params)
-        return pred
-
-    @staticmethod
-    def backward(ctx, grad):
-        if ctx.keep is None:
-            raise RuntimeError("decode: the backward frees the operands it keeps, so the prediction cannot be "
-                               "backpropagated a second time (retain_graph=True is not supported); run the forward again")
-        pred = ctx.saved_tensors[0]                # raises if a parameter was modified in place since the forward
-        needs = ctx.needs_input_grad[2:]
-        need = [(needs[2 * i], needs[2 * i + 1]) for i in range(4)]
-        grads, dfeat = _decode_backward(ctx.gen, ctx.keep, pred, grad, need, ctx.needs_input_grad[1])
-        ctx.keep = None
-        return (None, dfeat) + tuple(grads)
+    return (None, dfeat, *grads)
 
 
 class InpaintGeneratorHQ(InpaintGenerator):

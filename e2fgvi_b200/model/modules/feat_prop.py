@@ -15,6 +15,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ... import ops
+from .._kept import KeptLaunches, tracked
 from .flow_comp import flow_warp
 
 
@@ -132,12 +133,24 @@ class SecondOrderDeformableAlignment(nn.Module):
     def forward(self, x, extra_feat, flow_1, flow_2):
         """Reference boundary (feat_prop.py:35): extra_feat is the already concatenated condition tensor.  Under grad
         mode, with the fused kernel, and when x, extra_feat, a flow or a parameter requires grad, the result carries a
-        ``grad_fn`` (``_AlignGrad``); it is bit-identical to the untracked call."""
-        if self.fused and torch.is_grad_enabled() and (
-                any(t.requires_grad for t in (x, extra_feat, flow_1, flow_2)) or
-                any(p.requires_grad for p in self._params())):
-            return _AlignGrad.apply(self, x, extra_feat, flow_1, flow_2, *self._params())
+        ``grad_fn`` into all of them (``_align_backward``); it is bit-identical to the untracked call."""
+        params = self._params()
+        if self.fused and tracked((x, extra_feat, flow_1, flow_2), params):
+            return KeptLaunches.apply("SecondOrderDeformableAlignment", _align_run, _align_back, self, x, extra_feat,
+                                      flow_1, flow_2, *params)
         return self.align(x, [extra_feat], flow_1, flow_2)
+
+
+def _align_run(keep, mod, x, extra_feat, flow_1, flow_2, *params):
+    """The tracked launches of ``SecondOrderDeformableAlignment.forward`` (``_forward_keep``); saves the 10
+    parameters."""
+    keep["mod"] = mod
+    return mod._forward_keep(x, extra_feat, flow_1, flow_2, keep), params
+
+
+def _align_back(keep, saved, needs, grad):
+    """``_align_backward`` for ``_align_run``."""
+    return (None, *_align_backward(keep["mod"], keep, grad, needs[1:5], needs[5:]))
 
 
 def _align_backward(mod, keep, grad, need_in, need):
@@ -183,32 +196,6 @@ def _align_backward(mod, keep, grad, need_in, need):
             dflow1 = d8[..., 0:2].permute(0, 3, 1, 2) if nf1 else None
             dflow2 = d8[..., 2:4].permute(0, 3, 1, 2) if nf2 else None
     return (dx, dextra, dflow1, dflow2, *grads)
-
-
-class _AlignGrad(torch.autograd.Function):
-    """``SecondOrderDeformableAlignment.forward`` with a backward pass into x, extra_feat, both flows, the DCN weight
-    and bias and the four offset-head convs.  The forward is ``align``'s launch sequence, keeping its operands; the
-    parameters are saved with ``save_for_backward`` (changing one in place before the backward raises autograd's usual
-    error).  The backward frees the kept operands: a second backward (``retain_graph=True``) raises."""
-
-    @staticmethod
-    def forward(ctx, mod, x, extra_feat, flow_1, flow_2, *params):
-        keep = {}
-        out = mod._forward_keep(x, extra_feat, flow_1, flow_2, keep)
-        ctx.mod, ctx.keep = mod, keep
-        ctx.save_for_backward(*params)
-        return out
-
-    @staticmethod
-    def backward(ctx, grad):
-        if ctx.keep is None:
-            raise RuntimeError("SecondOrderDeformableAlignment: the backward frees the operands it keeps, so the output "
-                               "cannot be backpropagated a second time (retain_graph=True is not supported); run the "
-                               "forward again")
-        ctx.saved_tensors                       # raises if a parameter was modified in place since the forward
-        grads = _align_backward(ctx.mod, ctx.keep, grad, ctx.needs_input_grad[1:5], ctx.needs_input_grad[5:])
-        ctx.keep = None
-        return (None,) + tuple(grads)
 
 
 class BidirectionalPropagation(nn.Module):

@@ -18,6 +18,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ... import ops
+from .._kept import KeptLaunches, tracked
 
 # (cin, cout) of the five 7x7 convs of one pyramid level, ReLU after all but the last (flow_comp.py:181-215)
 _LEVEL_CONVS = ((8, 32), (32, 64), (64, 32), (32, 16), (16, 2))
@@ -120,53 +121,40 @@ def _level_backward(module, keep, dflow, need, conv_lo, want_input):
     return grads, None
 
 
-class _BidirectFlows(torch.autograd.Function):
-    """``SPyNet.bidirect_flows`` with a backward pass into SPyNet's 60 parameters.  The forward is the inference
-    sequence (the same kernels and operands), keeping the operands for the backward; the backward walks the levels from
-    fine to coarse and stops below the coarsest level with a parameter that needs a gradient.  The parameters are saved
-    with ``save_for_backward``, so that changing one in place between forward and backward (an ``optimizer.step()``)
-    raises autograd's usual error instead of giving the gradient of the new weights.  The backward frees the kept
-    operands: a second backward (``retain_graph=True``) raises."""
+def _flows_run(keep, spynet, frames, num_local_frames, unit, *params):
+    """``SPyNet.bidirect_flows``'s tracked launches: the inference sequence (the same kernels and operands), keeping
+    each level's operands; saves the 60 parameters."""
+    keep["spynet"], keep["levels"] = spynet, []
+    return spynet._bidirect_flows(frames, num_local_frames, unit, keep["levels"]), params
 
-    @staticmethod
-    def forward(ctx, spynet, frames, num_local_frames, unit, *params):
-        levels = []
-        fwd, bwd = spynet._bidirect_flows(frames, num_local_frames, unit, levels)
-        ctx.spynet, ctx.levels = spynet, levels
-        ctx.save_for_backward(*params)
-        return fwd, bwd
 
-    @staticmethod
-    def backward(ctx, d_forward, d_backward):
-        spynet, levels = ctx.spynet, ctx.levels
-        if levels is None:
-            raise RuntimeError("SPyNet.bidirect_flows: the backward frees the operands it keeps, so the flows cannot be "
-                               "backpropagated a second time (retain_graph=True is not supported); run the forward again")
-        ctx.saved_tensors                       # raises if a parameter was modified in place since the forward
-        needs = ctx.needs_input_grad[4:]
-        n_conv = len(_LEVEL_CONVS)
-        need = [[(needs[2 * (lv * n_conv + i)], needs[2 * (lv * n_conv + i) + 1]) for i in range(n_conv)]
-                for lv in range(_NUM_LEVELS)]
-        active = [lv for lv in range(_NUM_LEVELS) if any(a or b for a, b in need[lv])]
-        grads = [None] * (2 * _NUM_LEVELS * n_conv)
-        if not active:
-            return (None, None, None, None) + tuple(grads)
-        lowest = active[0]
-        pyr = levels[0][0]
-        dflow = ops.spynet_final_backward(d_forward, d_backward, pyr)
-        for lv in range(_NUM_LEVELS - 1, lowest - 1, -1):
-            _, keep, flow_up = levels[lv]
-            if lv > lowest:
-                conv_lo, want_input = 0, True
-            else:
-                conv_lo, want_input = min(i for i in range(n_conv) if any(need[lv][i])), False
-            g, d_in = _level_backward(spynet.basic_module[lv], keep, dflow, need[lv], conv_lo, want_input)
-            for (i, kind), v in g.items():
-                grads[2 * (lv * n_conv + i) + (kind == "bias")] = v
-            if want_input:
-                dflow = ops.spynet_level_input_backward(d_in, dflow, pyr, _NUM_LEVELS - 1 - lv, flow_up)
-        ctx.levels = None
-        return (None, None, None, None) + tuple(grads)
+def _flows_backward(keep, saved, needs, d_forward, d_backward):
+    """Gradients of SPyNet's parameters from the flows' gradients: walks the levels from fine to coarse and stops below
+    the coarsest level with a parameter that needs a gradient.  Returns (None, None, None, None, dW, db, ...) in
+    ``_flow_params`` order, None where not needed."""
+    spynet, levels = keep["spynet"], keep["levels"]
+    n_conv = len(_LEVEL_CONVS)
+    pairs = list(zip(needs[4::2], needs[5::2]))
+    need = [pairs[lv * n_conv:(lv + 1) * n_conv] for lv in range(_NUM_LEVELS)]
+    active = [lv for lv in range(_NUM_LEVELS) if any(a or b for a, b in need[lv])]
+    grads = [None] * (2 * _NUM_LEVELS * n_conv)
+    if not active:
+        return (None, None, None, None, *grads)
+    lowest = active[0]
+    pyr = levels[0][0]
+    dflow = ops.spynet_final_backward(d_forward, d_backward, pyr)
+    for lv in range(_NUM_LEVELS - 1, lowest - 1, -1):
+        _, kept, flow_up = levels[lv]
+        if lv > lowest:
+            conv_lo, want_input = 0, True
+        else:
+            conv_lo, want_input = min(i for i in range(n_conv) if any(need[lv][i])), False
+        g, d_in = _level_backward(spynet.basic_module[lv], kept, dflow, need[lv], conv_lo, want_input)
+        for (i, kind), v in g.items():
+            grads[2 * (lv * n_conv + i) + (kind == "bias")] = v
+        if want_input:
+            dflow = ops.spynet_level_input_backward(d_in, dflow, pyr, _NUM_LEVELS - 1 - lv, flow_up)
+    return (None, None, None, None, *grads)
 
 
 class SPyNet(nn.Module):
@@ -204,13 +192,15 @@ class SPyNet(nn.Module):
         7x7 convs, 1 final launch.  Returns (flows_forward, flows_backward), each (b, l_t-1, 2, H/4, W/4).
 
         With grad mode on and some SPyNet parameter requiring grad, the flows carry a ``grad_fn`` whose backward gives
-        those parameters their gradients (not the frames': frames that require grad raise ``ValueError``)."""
+        those parameters their gradients (``_flows_backward``; not the frames': frames that require grad raise
+        ``ValueError``)."""
         params = self._flow_params()
-        if torch.is_grad_enabled() and any(p.requires_grad for p in params):
+        if tracked((), params):
             if masked_frames.requires_grad:
                 raise ValueError("SPyNet.bidirect_flows: the gradient with respect to the frames is not implemented "
                                  "(detach them; the flows' gradient reaches SPyNet's parameters)")
-            return _BidirectFlows.apply(self, masked_frames, num_local_frames, unit, *params)
+            return KeptLaunches.apply("SPyNet.bidirect_flows", _flows_run, _flows_backward, self, masked_frames,
+                                      num_local_frames, unit, *params)
         return self._bidirect_flows(masked_frames, num_local_frames, unit)
 
     def _flow_params(self):

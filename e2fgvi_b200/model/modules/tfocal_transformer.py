@@ -16,21 +16,11 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ... import ops
+from .._kept import KeptLaunches, tracked
 
 
 def _token_grid(output_size, kernel_size, stride, padding):
     return tuple((output_size[i] + 2 * padding[i] - (kernel_size[i] - 1) - 1) // stride[i] + 1 for i in range(2))
-
-
-def _tracked(inputs, params):
-    """Grad mode is on and a tensor input or a parameter requires grad: the call gets a ``grad_fn``."""
-    return torch.is_grad_enabled() and (any(isinstance(t, torch.Tensor) and t.requires_grad for t in inputs)
-                                        or any(p.requires_grad for p in params))
-
-
-def _second_backward(what):
-    return RuntimeError(f"{what}: the backward frees the operands it keeps, so the output cannot be backpropagated a "
-                        "second time (retain_graph=True is not supported); run the forward again")
 
 
 class SoftSplit(nn.Module):
@@ -45,48 +35,42 @@ class SoftSplit(nn.Module):
 
     def forward(self, x, b, output_size=None):
         """x (BT, C, H, W) fp32 (or the encoder's ``SplitNHWC``) -> tokens (b, T, fh, fw, hidden).  Trainable
-        (``_SoftSplitGrad``) when grad mode is on and the tensor x or a parameter requires grad; the tokens are the same
-        bits as the untracked call."""
+        (``_soft_split_backward``) when grad mode is on and the tensor x or a parameter requires grad; the tokens are
+        the same bits as the untracked call."""
         output_size = output_size or self.output_size
         f_h, f_w = _token_grid(output_size, self.kernel_size, self.stride, self.padding)
         params = (self.embedding.weight, self.embedding.bias)
-        if isinstance(x, torch.Tensor) and _tracked([x], params):
-            feat = _SoftSplitGrad.apply(self, x, *params)
+        if isinstance(x, torch.Tensor) and tracked([x], params):
+            feat = KeptLaunches.apply("SoftSplit", _soft_split_run, _soft_split_backward, self, x, *params)
         else:
             # unfold + Linear == a 7x7 / stride-3 conv: one implicit-GEMM launch, the 49x unfolded operand never exists
             feat = ops.soft_split(x, *params, self.kernel_size, self.stride, self.padding)
         return feat.view(b, -1, f_h, f_w, feat.size(2))
 
 
-class _SoftSplitGrad(torch.autograd.Function):
-    """``SoftSplit``'s launch with a backward into ``embedding`` and x: dW = dT^T . unfold(x) (the unfold materialised as
-    a split operand), db = the sum of dT, dx = fold(dT . W) on ``soft_comp``'s transposed-conv launch with W^T."""
+def _soft_split_run(keep, mod, x, weight, bias):
+    """``SoftSplit``'s launch; saves x, weight and bias."""
+    keep["mod"] = mod
+    return ops.soft_split(x, weight, bias, mod.kernel_size, mod.stride, mod.padding), (x, weight, bias)
 
-    @staticmethod
-    def forward(ctx, mod, x, weight, bias):
-        ctx.mod, ctx.live = mod, True
-        ctx.save_for_backward(x, weight, bias)
-        return ops.soft_split(x, weight, bias, mod.kernel_size, mod.stride, mod.padding)
 
-    @staticmethod
-    def backward(ctx, grad):
-        if not ctx.live:
-            raise _second_backward("SoftSplit")
-        x, weight, bias = ctx.saved_tensors
-        ctx.live = False
-        mod = ctx.mod
-        n, c, h, w = x.shape
-        _, need_x, need_w, need_b = ctx.needs_input_grad
-        dx = dw = db = None
-        if need_w or need_b:
-            cols = ops.t2t_unfold(x, mod.kernel_size, mod.stride, mod.padding, out="split")
-            dw, db = ops.linear_wgrad(grad, cols, with_bias=need_b)
-            dw = dw if need_w else None
-        if need_x:
-            fh, fw = _token_grid((h, w), mod.kernel_size, mod.stride, mod.padding)
-            dx = ops.soft_comp(grad.reshape(n, fh, fw, -1), weight, None, (h, w), mod.kernel_size, mod.stride,
-                               mod.padding, transpose=True)
-        return None, dx, dw, db
+def _soft_split_backward(keep, saved, needs, grad):
+    """The backward into ``embedding`` and x: dW = dT^T . unfold(x) (the unfold materialised as a split operand),
+    db = the sum of dT, dx = fold(dT . W) on ``soft_comp``'s transposed-conv launch with W^T."""
+    mod = keep["mod"]
+    x, weight, bias = saved
+    n, c, h, w = x.shape
+    _, need_x, need_w, need_b = needs
+    dx = dw = db = None
+    if need_w or need_b:
+        cols = ops.t2t_unfold(x, mod.kernel_size, mod.stride, mod.padding, out="split")
+        dw, db = ops.linear_wgrad(grad, cols, with_bias=need_b)
+        dw = dw if need_w else None
+    if need_x:
+        fh, fw = _token_grid((h, w), mod.kernel_size, mod.stride, mod.padding)
+        dx = ops.soft_comp(grad.reshape(n, fh, fw, -1), weight, None, (h, w), mod.kernel_size, mod.stride,
+                           mod.padding, transpose=True)
+    return None, dx, dw, db
 
 
 class SoftComp(nn.Module):
@@ -104,19 +88,20 @@ class SoftComp(nn.Module):
             self.bias = nn.Parameter(torch.zeros((channel, output_size[0], output_size[1]), dtype=torch.float32))
 
     def params(self):
-        """The parameters in ``_SoftCompGrad``'s order: embedding weight and bias, then the bias map (base) or
-        bias_conv's weight and bias (HQ)."""
+        """The trainable parameters: embedding weight and bias, then the bias map (base) or bias_conv's weight and bias
+        (HQ)."""
         tail = (self.bias_conv.weight, self.bias_conv.bias) if self.hq else (self.bias,)
         return (self.embedding.weight, self.embedding.bias) + tail
 
     def forward(self, x, t, output_size=None, residual=None):
         """``residual`` (b*t, C, H, W), optional: added to the result by the fold kernel (base model) or the conv
         epilogue (HQ) — the ``enc_feat + trans_feat`` of e2fgvi.py:263; the result is then channels_last.  Trainable
-        (``_SoftCompGrad``) when grad mode is on and x, the residual or a parameter requires grad; the result is the
-        same bits as the untracked call."""
+        (``_soft_comp_backward``) when grad mode is on and x, the residual or a parameter requires grad; the result is
+        the same bits as the untracked call."""
         output_size = tuple(output_size or self.output_size)
-        if isinstance(x, torch.Tensor) and _tracked([x, residual], self.params()):
-            return _SoftCompGrad.apply(self, x, residual, output_size, *self.params())
+        if isinstance(x, torch.Tensor) and tracked([x, residual], self.params()):
+            return KeptLaunches.apply("SoftComp", _soft_comp_run, _soft_comp_backward, self, x, residual, output_size,
+                                      *self.params())
         return self._forward(x, t, output_size, residual)
 
     def _forward(self, x, t, output_size=None, residual=None, keep=None):
@@ -139,50 +124,42 @@ class SoftComp(nn.Module):
                              self.stride, self.padding, bias_map_extra=self.bias, residual=residual)
 
 
-class _SoftCompGrad(torch.autograd.Function):
-    """``SoftComp``'s launches with a backward into its parameters, the tokens and the residual.  With dfeat = the
-    gradient of the folded features (HQ: bias_conv's input gradient on ``conv_dgrad``, its weight gradient on
-    ``conv3x3_wgrad``): the base bias map gets the sum of dfeat over BT, the embedding dW = unfold(dfeat)^T . tokens
-    and db = the sum of unfold(dfeat), the tokens unfold(dfeat) . W on ``soft_split``'s launch with W^T; the residual
-    receives the gradient unchanged."""
+def _soft_comp_run(keep, mod, tokens, residual, output_size, *params):
+    """``SoftComp``'s launches (``_forward`` keeping the split tokens and, HQ, bias_conv's operand); saves the
+    parameters."""
+    keep["mod"], keep["shape"] = mod, tokens.shape
+    return mod._forward(tokens, tokens.shape[1], output_size, residual, keep), params
 
-    @staticmethod
-    def forward(ctx, mod, tokens, residual, output_size, *params):
-        keep = {}
-        out = mod._forward(tokens, tokens.shape[1], output_size, residual, keep)
-        ctx.mod, ctx.keep, ctx.output_size, ctx.shape = mod, keep, output_size, tokens.shape
-        ctx.save_for_backward(*params)
-        return out
 
-    @staticmethod
-    def backward(ctx, grad):
-        if ctx.keep is None:
-            raise _second_backward("SoftComp")
-        params = ctx.saved_tensors
-        mod, keep = ctx.mod, ctx.keep
-        ctx.keep = None
-        need_tok, need_res = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
-        needs = ctx.needs_input_grad[4:]
-        grads = [None] * len(params)
-        k, s, p = mod.kernel_size, mod.stride, mod.padding
-        dfeat = grad
-        if mod.hq:
-            if needs[2] or needs[3]:
-                dw, db = ops.conv3x3_wgrad(grad.permute(0, 2, 3, 1), [keep["feat"]], with_bias=needs[3])
-                grads[2], grads[3] = (dw if needs[2] else None), db
-            dfeat = None
-            if need_tok or needs[0] or needs[1]:
-                dfeat = ops.conv_dgrad(ops.split_nhwc(grad), params[2]).permute(0, 3, 1, 2)
-        elif needs[2]:
-            grads[2] = grad.sum(0)
-        if needs[0] or needs[1]:
-            cols = ops.t2t_unfold(dfeat, k, s, p, out="split")
-            dw, db = ops.linear_wgrad(cols, keep["tokens"], with_bias=needs[1])
-            grads[0], grads[1] = (dw if needs[0] else None), db
-        dtok = None
-        if need_tok:
-            dtok = ops.soft_split(dfeat, params[0], None, k, s, p, transpose=True).reshape(ctx.shape)
-        return (None, dtok, grad if need_res else None, None) + tuple(grads)
+def _soft_comp_backward(keep, saved, needs, grad):
+    """The backward into ``SoftComp``'s parameters, the tokens and the residual.  With dfeat = the gradient of the
+    folded features (HQ: bias_conv's input gradient on ``conv_dgrad``, its weight gradient on ``conv3x3_wgrad``): the
+    base bias map gets the sum of dfeat over BT, the embedding dW = unfold(dfeat)^T . tokens and db = the sum of
+    unfold(dfeat), the tokens unfold(dfeat) . W on ``soft_split``'s launch with W^T; the residual receives the gradient
+    unchanged."""
+    mod, params = keep["mod"], saved
+    need_tok, need_res = needs[1], needs[2]
+    needs = needs[4:]
+    grads = [None] * len(params)
+    k, s, p = mod.kernel_size, mod.stride, mod.padding
+    dfeat = grad
+    if mod.hq:
+        if needs[2] or needs[3]:
+            dw, db = ops.conv3x3_wgrad(grad.permute(0, 2, 3, 1), [keep["feat"]], with_bias=needs[3])
+            grads[2], grads[3] = (dw if needs[2] else None), db
+        dfeat = None
+        if need_tok or needs[0] or needs[1]:
+            dfeat = ops.conv_dgrad(ops.split_nhwc(grad), params[2]).permute(0, 3, 1, 2)
+    elif needs[2]:
+        grads[2] = grad.sum(0)
+    if needs[0] or needs[1]:
+        cols = ops.t2t_unfold(dfeat, k, s, p, out="split")
+        dw, db = ops.linear_wgrad(cols, keep["tokens"], with_bias=needs[1])
+        grads[0], grads[1] = (dw if needs[0] else None), db
+    dtok = None
+    if need_tok:
+        dtok = ops.soft_split(dfeat, params[0], None, k, s, p, transpose=True).reshape(keep["shape"])
+    return (None, dtok, grad if need_res else None, None, *grads)
 
 
 class FusionFeedForward(nn.Module):
@@ -200,14 +177,14 @@ class FusionFeedForward(nn.Module):
 
     def forward(self, x, output_size=None, residual=None):
         """conv1 -> [fold / fold(ones) -> unfold -> GELU] (one fused kernel on the token-major layout) -> conv2
-        (+ residual, fused into the GEMM epilogue).  Trainable (``_FusionFeedForwardGrad``) when grad mode is on, x is
-        an fp32 tensor (B, N, 512) and x, the residual or a Linear's parameter requires grad; the output is the same
-        bits as the untracked call."""
+        (+ residual, fused into the GEMM epilogue).  Trainable (``_ffn_backward``) when grad mode is on, x is an fp32
+        tensor (B, N, 512) and x, the residual or a Linear's parameter requires grad; the output is the same bits as the
+        untracked call."""
         params = (self.conv1[0].weight, self.conv1[0].bias, self.conv2[1].weight, self.conv2[1].bias)
-        if isinstance(x, torch.Tensor) and _tracked([x, residual], params):
-            p = self.t2t_params
-            return _FusionFeedForwardGrad.apply(self, x, residual, tuple(output_size or p.get("output_size")), *params)
         p = self.t2t_params
+        if isinstance(x, torch.Tensor) and tracked([x, residual], params):
+            return KeptLaunches.apply("FusionFeedForward", _ffn_run, _ffn_back, self, x, residual,
+                                      tuple(output_size or p.get("output_size")), *params)
         output_size = output_size or p.get("output_size")
         f_h, f_w = _token_grid(output_size, p["kernel_size"], p["stride"], p["padding"])
         n_vecs = f_h * f_w
@@ -225,17 +202,17 @@ class FusionFeedForward(nn.Module):
         return output_size, p["kernel_size"], p["stride"], p["padding"]
 
 
-def _ffn_forward(mod, xs, output_size, w1, b1, w2, b2, residual):
+def _ffn_forward(mod, xs, output_size, w1, b1, w2, b2, residual, keep):
     """``FusionFeedForward``'s training launches on the split operand xs (rows, 512): conv1, the fold/normalise/unfold
     kernel in its training mode (which also keeps u, the normalised values before GELU), conv2 (+ residual).  Returns
-    (out (rows, 512), the dict ``_ffn_backward`` reads)."""
+    out (rows, 512); ``keep`` (a dict) receives what ``_ffn_backward`` reads."""
     geo = mod.geometry(output_size)
     h = ops.linear(xs, w1, b1)
     hd = h.shape[-1]
     f_h, f_w = _token_grid(*geo)
     z, u = ops.t2t_fold_unfold_train(h.view(-1, f_h * f_w, hd), *geo, out="split", pitch=(hd + 63) // 64 * 64)
-    out = ops.linear(z.view(-1, z.shape[-1]), w2, b2, residual=residual)
-    return out, {"x": xs, "u": u, "z": z, "geo": geo}
+    keep.update(x=xs, u=u, z=z, geo=geo)
+    return ops.linear(z.view(-1, z.shape[-1]), w2, b2, residual=residual)
 
 
 def _ffn_backward(keep, grad, w1, w2, need_x, nw1, nb1, nw2, nb2):
@@ -262,30 +239,19 @@ def _ffn_backward(keep, grad, w1, w2, need_x, nw1, nb1, nw2, nb2):
     return dx, dw1, db1, dw2, db2
 
 
-class _FusionFeedForwardGrad(torch.autograd.Function):
-    """``FusionFeedForward``'s launches with a backward into both Linears, x and the residual: the forward splits x
-    once (conv1's operand, kept for its weight gradient) and runs ``_ffn_forward``; the backward is ``_ffn_backward``,
-    and the residual receives the output's gradient."""
+def _ffn_run(keep, mod, x, residual, output_size, w1, b1, w2, b2):
+    """``FusionFeedForward``'s tracked launches: x split once (conv1's operand, kept for its weight gradient), then
+    ``_ffn_forward``; saves w1 and w2."""
+    b, n, _ = x.shape
+    xs = ops.SplitMat(*ops.split_bf16(x.reshape(-1, x.shape[-1])))
+    keep["shape"] = x.shape
+    return _ffn_forward(mod, xs, output_size, w1, b1, w2, b2, residual, keep).view(b, n, -1), (w1, w2)
 
-    @staticmethod
-    def forward(ctx, mod, x, residual, output_size, w1, b1, w2, b2):
-        b, n, _ = x.shape
-        xs = ops.SplitMat(*ops.split_bf16(x.reshape(-1, x.shape[-1])))
-        out, ctx.keep = _ffn_forward(mod, xs, output_size, w1, b1, w2, b2, residual)
-        ctx.shape = x.shape
-        ctx.save_for_backward(w1, w2)
-        return out.view(b, n, -1)
 
-    @staticmethod
-    def backward(ctx, grad):
-        if ctx.keep is None:
-            raise _second_backward("FusionFeedForward")
-        w1, w2 = ctx.saved_tensors
-        keep = ctx.keep
-        ctx.keep = None
-        need_x, need_res = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
-        dx, dw1, db1, dw2, db2 = _ffn_backward(keep, grad, w1, w2, need_x, *ctx.needs_input_grad[4:])
-        return None, None if dx is None else dx.view(ctx.shape), grad if need_res else None, None, dw1, db1, dw2, db2
+def _ffn_back(keep, saved, needs, grad):
+    """``_ffn_backward`` for ``_ffn_run``; the residual receives the output's gradient."""
+    dx, *grads = _ffn_backward(keep, grad, *saved, needs[1], *needs[4:])
+    return (None, None if dx is None else dx.view(keep["shape"]), grad if needs[2] else None, None, *grads)
 
 
 def window_partition(x, window_size):
@@ -355,14 +321,15 @@ class WindowAttention(nn.Module):
         """x (B,T,H,W,C) normed tokens (tensor or ops.SplitMat), pooled (B,nWh,nWw,T,C) tensor or the SplitMat of
         ops.window_pool (already (B,T,nWh,nWw,C)) -> (B,T,H,W,C) after proj (+ residual).
         ``joint_shape`` = (B,T,H,W): x is the SplitMat of ``ops.layer_norm_pool`` (token rows followed by pooled rows) and
-        ONE qkv GEMM serves both.  Trainable (``_WindowAttentionGrad``) when grad mode is on, x is a tensor, no
+        ONE qkv GEMM serves both.  Trainable (``_attention_run``) when grad mode is on, x is a tensor, no
         ``joint_shape`` is given and x, pooled, the residual or a parameter of ``qkv`` / ``proj`` requires grad; the result
         is the same bits as the untracked call.  ``keep`` (a dict or None; untracked calls on a SplitMat x without pooled
         only) receives what ``_attention_backward`` reads: x, the fp16 qkv / qkv_pooled and the split attention output."""
         params = self.params()
         if (keep is None and joint_shape is None and isinstance(x, torch.Tensor) and not isinstance(pooled, ops.SplitMat)
-                and _tracked([x, pooled if self.uses_pooled else None, residual], [p for p in params if p is not None])):
-            return _WindowAttentionGrad.apply(self, x, pooled if self.uses_pooled else None, residual, *params)
+                and tracked([x, pooled if self.uses_pooled else None, residual], params)):
+            return KeptLaunches.apply("WindowAttention", _attention_run, _attention_back, self, x,
+                                      pooled if self.uses_pooled else None, residual, *params)
         if joint_shape is not None:
             B, T, H, W = joint_shape
             wh, ww = self.window_size
@@ -384,8 +351,7 @@ class WindowAttention(nn.Module):
         return ops.linear(out, self.proj.weight, self.proj.bias, residual=residual)
 
     def params(self):
-        """The parameters in ``_WindowAttentionGrad``'s order: qkv weight and bias (None without qkv_bias), proj weight
-        and bias."""
+        """The trainable parameters: qkv weight and bias (None without qkv_bias), proj weight and bias."""
         return self.qkv.weight, self.qkv.bias, self.proj.weight, self.proj.bias
 
     def forward(self, x_all, mask_all=None):
@@ -395,58 +361,47 @@ class WindowAttention(nn.Module):
         return window_partition(out, self.window_size)
 
 
-class _WindowAttentionGrad(torch.autograd.Function):
-    """``WindowAttention.attend``'s launches with a backward into qkv, proj, x, pooled and the residual.  The forward
-    splits the token rows and the pooled rows once, into one operand (kept for qkv's weight gradient), and runs the
-    same qkv, attention and proj launches as the untracked call.  Backward, with g = the output's gradient:
-      dW_proj = g^T . O (the attention's kept split output), db_proj = sum g;  dO = g . W_proj (``linear`` with W^T);
-      dqkv = the attention backward (token rows and pooled rows in one buffer);
-      dW_qkv = dqkv^T . [x; pooled] and db_qkv = sum dqkv over both sets of rows in one reduction;
-      [dx; dpooled] = dqkv . W_qkv (``linear`` with W^T); the residual receives g."""
+def _attention_run(keep, mod, x, pooled, residual, wq, bq, wp, bp):
+    """``WindowAttention.attend``'s tracked launches: the token rows and the pooled rows split once, into one operand
+    (kept for qkv's weight gradient), then the same qkv, attention and proj launches as the untracked call; saves the
+    qkv and proj weights."""
+    B, T, H, W, C = x.shape
+    wh, ww = mod.window_size
+    n_tok = B * T * H * W
+    rows = x.reshape(n_tok, C)
+    if pooled is not None:                                  # reference layout (B,nWh,nWw,T,C) -> (B,T,nWh,nWw,C)
+        rows = torch.cat([rows, pooled.permute(0, 3, 1, 2, 4).reshape(-1, C)])
+    xs = ops.SplitMat(*ops.split_bf16(rows))
+    qkv = ops.linear(ops.SplitMat(xs.hi[:n_tok], xs.lo[:n_tok]), wq, bq, out_dtype=torch.float16).view(B, T, H, W, -1)
+    qkv_pooled = None
+    if pooled is not None:
+        qkv_pooled = ops.linear(ops.SplitMat(xs.hi[n_tok:], xs.lo[n_tok:]), wq, bq, out_dtype=torch.float16)
+        qkv_pooled = qkv_pooled.view(B, T, H // wh, W // ww, -1)
+    out = ops.focal_window_attention(qkv, qkv_pooled, mod.num_heads, mod.window_size, mod.expand_size,
+                                     mod.pooled_kernel(), mod.scale, out_dtype="split")
+    keep.update(mod=mod, shape=x.shape, x=xs, qkv=qkv, qkv_pooled=qkv_pooled, out=out)
+    return ops.linear(out, wp, bp, residual=residual), (wq, wp)
 
-    @staticmethod
-    def forward(ctx, mod, x, pooled, residual, wq, bq, wp, bp):
-        B, T, H, W, C = x.shape
+
+def _attention_back(keep, saved, needs, grad):
+    """``_attention_backward`` for ``_attention_run`` at the output's gradient, [dx; dpooled] back in the layouts of x
+    and pooled; the residual receives the gradient."""
+    mod, shape = keep["mod"], keep["shape"]
+    need_x, need_pool, need_res, nwq, nbq, nwp, nbp = needs[1:]
+    B, T, H, W, C = shape
+    g = None
+    if nwp or nbp or need_x or need_pool or nwq or nbq:
+        g = ops.SplitMat(*ops.split_bf16(grad.reshape(-1, C)))
+    drows, dwq, dbq, dwp, dbp = _attention_backward(mod, keep, g, *saved, shape, need_x or need_pool, nwq, nbq, nwp,
+                                                    nbp)
+    dx = dpool = None
+    n_tok = B * T * H * W
+    if need_x:
+        dx = drows[:n_tok].view(B, T, H, W, C)
+    if need_pool:
         wh, ww = mod.window_size
-        n_tok = B * T * H * W
-        rows = x.reshape(n_tok, C)
-        if pooled is not None:                                  # reference layout (B,nWh,nWw,T,C) -> (B,T,nWh,nWw,C)
-            rows = torch.cat([rows, pooled.permute(0, 3, 1, 2, 4).reshape(-1, C)])
-        xs = ops.SplitMat(*ops.split_bf16(rows))
-        qkv = ops.linear(ops.SplitMat(xs.hi[:n_tok], xs.lo[:n_tok]), wq, bq, out_dtype=torch.float16).view(B, T, H, W, -1)
-        qkv_pooled = None
-        if pooled is not None:
-            qkv_pooled = ops.linear(ops.SplitMat(xs.hi[n_tok:], xs.lo[n_tok:]), wq, bq, out_dtype=torch.float16)
-            qkv_pooled = qkv_pooled.view(B, T, H // wh, W // ww, -1)
-        out = ops.focal_window_attention(qkv, qkv_pooled, mod.num_heads, mod.window_size, mod.expand_size,
-                                         mod.pooled_kernel(), mod.scale, out_dtype="split")
-        ctx.mod, ctx.keep, ctx.shape = mod, {"x": xs, "qkv": qkv, "qkv_pooled": qkv_pooled, "out": out}, x.shape
-        ctx.save_for_backward(wq, wp)
-        return ops.linear(out, wp, bp, residual=residual)
-
-    @staticmethod
-    def backward(ctx, grad):
-        if ctx.keep is None:
-            raise _second_backward("WindowAttention")
-        wq, wp = ctx.saved_tensors
-        keep, mod = ctx.keep, ctx.mod
-        ctx.keep = None
-        need_x, need_pool, need_res = ctx.needs_input_grad[1:4]
-        nwq, nbq, nwp, nbp = ctx.needs_input_grad[4:]
-        B, T, H, W, C = ctx.shape
-        g = None
-        if nwp or nbp or need_x or need_pool or nwq or nbq:
-            g = ops.SplitMat(*ops.split_bf16(grad.reshape(-1, C)))
-        drows, dwq, dbq, dwp, dbp = _attention_backward(mod, keep, g, wq, wp, ctx.shape, need_x or need_pool, nwq, nbq,
-                                                        nwp, nbp)
-        dx = dpool = None
-        n_tok = B * T * H * W
-        if need_x:
-            dx = drows[:n_tok].view(B, T, H, W, C)
-        if need_pool:
-            wh, ww = mod.window_size
-            dpool = drows[n_tok:].view(B, T, H // wh, W // ww, C).permute(0, 2, 3, 1, 4).contiguous()
-        return None, dx, dpool, grad if need_res else None, dwq, dbq, dwp, dbp
+        dpool = drows[n_tok:].view(B, T, H // wh, W // ww, C).permute(0, 2, 3, 1, 4).contiguous()
+    return None, dx, dpool, grad if need_res else None, dwq, dbq, dwp, dbp
 
 
 def _attention_backward(mod, keep, g, wq, wp, shape, need_rows, nwq, nbq, nwp, nbp):
@@ -503,17 +458,17 @@ class TemporalFocalTransformerBlock(nn.Module):
         self.mlp = FusionFeedForward(dim, n_vecs=n_vecs, t2t_params=t2t_params)
 
     def params(self):
-        """The parameters in ``_TransformerBlockGrad``'s order: norm1 weight and bias, pool_layers[0] weight and bias
-        (None without pooling), attn.qkv weight and bias (None without qkv_bias), attn.proj weight and bias, norm2
-        weight and bias, mlp.conv1[0] weight and bias, mlp.conv2[1] weight and bias."""
+        """The parameters in ``_block_backward``'s order: norm1 weight and bias, pool_layers[0] weight and bias (None
+        without pooling), attn.qkv weight and bias (None without qkv_bias), attn.proj weight and bias, norm2 weight and
+        bias, mlp.conv1[0] weight and bias, mlp.conv2[1] weight and bias."""
         pool = (self.pool_layers[0].weight, self.pool_layers[0].bias) if self.attn.uses_pooled else (None, None)
         return ((self.norm1.weight, self.norm1.bias) + pool + self.attn.params() + (self.norm2.weight, self.norm2.bias)
                 + (self.mlp.conv1[0].weight, self.mlp.conv1[0].bias, self.mlp.conv2[1].weight, self.mlp.conv2[1].bias))
 
     def _forward(self, x, output_size, keep=None):
-        """The launch sequence of ``forward`` (untracked); ``keep`` (a dict or None) receives what
-        ``_TransformerBlockGrad.backward`` reads: x1 = the attention's output (+ x), the attention's operands and the
-        feed-forward's (which then runs its training forward: the same bits)."""
+        """The launch sequence of ``forward`` (untracked); ``keep`` (a dict or None) receives what ``_block_backward``
+        reads: x1 = the attention's output (+ x), the attention's operands and the feed-forward's (which then runs its
+        training forward: the same bits)."""
         shortcut = x
         B, T, H, W, C = x.shape
         attn_keep = None if keep is None else keep.setdefault("attn", {})
@@ -534,62 +489,52 @@ class TemporalFocalTransformerBlock(nn.Module):
             return self.mlp(y.view(B, T * H * W, C), output_size, residual=x.view(B, T * H * W, C)).view(B, T, H, W, C)
         mlp = self.mlp
         size = tuple(output_size or mlp.t2t_params["output_size"])
-        out, keep["mlp"] = _ffn_forward(mlp, y.view(B * T * H * W, C), size, mlp.conv1[0].weight, mlp.conv1[0].bias,
-                                        mlp.conv2[1].weight, mlp.conv2[1].bias, x)
+        out = _ffn_forward(mlp, y.view(B * T * H * W, C), size, mlp.conv1[0].weight, mlp.conv1[0].bias,
+                           mlp.conv2[1].weight, mlp.conv2[1].bias, x, keep.setdefault("mlp", {}))
         keep["x1"] = x
         return out.view(B, T, H, W, C)
 
     def forward(self, x):
         """tokens (B,T,H,W,C) -> (B,T,H,W,C); HQ: [tokens, output_size] -> (tokens, output_size).  Trainable
-        (``_TransformerBlockGrad``) when grad mode is on and the tokens or a parameter requires grad; the result is the
-        same bits as the untracked call."""
+        (``_block_backward``) when grad mode is on and the tokens or a parameter requires grad; the result is the same
+        bits as the untracked call."""
         if self.hq:  # x = [tokens, (h, w)] -> (tokens, (h, w))   (_hq.py:492-495,562-565)
             tokens, output_size = x[0], x[1]
         else:
             tokens, output_size = x, None
         params = self.params()
-        if _tracked([tokens], [p for p in params if p is not None]):
-            out = _TransformerBlockGrad.apply(self, tokens, output_size, *params)
+        if tracked([tokens], params):
+            out = KeptLaunches.apply("TemporalFocalTransformerBlock", _block_run, _block_back, self, tokens,
+                                     output_size, *params)
         else:
             out = self._forward(tokens, output_size)
         return (out, output_size) if self.hq else out
 
 
-class _TransformerBlockGrad(torch.autograd.Function):
-    """``TemporalFocalTransformerBlock``'s launches (``_forward`` with ``keep``) with a backward into every parameter
-    and the tokens x.  With g = the output's gradient and x1 = x + attention(LN1(x)):
+def _block_run(keep, mod, x, output_size, *params):
+    """``TemporalFocalTransformerBlock``'s tracked launches (``_forward`` with ``keep``); saves x and the parameters
+    (``None`` where the block has none)."""
+    keep["mod"] = mod
+    return mod._forward(x, output_size, keep), (x, *params)
+
+
+def _block_back(keep, saved, needs, grad):
+    """``_block_backward`` for ``_block_run``."""
+    x, *params = saved
+    dx, grads = _block_backward(keep["mod"], keep, x, params, grad, needs[1], needs[3:])
+    return (None, dx, None, *grads)
+
+
+def _block_backward(mod, keep, x, params, grad, need_x, needs):
+    """The backward of ``TemporalFocalTransformerBlock._forward(x, output_size, keep)`` at the output's gradient grad:
+    (dx or None, the 14 parameter gradients in ``params()`` order, None where ``needs`` is False).  With
+    x1 = x + attention(LN1(x)):
       1. the feed-forward's backward (``_ffn_backward``) gives dy = the gradient of LN2's output and both Linears';
       2. dx1 = g + LN2'(x1; dy) (``layer_norm_backward``, fp32 and split), dgamma2, dbeta2;
       3. the attention's backward (``_attention_backward``) at dx1 gives [dxn; dpooled] and qkv's and proj's gradients;
       4. dx = dx1 + LN1'(x; dxn + w_pool dpooled) (``layer_norm_pool_backward``; without pooling ``layer_norm_backward``
          with the residual dx1), dgamma1, dbeta1, d w_pool, d b_pool.
     The walk stops at the lowest part that needs a gradient; a frozen part launches no weight gradient."""
-
-    @staticmethod
-    def forward(ctx, mod, x, output_size, *params):
-        keep = {}
-        out = mod._forward(x, output_size, keep)
-        ctx.mod, ctx.keep = mod, keep
-        ctx.save_for_backward(x, *[p for p in params if p is not None])
-        ctx.have = [p is not None for p in params]
-        return out
-
-    @staticmethod
-    def backward(ctx, grad):
-        if ctx.keep is None:
-            raise _second_backward("TemporalFocalTransformerBlock")
-        saved = list(ctx.saved_tensors)
-        x = saved.pop(0)
-        params = [saved.pop(0) if h else None for h in ctx.have]
-        keep = ctx.keep
-        ctx.keep = None
-        dx, grads = _block_backward(ctx.mod, keep, x, params, grad, ctx.needs_input_grad[1], ctx.needs_input_grad[3:])
-        return (None, dx, None) + tuple(grads)
-
-
-def _block_backward(mod, keep, x, params, grad, need_x, needs):
-    """The backward of ``TemporalFocalTransformerBlock._forward(x, output_size, keep)`` at the output's gradient grad:
-    (dx or None, the 14 parameter gradients in ``params()`` order, None where ``needs`` is False)."""
     n1w, n1b, pw, pb, wq, bq, wp, bp, n2w, n2b, w1, b1, w2, b2 = params
     (nn1w, nn1b, npw, npb, nwq, nbq, nwp, nbp, nn2w, nn2b, nw1, nb1, nw2, nb2) = needs
     grads = [None] * 14
