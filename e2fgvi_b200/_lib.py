@@ -17,6 +17,9 @@ SIGNATURES = {
     "e2f_last_error": (_c.c_char_p, []),
     "e2f_flow_warp": (_i, [_vp, _fp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "e2f_flow_warp_nchw": (_i, [_fp, _fp, _fp, _i, _i, _i, _i, _i, _vp]),
+    "e2f_flow_warp_backward_work_elems": (_c.c_int64, [_i] * 3),
+    "e2f_flow_warp_backward_nhwc": (_i, [_fp, _fp, _fp, _fp, _fp, _fp, _fp, _vp] + [_i] * 4 + [_vp]),
+    "e2f_flow_warp_backward_nchw": (_i, [_fp, _c.c_int64, _fp, _fp, _fp, _fp, _fp, _fp, _vp] + [_i] * 4 + [_vp]),
     "e2f_dcn_pack_weight": (_i, [_fp, _vp, _i, _i, _i, _vp]),
     "e2f_modulated_deform_conv2d": (_i, [_vp, _fp, _fp, _vp, _fp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "e2f_dcn_pack_input": (_i, [_fp, _fp, _vp, _i, _i, _i, _i, _i, _vp]),

@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_PATH = os.path.join(HERE, "libe2fgvi_b200.so")
 STAMP = LIB_PATH + ".stamp"
 
-SOURCES = ["api.cu", "flow_warp.cu", "dcn.cu", "dcn_grad.cu", "focal_attn.cu", "focal_attn_grad.cu", "t2t.cu", "gemm.cu", "conv.cu", "elementwise.cu", "video.cu", "spynet.cu", "conv_kxn.cu", "peer.cu", "i3d.cu", "metrics.cu", "dis_wgrad.cu", "encdec_grad.cu", "linear_wgrad.cu", "layernorm_grad.cu"]
+SOURCES = ["api.cu", "flow_warp.cu", "flow_warp_grad.cu", "dcn.cu", "dcn_grad.cu", "focal_attn.cu", "focal_attn_grad.cu", "t2t.cu", "gemm.cu", "conv.cu", "elementwise.cu", "video.cu", "spynet.cu", "conv_kxn.cu", "peer.cu", "i3d.cu", "metrics.cu", "dis_wgrad.cu", "encdec_grad.cu", "linear_wgrad.cu", "layernorm_grad.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

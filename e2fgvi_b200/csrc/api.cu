@@ -104,6 +104,48 @@ int e2f_flow_warp_nchw(const float* x, const float* flow, float* out, int n, int
   return finish(launch_flow_warp_nchw(x, flow, out, n, c, h, w, pad_mode, static_cast<cudaStream_t>(stream)), "e2f_flow_warp_nchw");
 }
 
+static int flow_warp_backward_checks(const char* who, const float* x, const float* flow, const float* dout,
+                                     const float* dflow_res, const float* dflow, const float* dx_res, const float* dx,
+                                     const void* work, int n, int h, int w, int c) {
+  if (!flow || !dout) { set_error("%s: null flow / dout", who); return E2F_ERR_BAD_ARG; }
+  if (!dflow && !dx) { set_error("%s: nothing to compute (need dflow or dx)", who); return E2F_ERR_BAD_ARG; }
+  if (dflow && !x) { set_error("%s: dflow needs x", who); return E2F_ERR_BAD_ARG; }
+  if (dx && !work) { set_error("%s: dx needs the scatter workspace", who); return E2F_ERR_BAD_ARG; }
+  if ((dflow_res && !dflow) || (dx_res && !dx)) { set_error("%s: a residual goes with its output", who); return E2F_ERR_BAD_ARG; }
+  if (n < 0 || h <= 0 || w <= 0 || c <= 0) { set_error("%s: bad shape n=%d h=%d w=%d c=%d", who, n, h, w, c); return E2F_ERR_BAD_ARG; }
+  if (static_cast<long long>(n) * h * w * 4 > INT_MAX) { set_error("%s: N*H*W=%lld too large (N*H*W*4 must fit in int)", who, static_cast<long long>(n) * h * w); return E2F_ERR_UNSUPPORTED; }
+  if (!aligned(flow, 8) || (dflow && !aligned(dflow, 8)) || (dflow_res && !aligned(dflow_res, 8)) || (work && !aligned(work, 256))) { set_error("%s: flow / dflow need 8-byte, work 256-byte alignment", who); return E2F_ERR_ALIGNMENT; }
+  return 0;
+}
+
+int64_t e2f_flow_warp_backward_work_elems(int n, int h, int w) {
+  const char* who = "e2f_flow_warp_backward_work_elems";
+  if (n < 0 || h <= 0 || w <= 0) { set_error("%s: bad shape n=%d h=%d w=%d", who, n, h, w); return E2F_ERR_BAD_ARG; }
+  if (static_cast<long long>(n) * h * w * 4 > INT_MAX) { set_error("%s: N*H*W=%lld too large (N*H*W*4 must fit in int)", who, static_cast<long long>(n) * h * w); return E2F_ERR_UNSUPPORTED; }
+  return static_cast<int64_t>(flow_warp_backward_work_elems(n, h, w));
+}
+
+int e2f_flow_warp_backward_nhwc(const float* x, const float* flow, const float* dout, const float* dflow_residual,
+                                float* dflow, const float* dx_residual, float* dx, void* work, int n, int h, int w,
+                                int c, void* stream) {
+  const char* who = "e2f_flow_warp_backward_nhwc";
+  if (const int st = flow_warp_backward_checks(who, x, flow, dout, dflow_residual, dflow, dx_residual, dx, work, n, h, w, c)) return st;
+  if (c % 4) { set_error("%s: C=%d must be a multiple of 4 (use e2f_flow_warp_backward_nchw)", who, c); return E2F_ERR_UNSUPPORTED; }
+  if ((x && !aligned(x, 16)) || !aligned(dout, 16) || (dx && !aligned(dx, 16)) || (dx_residual && !aligned(dx_residual, 16))) { set_error("%s: x / dout / dx / dx_residual need 16-byte alignment", who); return E2F_ERR_ALIGNMENT; }
+  return finish(launch_flow_warp_backward(x, 0, 0, flow, dout, dflow_residual, dflow, dx_residual, dx, work, n, h, w, c,
+                                          static_cast<cudaStream_t>(stream)), who);
+}
+
+int e2f_flow_warp_backward_nchw(const float* x, int64_t x_bstride, const float* flow, const float* dout,
+                                const float* dflow_residual, float* dflow, const float* dx_residual, float* dx,
+                                void* work, int n, int c, int h, int w, void* stream) {
+  const char* who = "e2f_flow_warp_backward_nchw";
+  if (const int st = flow_warp_backward_checks(who, x, flow, dout, dflow_residual, dflow, dx_residual, dx, work, n, h, w, c)) return st;
+  if (x && x_bstride < static_cast<int64_t>(c) * h * w) { set_error("%s: x batch stride %lld < C*H*W", who, static_cast<long long>(x_bstride)); return E2F_ERR_BAD_ARG; }
+  return finish(launch_flow_warp_backward(x, static_cast<long long>(x_bstride), 1, flow, dout, dflow_residual, dflow,
+                                          dx_residual, dx, work, n, h, w, c, static_cast<cudaStream_t>(stream)), who);
+}
+
 int e2f_dcn_pack_weight(const float* w, void* w_packed_f16, int cout, int cin, int deform_groups, void* stream) {
   if (!w || !w_packed_f16) { set_error("e2f_dcn_pack_weight: null pointer"); return E2F_ERR_BAD_ARG; }
   if (cout <= 0 || cin <= 0 || deform_groups <= 0 || cin % deform_groups) { set_error("e2f_dcn_pack_weight: bad shape"); return E2F_ERR_BAD_ARG; }

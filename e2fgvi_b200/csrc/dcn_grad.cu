@@ -12,13 +12,13 @@
 //     for corners outside the image), the source index (pixel*144 + sp)*4 + corner, and the coefficient mask * w_corner.
 // The list is sorted by key with CUB's radix sort (stable, so each destination's run stays in source order), and
 // gather_kernel walks every destination's run in that order: dx is the same bits on every run, no float atomics.
-#include <cub/device/device_radix_sort.cuh>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <climits>
 #include "common.cuh"
 #include "dcn_math.cuh"
 #include "launch.h"
+#include "scatter_sort.cuh"
 
 namespace e2f {
 namespace dcn_grad {
@@ -30,7 +30,6 @@ constexpr int HEAD_C = 3 * NSP;           // 432 raw head channels: 288 offsets 
 constexpr int FLOW_C = 8;                 // d flow rows: [d flow_1 (u, v), d flow_2 (u, v), 0, 0, 0, 0]
 constexpr int PIX_PER_CTA = 16;
 constexpr int THREADS = PIX_PER_CTA * DG;  // 256
-constexpr long long SORT_RESERVE_MIN = 65536;   // bytes of sort scratch besides one byte per list entry
 
 __device__ __forceinline__ uint32_t bf16_split_pair(float a, float b, uint32_t& lo) {
   const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
@@ -213,30 +212,13 @@ gather_kernel(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ va
   *reinterpret_cast<float4*>(dx + (n * hw + pix) * CIN + g * CPG + 4 * q) = s;
 }
 
-// workspace (32-bit elements): keys x 2, source indices x 2 (the sort's double buffers), coefficients, sort scratch
-struct Work {
-  uint32_t *keys0, *keys1, *vals0, *vals1;
-  float* coef;
-  void* temp;
-  size_t temp_bytes;
-};
-
 static long long list_len(long long M) { return M * NSP * 4; }
-static long long temp_elems(long long L) { return (L + SORT_RESERVE_MIN + 255) / 256 * 64; }
-
-static Work carve(void* work, long long L) {
-  uint32_t* w = static_cast<uint32_t*>(work);
-  const long long body = (5 * L + 63) / 64 * 64;                // 256-byte aligned scratch
-  return Work{w, w + L, w + 2 * L, w + 3 * L, reinterpret_cast<float*>(w + 4 * L), w + body,
-              static_cast<size_t>(temp_elems(L)) * 4};
-}
 
 }  // namespace dcn_grad
 
 long long dcn_backward_work_elems(int n, int h, int w) {
   using namespace dcn_grad;
-  const long long L = list_len(static_cast<long long>(n) * h * w);
-  return (5 * L + 63) / 64 * 64 + temp_elems(L);
+  return scatter::work_elems(list_len(static_cast<long long>(n) * h * w));
 }
 
 int launch_dcn_sample_backward(const void* x, const float* head, const float* flow1, const float* flow2, const float* da,
@@ -248,7 +230,7 @@ int launch_dcn_sample_backward(const void* x, const float* head, const float* fl
   uint32_t *keys = nullptr, *vals = nullptr;
   float* coef = nullptr;
   if (work) {
-    const Work wk = carve(work, list_len(M));
+    const scatter::Work wk = scatter::carve(work, list_len(M));
     keys = wk.keys0;
     vals = wk.vals0;
     coef = wk.coef;
@@ -275,23 +257,12 @@ int launch_dcn_scatter_backward(const float* da, void* work, float* dx, int n, i
   const long long M = static_cast<long long>(n) * h * w;
   if (M == 0) return 0;
   const long long L = list_len(M), D = M * DG;
-  Work wk = carve(work, L);
-  int end_bit = 0;
-  while (end_bit < 32 && (D >> end_bit) != 0) ++end_bit;        // keys are <= D (the sentinel)
-  cub::DoubleBuffer<uint32_t> kb(wk.keys0, wk.keys1), vb(wk.vals0, wk.vals1);
-  size_t need = 0;
-  cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, need, kb, vb, static_cast<int>(L), 0, end_bit, stream);
-  if (e != cudaSuccess) return static_cast<int>(e);
-  if (need > wk.temp_bytes) {
-    set_error("deformable conv backward: the radix sort asks for %zu bytes of scratch, the workspace reserves %zu", need,
-              wk.temp_bytes);
-    return -2;
-  }
-  // CUB's kernels are not this library's: they are not counted as its launches
-  e = cub::DeviceRadixSort::SortPairs(wk.temp, need, kb, vb, static_cast<int>(L), 0, end_bit, stream);
-  if (e != cudaSuccess) return static_cast<int>(e);
+  const scatter::Work wk = scatter::carve(work, L);
+  const uint32_t *keys = nullptr, *vals = nullptr;
+  const int st = scatter::sort_pairs(wk, L, D, "deformable conv backward", &keys, &vals, stream);   // keys <= D
+  if (st) return st;
   const long long threads = D * 4;
-  gather_kernel<<<static_cast<unsigned>((threads + 255) / 256), 256, 0, stream>>>(kb.Current(), vb.Current(), wk.coef,
+  gather_kernel<<<static_cast<unsigned>((threads + 255) / 256), 256, 0, stream>>>(keys, vals, wk.coef,
                                                                                  da, dx, L, D, h, w);
   count_launch();
   return static_cast<int>(cudaGetLastError());

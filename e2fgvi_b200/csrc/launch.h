@@ -67,6 +67,14 @@ int launch_flow_warp_nhwc(const void* x, const float* flow, void* out, int n, in
 int launch_flow_warp_nchw(const float* x, const float* flow, float* out, int n, int c, int h, int w, int pad_mode,
                           cudaStream_t stream);
 
+// flow_warp backward (flow_warp_grad.cu): d flow (optional residual) and the sorted-scatter dx (optional residual) of
+// an NHWC (nchw = 0, C % 4 == 0) or NCHW (nchw = 1, x batch stride x_bs elements, dout / dx dense) fp32 warp; workspace
+// of flow_warp_backward_work_elems 32-bit words when dx is asked for.
+long long flow_warp_backward_work_elems(int n, int h, int w);
+int launch_flow_warp_backward(const float* x, long long x_bs, int nchw, const float* flow, const float* dout,
+                              const float* dflow_res, float* dflow, const float* dx_res, float* dx, void* work, int n,
+                              int h, int w, int c, cudaStream_t stream);
+
 int launch_prop_prologue(const float* prop, const float* feat2, const float* flow1, long long f1_bs, const float* flowp,
                          long long fp_bs, void* c1h, void* c1l, void* c2h, void* c2l, float* f1_out, float* f2_out,
                          void* flh, void* fll, void* xg, int n, int h, int w, int c, cudaStream_t stream);

@@ -273,10 +273,85 @@ class BidirectionalPropagation(nn.Module):
                                 residual=x32[:, i].permute(0, 3, 1, 2), out="both", into=(o32[:, i], ohi[:, i], olo[:, i]))
         return o32, ohi, olo
 
+    def _params(self):
+        """The 30 parameters in the order of the tracked call: per direction the alignment's 10 and the backbone's 4,
+        then the fusion's weight and bias."""
+        ps = []
+        for name in self.DIRECTIONS:
+            bb = self.backbone[name]
+            ps += self.deform_align[name]._params() + [bb[0].weight, bb[0].bias, bb[2].weight, bb[2].bias]
+        return ps + [self.fusion.weight, self.fusion.bias]
+
+    def _propagate_keep(self, x32, x_hi, x_lo, flows_backward, flows_forward, keep):
+        """``propagate_frames``' launches for (b,t,h,w,c) x, keeping the operands of the backward: per step the
+        prologue's outputs, the grouped fp16 DCN input, the offset head's split inputs and fp32 LeakyReLU outputs, the
+        raw head, the backbone conv 0's output (fp32 and split) and the aligned features' split; per direction the
+        results' (t,b,h,w,c) fp32 and split buffers.  The head convs and backbone conv 0 store their fp32 output too
+        (out="both"); the same kernels compute the same bits, so the result is ``propagate_frames``' to the bit."""
+        b, t, h, w, c = x32.shape
+        cur = [ops.SplitNHWC(x_hi[:, i], x_lo[:, i], (b, c, h, w)) for i in range(t)]
+        zero = torch.zeros((b, h, w, c), dtype=x_hi.dtype, device=x32.device)
+        zero_sp = ops.SplitNHWC(zero, zero, (b, c, h, w))
+        bufs, steps = {}, {}
+        for name in self.DIRECTIONS:
+            bufs[name] = (torch.empty((t, b, h, w, c), dtype=torch.float32, device=x32.device),
+                          torch.empty((t, b, h, w, c), dtype=x_hi.dtype, device=x32.device),
+                          torch.empty((t, b, h, w, c), dtype=x_lo.dtype, device=x32.device))
+        swept_sp = {}
+        for name in self.DIRECTIONS:
+            backward = name == "backward_"
+            order = list(range(t - 1, -1, -1)) if backward else list(range(t))
+            flows = flows_backward if backward else flows_forward
+            align, backbone = self.deform_align[name], self.backbone[name]
+            co = align.conv_offset
+            r32, rhi, rlo = bufs[name]
+            hist32, steps[name] = [], []
+            for i, idx in enumerate(order):
+                st = {"idx": idx}
+                prop32, prop_sp = None, zero_sp
+                if i > 0:
+                    xg, cond_n1, cond_n2, flows_op, flow_n1, flow_n2 = ops.prop_prologue(
+                        hist32[-1], hist32[-2] if i > 1 else None, flows[:, i - 1], flows[:, i - 2] if i > 1 else None)
+                    y1_32, y1 = ops.conv_frames([cond_n1, cur[idx], cond_n2, flows_op], co[0].weight, co[0].bias,
+                                                negative_slope=0.1, out="both")
+                    y2_32, y2 = ops.conv_frames([y1], co[2].weight, co[2].bias, negative_slope=0.1, out="both")
+                    y3_32, y3 = ops.conv_frames([y2], co[4].weight, co[4].bias, negative_slope=0.1, out="both")
+                    head = ops.conv_frames([y3], co[6].weight, co[6].bias)
+                    prop32, prop_sp = ops.deform_align_fused(xg, head, flow_n1, flow_n2, align.packed_weight(),
+                                                             align.bias, align.deform_groups,
+                                                             align.max_residue_magnitude, out_split=True)
+                    st.update(xg=xg.data, head=head, flow_n1=flow_n1, flow_n2=flow_n2, conds=(cond_n1, cond_n2),
+                              flows_op=flows_op, head_srcs=[[y1], [y2], [y3]], acts=[None, y1_32, y2_32, y3_32])
+                parts = [cur[idx], prop_sp] if backward else [cur[idx], swept_sp["backward_"][idx], prop_sp]
+                y32, y = ops.conv_frames(parts, backbone[0].weight, backbone[0].bias, negative_slope=0.1, out="both")
+                new32, _ = ops.conv_frames([y], backbone[2].weight, backbone[2].bias, residual=prop32, out="both",
+                                           into=(r32[idx], rhi[idx], rlo[idx]))
+                st.update(parts=parts, y32=y32, y=y)
+                hist32.append(new32)
+                steps[name].append(st)
+            swept_sp[name] = [ops.SplitNHWC(rhi[i], rlo[i], (b, c, h, w)) for i in range(t)]
+        o32, ohi, olo = torch.empty_like(x32), torch.empty_like(x_hi), torch.empty_like(x_lo)
+        if b == 1:
+            srcs = [ops.SplitNHWC(bufs[n_][1].view(t, h, w, c), bufs[n_][2].view(t, h, w, c), (t, c, h, w)) for n_ in self.DIRECTIONS]
+            ops.conv_frames(srcs, self.fusion.weight, self.fusion.bias, residual=x32[0].permute(0, 3, 1, 2), out="both",
+                            into=(o32[0], ohi[0], olo[0]))
+        else:
+            for i in range(t):
+                ops.conv_frames([swept_sp["backward_"][i], swept_sp["forward_"][i]], self.fusion.weight, self.fusion.bias,
+                                residual=x32[:, i].permute(0, 3, 1, 2), out="both", into=(o32[:, i], ohi[:, i], olo[:, i]))
+        keep.update(bufs=bufs, steps=steps, x_split=(x_hi, x_lo), shape=(b, t, h, w, c))
+        return o32
+
     def forward(self, x, flows_backward, flows_forward):
-        """x (b,t,c,h,w); flows_* (b,t-1,2,h,w) -> (b,t,c,h,w)."""
+        """x (b,t,c,h,w); flows_* (b,t-1,2,h,w) -> (b,t,c,h,w).  Under grad mode, on the fused path, and when x, a flow or
+        a parameter requires grad, the result carries a ``grad_fn`` into all of them (``_prop_backward``); it is
+        bit-identical to the untracked call."""
         b, t, c, h, w = x.shape
         if self.fused_prologue and c % 16 == 0:
+            params = self._params()
+            if tracked((x, flows_backward, flows_forward), params):
+                return KeptLaunches.apply("BidirectionalPropagation", _prop_run, _prop_back, self, x, flows_backward,
+                                          flows_forward, *params)
             x32 = x.permute(0, 1, 3, 4, 2).contiguous().float()          # no-op for (b,t,h,w,c) storage
             x_hi, x_lo = ops.split_bf16(x32)
             o32, _, _ = self.propagate_frames(x32, x_hi, x_lo, flows_backward, flows_forward)
@@ -322,3 +397,176 @@ class BidirectionalPropagation(nn.Module):
             tokens[:, i, :, :, c:].copy_(swept["forward_"][i].permute(0, 2, 3, 1))
         out = ops.linear(tokens, self.fusion.weight, self.fusion.bias, residual=x.permute(0, 1, 3, 4, 2))
         return out.permute(0, 1, 4, 2, 3)
+
+
+def _prop_run(keep, mod, x, flows_backward, flows_forward, *params):
+    """The tracked launches of ``BidirectionalPropagation.forward`` (``_propagate_keep``); saves the 30 parameters."""
+    x32 = x.permute(0, 1, 3, 4, 2).contiguous().float()
+    x_hi, x_lo = ops.split_bf16(x32)
+    keep.update(mod=mod, flows={"backward_": flows_backward, "forward_": flows_forward})
+    o32 = mod._propagate_keep(x32, x_hi, x_lo, flows_backward, flows_forward, keep)
+    return o32.permute(0, 1, 4, 2, 3), params
+
+
+def _prop_back(keep, saved, needs, grad):
+    """``_prop_backward`` for ``_prop_run``."""
+    return (None, *_prop_backward(keep["mod"], keep, grad, needs[1:4], needs[4:]))
+
+
+def _dense(sources):
+    """One dense ``SplitNHWC`` of split operands (batch-strided frame slices allowed), channel-concatenated: the weight
+    gradient reads dense sources, at most two of them."""
+    if len(sources) == 1 and sources[0].hi.is_contiguous():
+        return sources[0]
+    n, _, h, w = sources[0].shape
+    hi = torch.cat([s.hi for s in sources], -1) if len(sources) > 1 else sources[0].hi.contiguous()
+    lo = torch.cat([s.lo for s in sources], -1) if len(sources) > 1 else sources[0].lo.contiguous()
+    return ops.SplitNHWC(hi, lo, (n, hi.shape[-1], h, w))
+
+
+def _accumulate(grads, first, parts):
+    """Adds each step's parameter gradients to the sum of the steps walked before it (None: nothing to add)."""
+    for j, v in enumerate(parts):
+        if v is not None:
+            grads[first + j] = v if grads[first + j] is None else grads[first + j].add_(v)
+
+
+def _prop_backward(mod, keep, grad, need_in, need):
+    """Gradients of the tracked ``BidirectionalPropagation.forward``.  need_in = (x, flows_backward, flows_forward) need a
+    gradient; need = the 30 parameters of ``_params()``.  Returns (dx, d flows_backward, d flows_forward, *parameter
+    gradients).
+
+    The walk: the fusion, then the forward_ sweep last frame first, then the backward_ sweep in the reverse of its order.
+    A step's result gradient G is, in this order: the fusion's share, the next step's (cond_n1 warp scatter + first half
+    of its DCN dx), the step after's (cond_n2 warp scatter + second half of that DCN dx) and, for backward_ results, the
+    forward_ backbone's read.  Per step: backbone conv 2 (its residual passes G to the aligned features), LeakyReLU(0.1)'s
+    derivative and backbone conv 0, the alignment (``_align_backward`` on the step's kept operands) and the prologue's
+    adjoint (``ops.flow_warp_backward``).  Steps whose result needs no gradient are skipped, frozen convs launch no weight
+    gradient, and inputs that need none get no scatter."""
+    nx, nfb, nff = need_in
+    b, t, h, w, c = keep["shape"]
+    bufs, steps = keep["bufs"], keep["steps"]
+    names = mod.DIRECTIONS
+    nflows = {"backward_": nfb, "forward_": nff}
+    pn = {name: need[14 * k: 14 * k + 14] for k, name in enumerate(names)}     # [0:10] alignment, [10:14] backbone
+    al_need = {n_: any(pn[n_][:10]) for n_ in names}
+    bb_need = {n_: any(pn[n_][10:]) for n_ in names}
+    # below[name][i]: the result of step i needs a gradient (something it reaches does)
+    below = {}
+    for name in names:
+        below[name] = []
+        for i in range(t):
+            v = nx or bb_need[name] or (i >= 1 and (al_need[name] or nflows[name] or below[name][i - 1])) or \
+                (i >= 2 and below[name][i - 2])
+            if name == "forward_":
+                v = v or below["backward_"][t - 1 - i]
+            below[name].append(v)
+    any_below = any(any(v) for v in below.values())
+    grads = [None] * 30
+    rows = t * b * h * w
+    go = dcat = None
+    if nx or need[28] or need[29] or any_below:
+        go = grad.permute(1, 0, 3, 4, 2).contiguous().float()            # (t, b, h, w, c): the results' row order
+    if need[28] or need[29]:
+        gsp = ops.SplitMat(*ops.split_bf16(go.view(rows, c)))
+        halves = []
+        for k, name in enumerate(names):
+            _, rhi, rlo = bufs[name]
+            dw_k, db_k = ops.linear_wgrad(gsp, ops.SplitMat(rhi.view(rows, c), rlo.view(rows, c)),
+                                          with_bias=need[29] and k == 0)
+            halves.append(dw_k)
+            if k == 0:
+                grads[29] = db_k
+            if not need[28]:
+                break
+        if need[28]:
+            grads[28] = torch.cat(halves, 1).view(c, 2 * c, 1, 1)
+    if any_below:
+        dcat = ops.linear(go, mod.fusion.weight, transpose=True)           # (t, b, h, w, 2c)
+    # the fusion's "+ x" passes the gradient on; a copy, since go may be the incoming gradient itself (b == 1), which
+    # autograd may also hand to other branches
+    dxs = go.clone() if nx else None
+    dflows = {n_: torch.zeros((b, t - 1, 2, h, w), dtype=torch.float32, device=grad.device) if nflows[n_] else None
+              for n_ in names}
+    pend = {n_: [{} for _ in range(t)] for n_ in names}
+    for k, name in reversed(list(enumerate(names))):
+        off = 14 * k
+        r32 = bufs[name][0]
+        flows = keep["flows"][name]
+        nf = nflows[name]
+        align, bb = mod.deform_align[name], mod.backbone[name]
+        pb = pn[name][10:]
+        for i in range(t - 1, -1, -1):
+            if not below[name][i]:
+                continue
+            st = steps[name][i]
+            idx = st["idx"]
+            g = dcat[idx, ..., k * c:(k + 1) * c].contiguous()
+            for key in ("n1", "n2", "bb"):
+                if key in pend[name][i]:
+                    g.add_(pend[name][i].pop(key))
+            if pb[2] or pb[3]:
+                dw2, db2 = ops.conv3x3_wgrad(g, [st["y"]], with_bias=pb[3])
+                _accumulate(grads, off + 12, [dw2 if pb[2] else None, db2])
+            parts = st["parts"]
+            need_rb = name == "forward_" and below["backward_"][t - 1 - idx]
+            need_prop = i >= 1 and (al_need[name] or nf or nx or below[name][i - 1] or (i >= 2 and below[name][i - 2]))
+            if not (pb[0] or pb[1] or nx or need_rb or need_prop):
+                continue
+            d = ops.conv_dgrad(ops.SplitNHWC(*ops.split_bf16(g), (b, c, h, w)), bb[2].weight)
+            g0, g0_sp = ops.leaky_relu_backward(d, st["y32"].permute(0, 2, 3, 1), 0.1, out="both")
+            if pb[0] or pb[1]:
+                srcs = [_dense([s]) for s in parts] if len(parts) == 2 else [_dense(parts)]
+                dw0, db0 = ops.conv3x3_wgrad(g0, srcs, with_bias=pb[1])
+                _accumulate(grads, off + 10, [dw0 if pb[0] else None, db0])
+            chans = [c] * len(parts)
+            if nx:
+                dxs[idx].add_(ops.conv_dgrad(g0_sp, bb[0].weight, src_channels=chans, source=0))
+            if need_rb:
+                pend["backward_"][t - 1 - idx]["bb"] = ops.conv_dgrad(g0_sp, bb[0].weight, src_channels=chans, source=1)
+            if not need_prop:
+                continue
+            da = ops.conv_dgrad(g0_sp, bb[0].weight, src_channels=chans, source=len(parts) - 1, residual=g)
+            # the alignment, on a keep dict of the step's operands
+            need_r1, need_r2 = below[name][i - 1], i >= 2 and below[name][i - 2]
+            n_dx = need_r1 or need_r2
+            n_extra = n_dx or nx or nf
+            cond_n1, cond_n2 = st["conds"]
+            akeep = dict(x=st["xg"].permute(0, 2, 3, 1, 4).reshape(b, h, w, 2 * c).permute(0, 3, 1, 2),
+                         head=st["head"], flow_1=st["flow_n1"], flow_2=st["flow_n2"],
+                         srcs=[[_dense([cond_n1, parts[0], cond_n2]), st["flows_op"]]] + st["head_srcs"], acts=st["acts"])
+            ddx, dextra, dfl1, dfl2, *ag = _align_backward(align, akeep, da.permute(0, 3, 1, 2),
+                                                           (n_dx, n_extra, nf, nf and i >= 2), pn[name][:10])
+            _accumulate(grads, off, ag)
+            if nx:
+                dxs[idx].add_(dextra[:, c:2 * c].permute(0, 2, 3, 1))
+            # the prologue's adjoint
+            f1n, f2n = st["flow_n1"].permute(0, 2, 3, 1), st["flow_n2"].permute(0, 2, 3, 1)
+            dflow_n2 = None
+            if i >= 2 and (need_r2 or nf):
+                r2 = r32[steps[name][i - 2]["idx"]].permute(0, 3, 1, 2)
+                c2, dflow_n2 = ops.flow_warp_backward(
+                    r2, f2n, dextra[:, 2 * c:], need_x=need_r2, need_flow=nf,
+                    residual=ddx[:, c:] if need_r2 else None, flow_residual=dfl2.permute(0, 2, 3, 1) if nf else None)
+                if need_r2:
+                    pend[name][i - 2]["n2"] = c2.permute(0, 2, 3, 1)
+            dflow_n1 = None
+            if need_r1 or nf:
+                r1 = r32[steps[name][i - 1]["idx"]].permute(0, 3, 1, 2)
+                fres = None
+                if nf:
+                    fres = dfl1.permute(0, 2, 3, 1)
+                    if dflow_n2 is not None:
+                        fres = fres + dflow_n2
+                c1, dflow_n1 = ops.flow_warp_backward(r1, f1n, dextra[:, :c], need_x=need_r1, need_flow=nf,
+                                                      residual=ddx[:, :c] if need_r1 else None, flow_residual=fres)
+                if need_r1:
+                    pend[name][i - 1]["n1"] = c1.permute(0, 2, 3, 1)
+            if nf:
+                if dflow_n2 is not None:
+                    dprev, dflow_n1 = ops.flow_warp_backward(flows[:, i - 2], f1n, dflow_n2.permute(0, 3, 1, 2),
+                                                             flow_residual=dflow_n1)
+                    dflows[name][:, i - 2].add_(dprev)
+                dflows[name][:, i - 1].add_(dflow_n1.permute(0, 3, 1, 2))
+    dx = None if dxs is None else dxs.permute(1, 0, 4, 2, 3)
+    return (dx, dflows["backward_"], dflows["forward_"], *grads)

@@ -99,6 +99,70 @@ def flow_warp(x, flow, interpolation="bilinear", padding_mode="zeros", align_cor
     return out if out.dtype == x.dtype else out.to(x.dtype)
 
 
+def flow_warp_backward_work_elems(n, h, w):
+    """32-bit words of the dx scatter workspace of ``flow_warp_backward`` (``e2f_flow_warp_backward_work_elems``)."""
+    elems = int(_lib.load().e2f_flow_warp_backward_work_elems(n, h, w))
+    if elems < 0:
+        _lib.check(elems, "e2f_flow_warp_backward_work_elems")
+    return elems
+
+
+def flow_warp_backward(x, flow, dout, need_x=True, need_flow=True, residual=None, flow_residual=None):
+    """Gradients of ``flow_warp(x, flow)`` (zeros padding, fp32) from dout = d loss / d out, the same bits on every run:
+
+    * dx (n, c, h, w) fp32 = ``residual`` + the scatter of the bilinear weights x dout to each sample's corners
+      (sorted by destination, added in source order);
+    * d flow (n, h, w, 2) fp32 = ``flow_residual`` + sum over c of dout x the floor-based bilinear slopes.
+
+    x, flow: the forward's tensors.  An NHWC x (channels_last or a permuted NHWC view, C % 4 == 0) runs
+    ``e2f_flow_warp_backward_nhwc`` and dx comes back NHWC; otherwise ``e2f_flow_warp_backward_nchw`` reads x's
+    planes in place when they are dense (a slice ``flows[:, i]`` of a (b, t-1, 2, h, w) tensor) and dx comes back NCHW.
+    dout / residual: (n, c, h, w), any layout; flow_residual (n, h, w, 2).  Returns (dx, d flow), None where not asked
+    for."""
+    if not (need_x or need_flow):
+        raise ValueError("flow_warp_backward: nothing to compute")
+    _need_cuda(x, flow, dout, residual, flow_residual)
+    n, c, h, w = x.shape
+    if tuple(flow.shape) != (n, h, w, 2):
+        raise ValueError(f"flow_warp_backward: flow {tuple(flow.shape)} != {(n, h, w, 2)} of x {tuple(x.shape)}")
+    for what, t in (("dout", dout), ("residual", residual)):
+        if t is not None and tuple(t.shape) != (n, c, h, w):
+            raise ValueError(f"flow_warp_backward: {what} {tuple(t.shape)} != x {tuple(x.shape)}")
+    if flow_residual is not None and tuple(flow_residual.shape) != (n, h, w, 2):
+        raise ValueError(f"flow_warp_backward: flow_residual {tuple(flow_residual.shape)} != {(n, h, w, 2)}")
+    lib = _lib.load()
+    dev = flow.device
+    flow = flow.contiguous().float()
+    fres = None if flow_residual is None else flow_residual.contiguous().float()
+    dflow = torch.empty((n, h, w, 2), dtype=torch.float32, device=dev) if need_flow else None
+    work = torch.empty(flow_warp_backward_work_elems(n, h, w), dtype=torch.int32, device=dev) if need_x else None
+    nhwc = x.dtype == torch.float32 and _is_cl(x) and c % 4 == 0
+
+    def ptr(t):
+        return None if t is None else t.data_ptr()
+
+    if nhwc:
+        xs = x.permute(0, 2, 3, 1)
+        d = dout.permute(0, 2, 3, 1).contiguous().float()
+        res = None if residual is None else residual.permute(0, 2, 3, 1).contiguous().float()
+        dx = torch.empty((n, h, w, c), dtype=torch.float32, device=dev) if need_x else None
+        with _timed("flow_warp_backward", float(n * h * w * c * 4 * (need_flow * 5 + need_x * 3))):
+            st = lib.e2f_flow_warp_backward_nhwc(xs.data_ptr(), flow.data_ptr(), d.data_ptr(), ptr(fres), ptr(dflow),
+                                                 ptr(res), ptr(dx), ptr(work), n, h, w, c, _stream())
+        _lib.check(st, "e2f_flow_warp_backward_nhwc")
+        return (None if dx is None else dx.permute(0, 3, 1, 2)), dflow
+    if x.dtype != torch.float32 or x.stride()[1:] != (h * w, w, 1):
+        x = x.contiguous().float()
+    d = dout.contiguous().float()
+    res = None if residual is None else residual.contiguous().float()
+    dx = torch.empty((n, c, h, w), dtype=torch.float32, device=dev) if need_x else None
+    with _timed("flow_warp_backward", float(n * h * w * c * 4 * (need_flow * 5 + need_x * 3))):
+        st = lib.e2f_flow_warp_backward_nchw(x.data_ptr(), x.stride(0), flow.data_ptr(), d.data_ptr(), ptr(fres),
+                                             ptr(dflow), ptr(res), ptr(dx), ptr(work), n, c, h, w, _stream())
+    _lib.check(st, "e2f_flow_warp_backward_nchw")
+    return dx, dflow
+
+
 def pack_dcn_weight(weight, deform_groups):
     """fp32 [Cout,Cin,3,3] -> fp16 [Cout, 9*Cin] GEMM operand in sampler K-order (k = (g*9+tap)*cpg + c).
 

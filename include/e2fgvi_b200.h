@@ -60,6 +60,27 @@ int e2f_flow_warp(const void* x, const float* flow, void* out, int n, int h, int
 int e2f_flow_warp_nchw(const float* x, const float* flow, float* out, int n, int c, int h, int w, int pad_mode,
                        void* stream);
 
+/* Backward of e2f_flow_warp (zeros padding) and e2f_flow_warp_nchw (zeros padding), fp32.  Given dout (the gradient of
+ * out), each written when its pointer is not NULL:
+ *   dflow [N][H][W][2] = dflow_residual (or 0) + sum_c dout[c] . d out[c] / d (u, v): the floor-based slopes of the
+ *                        bilinear form (a corner outside the image has neither value nor slope), the channels summed in
+ *                        a fixed order (needs x)
+ *   dx                 = dx_residual (or 0) + the scatter of the bilinear weights x dout to each sample's 4 corners,
+ *                        added per destination in source order after a stable radix sort (needs work)
+ * Both are the same bits on every run: no float atomics.
+ * e2f_flow_warp_backward_nhwc: x, dout, dx, dx_residual [N][H][W][C] with C % 4 == 0.
+ * e2f_flow_warp_backward_nchw: x planes [N][C][H][W] with a batch stride of x_bstride elements (a slice flows[:, i] of
+ *   a (b, t-1, 2, h, w) tensor), dout, dx, dx_residual dense [N][C][H][W].
+ * flow, dflow_residual, dflow [N][H][W][2] (u = x-displacement first).  N*H*W*4 must fit in int.
+ * work: e2f_flow_warp_backward_work_elems 32-bit words, 256-byte aligned (negative = bad arguments). */
+int64_t e2f_flow_warp_backward_work_elems(int n, int h, int w);
+int e2f_flow_warp_backward_nhwc(const float* x, const float* flow, const float* dout, const float* dflow_residual,
+                                float* dflow, const float* dx_residual, float* dx, void* work, int n, int h, int w,
+                                int c, void* stream);
+int e2f_flow_warp_backward_nchw(const float* x, int64_t x_bstride, const float* flow, const float* dout,
+                                const float* dflow_residual, float* dflow, const float* dx_residual, float* dx,
+                                void* work, int n, int c, int h, int w, void* stream);
+
 /* Pack a DCN weight [Cout][Cin][3][3] fp32 (mmcv / torch layout, feat_prop.py:13 via ModulatedDeformConv2d)
  * into the fp16 GEMM operand [Cout][K], K = 9*Cin, k = (g*9 + tap)*cpg + c_in_group with cpg = Cin/deform_groups.
  * This K order makes one 64-wide K block = 64/cpg consecutive sample points of the sampler. */
